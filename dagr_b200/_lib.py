@@ -20,6 +20,7 @@ _lib = None
 ELL = 16
 KU = 15
 TABW = 16
+L1_TC_WFRAG_FLOATS = 8192               # DAGR_L1_TC_WFRAG_FLOATS
 
 p = C.c_void_p
 i32 = C.c_int32
@@ -92,6 +93,9 @@ _SIGS = {
     "dagr_l1_conv_a": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, C.POINTER(L1AParams), p, p]),
     "dagr_l1_conv_b_pool": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1BParams), p, p, p]),
     "dagr_l1_conv_b_pool_voxel": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, p, C.POINTER(L1BParams), p, C.c_int, p, p, p, p, p, p, p, C.c_int, p, p, C.c_int, p]),
+    "dagr_l1_tc_weights": (C.c_int, [p, p, C.c_int, p]),
+    "dagr_l1_conv_b_pool_voxel_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, C.POINTER(L1BParams), p, p, C.c_int, p, p, p, p, p, p, p, C.c_int, p, p, C.c_int, p]),
+    "dagr_l1_conv_a_image_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1ImgParams), p, p, p, p, p, C.c_int, p]),
     "dagr_pool1_finalize": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, p, p, p, p, p, p]),
     "dagr_grid_cat_pos": (C.c_int, [C.POINTER(Grid), p, p, p, C.c_int, p, p]),
     "dagr_grid_conv": (C.c_int, [C.POINTER(Grid), p, p, p, p, C.c_int, C.c_int, C.c_int, p, p, p, p, p, p, C.c_int, f32, f32, p, p]),

@@ -14,6 +14,7 @@
 // parameter, so every FFMA takes its weight straight from the constant bank (no load instructions).
 // One thread per destination node; nodes are in cell-major sorted order, so own rows, ELL columns
 // and outputs are fully coalesced and the pool1 max is a warp-segmented reduction.
+#include <string.h>
 #include "common.cuh"
 
 #define L1_THREADS 128
@@ -353,6 +354,94 @@ struct CB2Tile {
     int run_start[3], run_len[3], run_off[3];
 };
 
+// ---- phase 2 on tensor cores (CB2_TC = 1) ------------------------------------------------------------------------------
+// Phase 2 of a pass is a dense product with node-independent weights, [32 nodes of a warp x 40] x [40 x 16]: on CUDA cores it
+// costs as many issue slots as the edge loop (every FFMA needs its weight through a uniform constant load on sm_90).  With
+// CB2_TC it runs as mma.sync.m16n8k8 TF32 in 3xTF32 form (a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, hi = cvt.rna.tf32(x),
+// lo = x - hi; relative error ~1e-6): the warp's 32 nodes are two m16 tiles, the 16 outputs two n8 tiles, one k8 step per
+// spline slot (8 channels of the current half) plus one per half for the root weight.  o2[8] then holds the FP32 C fragments
+// across all passes: o2[4 mt + 2 nt] = (c0, c1), o2[4 mt + 2 nt + 1] = (c2, c3) of m-tile mt, n-tile nt.  An output element
+// depends only on its own node's row and the fixed k order, so a node gets the same bits in every instance and CTA shape.
+// The weight fragments (per lane, already split into hi / lo) come from global memory in the order of dagr_l1_tc_weights:
+// float4 [half][k-step: slot 0..14, root = 15][lane][n-tile] = (hi k=t, hi k=t+4, lo k=t, lo k=t+4), t = lane & 3.
+// Phase 1 leaves one node per lane; the A fragment needs other lanes' values, which go through a 256-byte per-warp tile
+// (16 rows x 4 floats: one m-tile and half a k-step at a time, so that four CTAs still fit an SM).
+#ifndef CB2_TC
+#define CB2_TC 1
+#endif
+#define CB2_TC_KSTEPS 16                   // per channel half: 15 spline slots + root
+
+__device__ __forceinline__ uint32_t tf32_rna(float x)
+{
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+__device__ __forceinline__ void mma_tf32(float2 &c01, float2 &c23, const uint32_t a[4], uint32_t b0, uint32_t b1)
+{
+    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(c01.x), "+f"(c01.y), "+f"(c23.x), "+f"(c23.y)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// o2 (C fragments) += [this warp's nodes x 8] x [8 x 16]; this lane's node contributes a[0..7], wf = this k-step's fragments
+// of this lane.  Warp-uniform call; lanes without a node pass zeros.
+__device__ __forceinline__ void cb2_tc_kstep(float *xt, const float a[8], const float4 *__restrict__ wf, float2 o2[8])
+{
+    const int lane = threadIdx.x & 31;
+    const float4 w0 = __ldg(wf), w1 = __ldg(wf + 1);
+    const uint32_t bh[2][2] = {{__float_as_uint(w0.x), __float_as_uint(w0.y)}, {__float_as_uint(w1.x), __float_as_uint(w1.y)}};
+    const uint32_t bl[2][2] = {{__float_as_uint(w0.z), __float_as_uint(w0.w)}, {__float_as_uint(w1.z), __float_as_uint(w1.w)}};
+    float *row = xt + 4 * (lane & 15);
+    const uint32_t ra = smem_u32(row);
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++) {
+        uint32_t ah[4], al[4];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {                              // k = 4h .. 4h+3 of rows 16mt .. 16mt+15
+            __syncwarp();
+            if ((lane >> 4) == mt) *reinterpret_cast<float4 *>(row) = make_float4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
+            __syncwarp();
+            uint32_t r0, r1;                                       // r0 = A[g][4h + t], r1 = A[g + 8][4h + t]
+            asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(ra) : "memory");
+            ah[2 * h] = tf32_rna(__uint_as_float(r0));
+            ah[2 * h + 1] = tf32_rna(__uint_as_float(r1));
+            al[2 * h] = __float_as_uint(__uint_as_float(r0) - __uint_as_float(ah[2 * h]));
+            al[2 * h + 1] = __float_as_uint(__uint_as_float(r1) - __uint_as_float(ah[2 * h + 1]));
+        }
+        // (a0, a1, a2, a3) = (A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]): the order of ah / al above
+        const uint32_t fa[4] = {ah[0], ah[1], ah[2], ah[3]}, fl[4] = {al[0], al[1], al[2], al[3]};
+#pragma unroll
+        for (int nt = 0; nt < 2; nt++) {
+            mma_tf32(o2[4 * mt + 2 * nt], o2[4 * mt + 2 * nt + 1], fl, bh[nt][0], bh[nt][1]);
+            mma_tf32(o2[4 * mt + 2 * nt], o2[4 * mt + 2 * nt + 1], fa, bl[nt][0], bl[nt][1]);
+            mma_tf32(o2[4 * mt + 2 * nt], o2[4 * mt + 2 * nt + 1], fa, bh[nt][0], bh[nt][1]);
+        }
+    }
+}
+
+// C fragments -> thread-per-node layout (o2[c] = channels 2c, 2c+1 of this lane's node), through the same tile.  Warp-uniform.
+__device__ __forceinline__ void cb2_tc_unfrag(float *xt, float2 o2[8])
+{
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    float2 r[8];
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+        for (int q = 0; q < 4; q++) {                              // channels 4q .. 4q+3 = n-tile q/2, lanes with t/2 == q%2
+            __syncwarp();
+            if ((t >> 1) == (q & 1)) {
+                *reinterpret_cast<float2 *>(xt + 4 * g + 2 * (t & 1)) = o2[4 * mt + 2 * (q >> 1)];
+                *reinterpret_cast<float2 *>(xt + 4 * (g + 8) + 2 * (t & 1)) = o2[4 * mt + 2 * (q >> 1) + 1];
+            }
+            __syncwarp();
+            const float4 v = *reinterpret_cast<const float4 *>(xt + 4 * (lane & 15));
+            if ((lane >> 4) == mt) { r[2 * q] = make_float2(v.x, v.y); r[2 * q + 1] = make_float2(v.z, v.w); }
+        }
+#pragma unroll
+    for (int c = 0; c < 8; c++) o2[c] = r[c];
+}
+
 // One pass = one input-channel half (8 channels) x one x-slot k (the 5 spline slots u = k + 3 j, j = 0..4) of one node:
 //     A_j = sum_{e in N(i) + self} tabx[dx_e][k] * taby[dy_e][j] * x_e[half]      (5 x 8 accumulators)
 //     o  += sum_j W_{k+3j}[half]^T A_j
@@ -364,11 +453,13 @@ struct CB2Tile {
 // Variants measured and rejected (ELL entries ordered by the x-slots they feed so that the outer x-slot passes skip their
 // exact-zero edges: slower, the per-lane loop bounds cost more than the skipped iterations save): 15 slots x 8 channels per pass (120
 // accumulators, 2 CTAs/SM), 15 slots x 4 channels, phase-2 weights from shared memory or half/half.
-template <bool STAGED, int half, int grp, int THREADS, class PT>
+// With TC, phase 2 runs on tensor cores (see cb2_tc_kstep) and o2 holds C fragments; the call is then warp-uniform and a lane
+// without a node passes n = -1 (no edge, A = 0).
+template <bool STAGED, int half, int grp, int THREADS, bool TC, class PT>
 __device__ __forceinline__ void cb2_pass(int64_t N, int p, int n, const float *__restrict__ xa, const float *s_rows,
                                          const float *s_wx, const float4 *s_wy, const float *s_wy4, const uint32_t *s_ell, const uint16_t *s_sp,
                                          const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
-                                         const PT &P, int own_row, int r, int tix, float2 o2[8])
+                                         const PT &P, const float4 *__restrict__ wfrag, float *xt, int own_row, int r, int tix, float2 o2[8])
 {
     float2 A[CB2_G][4];
 #pragma unroll
@@ -432,6 +523,23 @@ __device__ __forceinline__ void cb2_pass(int64_t N, int p, int n, const float *_
         }
     }
 #undef CB2_EDGE_FMA
+    if constexpr (TC) {
+        // phase 2 on tensor cores: k-step j = spline slot grp + 3 j, k = channel of this half
+        // The pass sums into fresh fragments which are then added to o2 with IEEE fp32 adds: the tensor cores' fp32
+        // accumulation truncates, and chaining all 6 passes x 15 mma through it doubled the largest errors against the oracle.
+        const float4 *wf = wfrag + ((size_t)half * CB2_TC_KSTEPS * 32 + (threadIdx.x & 31)) * 2;
+        float2 c2[8];
+#pragma unroll
+        for (int i = 0; i < 8; i++) c2[i] = make_float2(0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < CB2_G; j++) {
+            const float a[8] = {A[j][0].x, A[j][0].y, A[j][1].x, A[j][1].y, A[j][2].x, A[j][2].y, A[j][3].x, A[j][3].y};
+            cb2_tc_kstep(xt, a, wf + (grp + 3 * j) * 64, c2);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; i++) o2[i] = make_float2(__fadd_rn(o2[i].x, c2[i].x), __fadd_rn(o2[i].y, c2[i].y));
+        return;
+    }
     // phase 2: weights from the constant bank through uniform 128-bit loads, two FFMA2 per load
 #pragma unroll
     for (int j = 0; j < CB2_G; j++)
@@ -477,6 +585,7 @@ struct CB2Shared {
     float red[THREADS / 32][16];
     long long sum[THREADS / 32][3];
     int tm[THREADS / 32];
+    __align__(16) float xt[THREADS / 32][64];   // per-warp exchange tile of the tensor-core phase 2
 };
 
 // The per-voxel routine is a template over the input rows: <dagr_l1b_params_t, 2, false> is conv_block2 (16 channels = 2
@@ -486,11 +595,11 @@ struct CB2Shared {
 // chunk-major for conv_block2, plus the layer's skip branch BN(Linear(x0)) -> skip_out; no pooling).
 // work list: wl_hdr[0] = number of voxels beyond this instance's staging capacity (queued in wl_ids when `defer`, otherwise
 // only counted and gathered from global memory / L2), wl_hdr[1] = pop cursor of the dense kernel
-template <class PT, int NCH, bool MODE_A, int CAP, int THREADS, bool POOL_MEAN, bool PLAIN>
+template <class PT, int NCH, bool MODE_A, int CAP, int THREADS, bool POOL_MEAN, bool PLAIN, bool TC>
 __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
              const int2 *__restrict__ ti, const float *__restrict__ feat_s, const float *__restrict__ xa,
              const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
-             const PT &P, const float *__restrict__ skip_pre_in, const int min_idx_in,
+             const PT &P, const float4 *__restrict__ wfrag, const float *__restrict__ skip_pre_in, const int min_idx_in,
              float *__restrict__ persist_in, float *__restrict__ x1_in, int32_t *__restrict__ cnt, int32_t *__restrict__ pxy,
              float *__restrict__ tmean, float *__restrict__ tmax, float *__restrict__ xg, int ldx,
              float *__restrict__ xa_out, float *__restrict__ skip_out,
@@ -509,7 +618,8 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
     auto &s_red = S.red;
     auto &s_sum = S.sum;
     auto &s_tm = S.tm;
-    float *s_rows = (float *)smem_raw;                                   // [CAP][8]   one channel half of the 3 runs
+    float *const xt = S.xt[threadIdx.x >> 5];
+    float *s_rows = (float *)smem_raw;                                  // [CAP][8]   one channel half of the 3 runs
     float *s_wx = s_rows + (size_t)CAP * 8;                              // [3][32]   x factor of the slot weights, per x-slot
     float4 *s_wy = (float4 *)(s_wx + 128);                               // [32]      y factors 0..3
     float *s_wy4 = (float *)(s_wy + 32);                                 // [32]      y factor 4
@@ -628,21 +738,33 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
                 mbar_wait(&s_bar, parity);                              // (one waiting thread + a CTA barrier instead: slower)
                 parity ^= 1;
             }
-            if (active) {
+            // with TC the warp's lanes run the passes together (mma.sync): a lane without a node joins with no edges
+            if (TC ? __any_sync(0xffffffffu, active) : active) {
+                const int nn = active ? n : -1;
                 // root weight on this half of x_i.  `half` must be a compile-time constant here as well: with a run-time index
                 // the 64 weight fetches per half become register-indexed LDC through the address-divergence unit
 #define CB2_ROOT(H)                                                                                                  \
     do {                                                                                                            \
         const float4 *src = staged ? reinterpret_cast<const float4 *>(s_rows + (int64_t)(p + d1) * 8)               \
                                    : reinterpret_cast<const float4 *>(xa + ((int64_t)(H) * N + p) * 8);             \
-        const float4 t0 = src[XA_SWZ(p)], t1 = src[XA_SWZ(p) ^ 1];                                                  \
+        const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);                                                         \
+        const float4 t0 = active ? src[XA_SWZ(p)] : z4, t1 = active ? src[XA_SWZ(p) ^ 1] : z4;                      \
         const float v[8] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w};                                        \
+        if constexpr (TC) {                                                                                         \
+            float2 c2[8];                                                                                           \
+            _Pragma("unroll") for (int i = 0; i < 8; i++) c2[i] = make_float2(0.f, 0.f);                            \
+            cb2_tc_kstep(xt, v, wfrag + (((H) * CB2_TC_KSTEPS + 15) * 32 + lane_) * 2, c2);                         \
+            _Pragma("unroll") for (int i = 0; i < 8; i++)                                                           \
+                o2[i] = make_float2(__fadd_rn(o2[i].x, c2[i].x), __fadd_rn(o2[i].y, c2[i].y));                      \
+        }                                                                                                           \
         _Pragma("unroll") for (int k = 0; k < 8; k++)                                                               \
             _Pragma("unroll") for (int c4 = 0; c4 < 4; c4++) {                                                      \
-                const float4 w4 = *reinterpret_cast<const float4 *>(&P.root[8 * (H) + k][4 * c4]);                  \
-                o2[2 * c4] = ffma2(make_float2(v[k], v[k]), make_float2(w4.x, w4.y), o2[2 * c4]);                   \
-                o2[2 * c4 + 1] = ffma2(make_float2(v[k], v[k]), make_float2(w4.z, w4.w), o2[2 * c4 + 1]);           \
-                if constexpr (MODE_A) {                  /* the layer's skip branch Linear(x0) (conv.py:41-52) */    \
+                if constexpr (!TC) {                                                                                \
+                    const float4 w4 = *reinterpret_cast<const float4 *>(&P.root[8 * (H) + k][4 * c4]);              \
+                    o2[2 * c4] = ffma2(make_float2(v[k], v[k]), make_float2(w4.x, w4.y), o2[2 * c4]);               \
+                    o2[2 * c4 + 1] = ffma2(make_float2(v[k], v[k]), make_float2(w4.z, w4.w), o2[2 * c4 + 1]);       \
+                }                                                                                                   \
+                if constexpr (MODE_A) {                 /* the layer's skip branch Linear(x0) (conv.py:41-52) */    \
                     const float4 k4 = *reinterpret_cast<const float4 *>(&P.skip[8 * (H) + k][4 * c4]);              \
                     sk2[2 * c4] = ffma2(make_float2(v[k], v[k]), make_float2(k4.x, k4.y), sk2[2 * c4]);             \
                     sk2[2 * c4 + 1] = ffma2(make_float2(v[k], v[k]), make_float2(k4.z, k4.w), sk2[2 * c4 + 1]);     \
@@ -657,8 +779,8 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
 #undef CB2_ROOT
 #define CB2_PASS(H, G)                                                                                               \
     do {                                                                                                            \
-        if (staged) cb2_pass<true, H, G, THREADS>(N, p, n, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, P, p + d1, g.r, tix, o2); \
-        else        cb2_pass<false, H, G, THREADS>(N, p, n, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, P, 0, g.r, tix, o2);     \
+        if (staged) cb2_pass<true, H, G, THREADS, TC>(N, p, nn, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, P, wfrag, xt, p + d1, g.r, tix, o2); \
+        else        cb2_pass<false, H, G, THREADS, TC>(N, p, nn, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, P, wfrag, xt, 0, g.r, tix, o2);     \
     } while (0)
 #define CB2_HALF(H)                                                                                                  \
     do {                                                                                                            \
@@ -673,6 +795,9 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
 #undef CB2_HALF
 #undef CB2_PASS
             }
+        }
+        if constexpr (TC) {
+            if (__any_sync(0xffffffffu, active)) cb2_tc_unfrag(xt, o2);
         }
         if (sparse) {
             // add the partial sums of warps 1 and 2 (x-slots 1 and 2) to warp 0's: the staged rows are dead by now
@@ -827,38 +952,39 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
 }
 
 
-template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN>
+template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN, bool TC>
 __global__ void __launch_bounds__(CB2_THREADS, MODE_A ? 3 : 4)       // (3 CTAs / 128 registers, no spills: slower)
 k_l1_conv_b2(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
              const int2 *__restrict__ ti, const float *__restrict__ feat_s, const float *__restrict__ xa,
              const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
-             const __grid_constant__ PT P, const float *__restrict__ skip_pre, const int min_idx,
+             const __grid_constant__ PT P, const float4 *__restrict__ wfrag, const float *__restrict__ skip_pre, const int min_idx,
              float *__restrict__ persist, float *__restrict__ x1, int32_t *__restrict__ cnt, int32_t *__restrict__ pxy,
              float *__restrict__ tmean, float *__restrict__ tmax, float *__restrict__ xg, int ldx,
              float *__restrict__ xa_out, float *__restrict__ skip_out, int32_t *__restrict__ wl_hdr, int32_t *__restrict__ wl_ids,
              const int defer)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ __align__(8) CB2Shared<CB2_THREADS> S;
+    __shared__ __align__(16) CB2Shared<CB2_THREADS> S;
     if (threadIdx.x == 0) mbar_init(&S.bar, 1);                         // made visible by the routine's first __syncthreads
     uint32_t parity = 0;
-    cb2_voxel<PT, NCH, MODE_A, CB2_CAP, CB2_THREADS, POOL_MEAN, PLAIN>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, skip_pre, min_idx, persist, x1, cnt, pxy,
-                                                      tmean, tmax, xg, ldx, xa_out, skip_out, (int)blockIdx.x, smem_raw, S, parity, wl_hdr, wl_ids, defer);
+    cb2_voxel<PT, NCH, MODE_A, CB2_CAP, CB2_THREADS, POOL_MEAN, PLAIN, TC>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, wfrag, skip_pre, min_idx,
+                                                      persist, x1, cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out, (int)blockIdx.x,
+                                                      smem_raw, S, parity, wl_hdr, wl_ids, defer);
 }
 
 // dense voxels: persistent CTAs (one per SM) pop voxel ids from the work list the regular kernel filled
-template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN>
+template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN, bool TC>
 __global__ void __launch_bounds__(CB2_THREADS_BIG, 1)
 k_l1_conv_b2_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
                    const int2 *__restrict__ ti, const float *__restrict__ feat_s, const float *__restrict__ xa,
                    const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
-                   const __grid_constant__ PT P, const float *__restrict__ skip_pre, const int min_idx,
+                   const __grid_constant__ PT P, const float4 *__restrict__ wfrag, const float *__restrict__ skip_pre, const int min_idx,
                    float *__restrict__ persist, float *__restrict__ x1, int32_t *__restrict__ cnt, int32_t *__restrict__ pxy,
                    float *__restrict__ tmean, float *__restrict__ tmax, float *__restrict__ xg, int ldx,
                    float *__restrict__ xa_out, float *__restrict__ skip_out, int32_t *__restrict__ wl_hdr, const int32_t *__restrict__ wl_ids)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ __align__(8) CB2Shared<CB2_THREADS_BIG> S;
+    __shared__ __align__(16) CB2Shared<CB2_THREADS_BIG> S;
     __shared__ int s_next;
     if (threadIdx.x == 0) mbar_init(&S.bar, 1);
     uint32_t parity = 0;                                                // the barrier's phase carries over from voxel to voxel
@@ -869,9 +995,9 @@ k_l1_conv_b2_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ s
         __syncthreads();
         const int i = s_next;
         if (i >= count) break;
-        cb2_voxel<PT, NCH, MODE_A, CB2_CAP_BIG, CB2_THREADS_BIG, POOL_MEAN, PLAIN>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, skip_pre, min_idx, persist, x1,
-                                                                  cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out, wl_ids[i],
-                                                                  smem_raw, S, parity, nullptr, nullptr, 0);
+        cb2_voxel<PT, NCH, MODE_A, CB2_CAP_BIG, CB2_THREADS_BIG, POOL_MEAN, PLAIN, TC>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, wfrag, skip_pre,
+                                                                  min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out,
+                                                                  wl_ids[i], smem_raw, S, parity, nullptr, nullptr, 0);
     }
 }
 
@@ -880,18 +1006,18 @@ static size_t cb2_smem_bytes(const dagr_geom_t *g, int cap, int threads)
     return (size_t)cap * 32 + 96 * 16 + (size_t)DAGR_ELL * threads * 4 + (size_t)g->ncell * 2 + 32;
 }
 
-template <class PT, int NCH, bool MODE_A, bool POOL_MEAN = false, bool PLAIN = false>
+template <class PT, int NCH, bool MODE_A, bool TC, bool POOL_MEAN = false, bool PLAIN = false>
 static int cb2_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int2 *ti, const float *feat_s,
-                      const float *xa, const int32_t *nbr, const uint16_t *off, const PT *p_host, const float *skip_pre, int min_idx,
-                      float *persist, float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx,
+                      const float *xa, const int32_t *nbr, const uint16_t *off, const PT *p_host, const float4 *wfrag, const float *skip_pre,
+                      int min_idx, float *persist, float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx,
                       float *xa_out, float *skip_out, int32_t *wl_hdr, int32_t *wl_ids, int defer, cudaStream_t st)
 {
     const int cells = g->B * g->ny1 * g->nx1;
     const size_t smem = cb2_smem_bytes(g, CB2_CAP, CB2_THREADS);
-    auto kern = k_l1_conv_b2<PT, NCH, MODE_A, POOL_MEAN, PLAIN>;
+    auto kern = k_l1_conv_b2<PT, NCH, MODE_A, POOL_MEAN, PLAIN, TC>;
     DAGR_CUDA(dagr_allow_smem(kern, smem, true));
-    kern<<<cells, CB2_THREADS, smem, st>>>(*g, N, start, xyb, ti, feat_s, xa, nbr, off, *p_host, skip_pre, min_idx, persist, x1, cnt, pxy,
-                                           tmean, tmax, xg, ldx, xa_out, skip_out, wl_hdr, wl_ids,
+    kern<<<cells, CB2_THREADS, smem, st>>>(*g, N, start, xyb, ti, feat_s, xa, nbr, off, *p_host, wfrag, skip_pre, min_idx, persist, x1, cnt,
+                                           pxy, tmean, tmax, xg, ldx, xa_out, skip_out, wl_hdr, wl_ids,
                                            (wl_hdr != nullptr && wl_ids != nullptr && defer) ? 1 : 0);
     DAGR_CHECK_LAUNCH();
     if (wl_hdr != nullptr && wl_ids != nullptr && defer) {
@@ -902,13 +1028,36 @@ static int cb2_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, con
             DAGR_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
         }
         const size_t smem_big = cb2_smem_bytes(g, CB2_CAP_BIG, CB2_THREADS_BIG);
-        auto kd = k_l1_conv_b2_dense<PT, NCH, MODE_A, POOL_MEAN, PLAIN>;
+        auto kd = k_l1_conv_b2_dense<PT, NCH, MODE_A, POOL_MEAN, PLAIN, TC>;
         DAGR_CUDA(dagr_allow_smem(kd, smem_big));
-        kd<<<n_sm, CB2_THREADS_BIG, smem_big, st>>>(*g, N, start, xyb, ti, feat_s, xa, nbr, off, *p_host, skip_pre, min_idx, persist, x1,
-                                                    cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out, wl_hdr, wl_ids);
+        kd<<<n_sm, CB2_THREADS_BIG, smem_big, st>>>(*g, N, start, xyb, ti, feat_s, xa, nbr, off, *p_host, wfrag, skip_pre, min_idx, persist,
+                                                    x1, cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out, wl_hdr, wl_ids);
         DAGR_CHECK_LAUNCH();
     }
     return DAGR_OK;
+}
+
+template <bool TC>
+static int conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                             const float *feat_s, const float *xa, const int32_t *nbr, const uint16_t *off, const dagr_l1b_params_t *p_host,
+                             const float4 *wfrag, const float *skip_pre, int min_idx, float *persist, float *x1, int32_t *cnt,
+                             int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx, int32_t *wl_hdr, int32_t *wl_ids, int defer,
+                             cudaStream_t st)
+{
+    DAGR_CHECK_ARG(g && p_host, "null argument");
+    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
+    DAGR_CHECK_ARG(!(p_host->pool_mean && persist), "the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
+    if (p_host->pool_mean)
+        return cb2_launch<dagr_l1b_params_t, 2, false, TC, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag,
+                                                                 skip_pre, min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr,
+                                                                 nullptr, wl_hdr, wl_ids, defer, st);
+    if (min_idx <= 0 && persist == nullptr && x1 == nullptr && skip_pre == nullptr && p_host->relu)
+        return cb2_launch<dagr_l1b_params_t, 2, false, TC, false, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag,
+                                                                        nullptr, 0, nullptr, nullptr, cnt, pxy, tmean, tmax, xg, ldx, nullptr,
+                                                                        nullptr, wl_hdr, wl_ids, defer, st);
+    return cb2_launch<dagr_l1b_params_t, 2, false, TC>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag, skip_pre,
+                                                       min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr, nullptr, wl_hdr, wl_ids,
+                                                       defer, st);
 }
 
 extern "C" int dagr_l1_conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
@@ -919,35 +1068,81 @@ extern "C" int dagr_l1_conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const 
                                          int defer, void *stream)
 {
     (void)tab;
-    DAGR_CHECK_ARG(g && p_host, "null argument");
-    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
-    DAGR_CHECK_ARG(!(p_host->pool_mean && persist), "the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
-    if (p_host->pool_mean)
-        return cb2_launch<dagr_l1b_params_t, 2, false, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, skip_pre, min_idx,
-                                                             persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr, nullptr, wl_hdr, wl_ids,
-                                                             defer, (cudaStream_t)stream);
-    if (min_idx <= 0 && persist == nullptr && x1 == nullptr && skip_pre == nullptr && p_host->relu)
-        return cb2_launch<dagr_l1b_params_t, 2, false, false, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, nullptr, 0,
-                                                                    nullptr, nullptr, cnt, pxy, tmean, tmax, xg, ldx, nullptr, nullptr, wl_hdr,
-                                                                    wl_ids, defer, (cudaStream_t)stream);
-    return cb2_launch<dagr_l1b_params_t, 2, false>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, skip_pre, min_idx,
-                                                   persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr, nullptr, wl_hdr, wl_ids, defer,
-                                                   (cudaStream_t)stream);
+    return conv_b_pool_voxel<false>(g, N, start, xyb, ti, feat_s, xa, nbr, off, p_host, nullptr, skip_pre, min_idx, persist, x1, cnt, pxy,
+                                    tmean, tmax, xg, ldx, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
+}
+
+extern "C" int dagr_l1_conv_b_pool_voxel_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
+                                            const int32_t *ti, const float *feat_s, const float *xa, const int32_t *nbr,
+                                            const uint16_t *off, const dagr_l1b_params_t *p_host, const float *wfrag,
+                                            const float *skip_pre, int min_idx, float *persist, float *x1, int32_t *cnt,
+                                            int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx, int32_t *wl_hdr, int32_t *wl_ids,
+                                            int defer, void *stream)
+{
+    DAGR_CHECK_ARG(wfrag, "null weight fragments (dagr_l1_tc_weights)");
+    return conv_b_pool_voxel<CB2_TC != 0>(g, N, start, xyb, ti, feat_s, xa, nbr, off, p_host, (const float4 *)wfrag, skip_pre, min_idx,
+                                          persist, x1, cnt, pxy, tmean, tmax, xg, ldx, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
 }
 
 // image fusion: the 16 image channels of conv_block1.conv_block1 (x0 chunk-major [2][N][8], chunks swizzled like xa) on top
 // of the event-channel sums the probe kernel left in xa
+template <bool TC>
+static int conv_a_image(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s, const float *x0,
+                        const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host, const float4 *wfrag, float *xa,
+                        float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, cudaStream_t st)
+{
+    DAGR_CHECK_ARG(g && p_host && xyb && feat_s, "null argument");
+    if (N <= 0) return DAGR_OK;
+    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
+    return cb2_launch<dagr_l1img_params_t, 2, true, TC>(g, N, start, xyb, nullptr, feat_s, x0, nbr, off, p_host, wfrag, nullptr, 0, nullptr,
+                                                        nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr, wl_ids,
+                                                        defer, st);
+}
+
 extern "C" int dagr_l1_conv_a_image(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
                                     const float *x0, const int32_t *nbr,
                                     const uint16_t *off, const dagr_l1img_params_t *p_host, float *xa, float *skipv,
                                     int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
 {
-    DAGR_CHECK_ARG(g && p_host && xyb && feat_s, "null argument");
-    if (N <= 0) return DAGR_OK;
-    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
-    return cb2_launch<dagr_l1img_params_t, 2, true>(g, N, start, xyb, nullptr, feat_s, x0, nbr, off, p_host, nullptr, 0, nullptr,
-                                                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr, wl_ids, defer,
-                                                    (cudaStream_t)stream);
+    return conv_a_image<false>(g, N, start, xyb, feat_s, x0, nbr, off, p_host, nullptr, xa, skipv, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
+}
+
+extern "C" int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                                       const float *x0, const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host,
+                                       const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
+{
+    DAGR_CHECK_ARG(wfrag, "null weight fragments (dagr_l1_tc_weights)");
+    return conv_a_image<CB2_TC != 0>(g, N, start, xyb, feat_s, x0, nbr, off, p_host, (const float4 *)wfrag, xa, skipv, wl_hdr, wl_ids, defer,
+                                     (cudaStream_t)stream);
+}
+
+// host-side packing of the weight fragments the tensor-core instances read (layout: see cb2_tc_kstep)
+static float tf32_rna_host(float x)
+{
+    uint32_t u;
+    memcpy(&u, &x, 4);
+    if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & 0xffffe000u;   // cvt.rna.tf32.f32: nearest, ties away from zero
+    float r;
+    memcpy(&r, &u, 4);
+    return r;
+}
+
+extern "C" int dagr_l1_tc_weights(const float *w_host, const float *root_host, int cin, float *wfrag_host)
+{
+    DAGR_CHECK_ARG(w_host && root_host && wfrag_host, "null argument");
+    DAGR_CHECK_ARG(cin >= 16, "the tensor-core instances take input channels 0..15");
+    for (int half = 0; half < 2; half++)
+        for (int s = 0; s < CB2_TC_KSTEPS; s++)
+            for (int lane = 0; lane < 32; lane++)
+                for (int nt = 0; nt < 2; nt++) {
+                    const int g = lane >> 2, t = lane & 3, n = 8 * nt + g;
+                    const float *W = s < DAGR_KU ? w_host + (size_t)s * cin * 16 : root_host;
+                    const float x0 = W[(8 * half + t) * 16 + n], x1 = W[(8 * half + t + 4) * 16 + n];
+                    const float h0 = tf32_rna_host(x0), h1 = tf32_rna_host(x1);
+                    float *o = wfrag_host + ((((size_t)half * CB2_TC_KSTEPS + s) * 32 + lane) * 2 + nt) * 4;
+                    o[0] = h0; o[1] = h1; o[2] = x0 - h0; o[3] = x1 - h1;
+                }
+    return DAGR_OK;
 }
 
 

@@ -24,6 +24,14 @@ def _fold_bn(bn):
     return scale.contiguous(), shift.contiguous()
 
 
+def _tc_weights(lib, params, cin: int, device) -> torch.Tensor:
+    """params.w / params.root (input channels 0..15) in the mma fragment order of the tensor-core conv kernels (dagr_l1_tc_weights)."""
+    out = (C.c_float * _lib.L1_TC_WFRAG_FLOATS)()
+    _lib.check(lib.dagr_l1_tc_weights(C.cast(params.w, C.c_void_p), C.cast(params.root, C.c_void_p), cin, C.cast(out, C.c_void_p)),
+               "dagr_l1_tc_weights")
+    return torch.frombuffer(out, dtype=torch.float32).clone().to(device)
+
+
 def _fill(arr, t: torch.Tensor):
     flat = t.detach().float().cpu().contiguous().view(-1)
     assert flat.numel() == len(arr), (flat.numel(), len(arr))
@@ -137,7 +145,7 @@ class Engine:
         self._out_slot = {}
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
-    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_x0_image=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_voxel_sample_max=1,
+    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
                      dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
                      dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1)
@@ -224,6 +232,7 @@ class Engine:
             pb.ys[j] = geom.slots_y[j]
         pb.den_x, pb.den_y = geom.den1_x, geom.den1_y
         pk = dict(l1b=pb, l1a=None, l1img=None)
+        pk["l1b_wfrag"] = _tc_weights(self.lib, pb, 16, device)
         if cin0 == 3:
             pa = _lib.L1AParams()
             _fill(pa.w, ca.conv.weight.detach().cpu()[slots])                # [15,3,16]
@@ -251,6 +260,7 @@ class Engine:
             s, b = _fold_bn(cb.norm_skip); _fill(pi.sscale, s); _fill(pi.sshift, b)
             pi.relu = 1
             pk["l1img"] = pi
+            pk["l1img_wfrag"] = _tc_weights(self.lib, pi, 24, device)
         pk["layers"] = [_LayerPack(getattr(bb, n), relu, device) for n in ("layer2", "layer3", "layer4", "layer5")]
         heads = []
         for k in range(hd.num_scales):
@@ -566,9 +576,9 @@ class Engine:
             skipv = self._buf(ws, "skipv", (max(N, 1), 16), torch.float32, dev)
             self._run("l1_x0_image", lib.dagr_l1_x0_image, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(f0),
                       int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
-            self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
+            self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
                       _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off),
-                      C.byref(pk["l1img"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
+                      C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
                       _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
         elif self.fused_build or stream_state is not None:
             if min_idx > 0:
@@ -595,9 +605,9 @@ class Engine:
         c1 = 16 + (int(image_feats[1].shape[1]) if use_image else 0)
         g1.x = self._buf(ws, "gx0", (g1.cells, c1), torch.float32, dev)
         if self.voxel_conv_b or use_image or stream_state is not None:
-            self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+            self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
                       _lib.ptr(ws["ti"]), _lib.ptr(ws["feat_s"]), _lib.ptr(ws["xa"]), _lib.ptr(nbr), _lib.ptr(off),
-                      _lib.ptr(geom.d_tab1), C.byref(pk["l1b"]), _lib.ptr(skipv) if use_image else None, min_idx, _lib.ptr(persist),
+                      C.byref(pk["l1b"]), _lib.ptr(pk["l1b_wfrag"]), _lib.ptr(skipv) if use_image else None, min_idx, _lib.ptr(persist),
                       _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy), _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1,
                       _lib.ptr(wl_hdr[4:]), _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
             self._dense_report(ws, wl_hdr)

@@ -266,6 +266,26 @@ int dagr_l1_conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const int32_t *st
                                            6144 rows (196 KB of shared memory per SM); 0: counted only, rows gathered from L2 */,
                               void *stream);
 
+/* Tensor-core forms of the two per-voxel conv calls above (the engine's path).  Same arguments (conv_b drops the unused `tab`)
+ * plus `wfrag` f32[DAGR_L1_TC_WFRAG_FLOATS] on the DEVICE: the weights of input channels 0..15 (w and root) in mma fragment order,
+ * split for 3xTF32, as written by dagr_l1_tc_weights.  The slot-weight products of phase 2 and the root term then run as
+ * mma.sync TF32 (hi*hi + hi*lo + lo*hi, ~1e-6 relative to the fp32 sums) instead of fp32 FMA; every node gets the same bits in
+ * every instance (regular / dense, staged / gathered), as with the plain calls.  Re-run dagr_l1_tc_weights whenever the weights
+ * change. */
+#define DAGR_L1_TC_WFRAG_FLOATS 8192   /* 2 channel halves x 16 k-steps (15 slots + root) x 32 lanes x 2 n-tiles x 4 */
+int dagr_l1_tc_weights(const float *w_host /* [DAGR_KU][cin][16] slot-major, as in the params structs */,
+                       const float *root_host /* [cin][16] */, int cin /* 16 (dagr_l1b_params_t) or 24 (dagr_l1img_params_t) */,
+                       float *wfrag_host /* f32[DAGR_L1_TC_WFRAG_FLOATS] */);
+int dagr_l1_conv_b_pool_voxel_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
+                                 const int32_t *ti, const float *feat_s, const float *xa, const int32_t *nbr,
+                                 const uint16_t *off, const dagr_l1b_params_t *p_host, const float *wfrag,
+                                 const float *skip_pre, int min_idx, float *persist,
+                                 float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx,
+                                 int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
+int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                            const float *x0, const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host,
+                            const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Coarse levels live on dense voxel grids [B, ny, nx]: per cell  valid, pixel position, features,
  * and an 8-neighbour in-edge mask (bit (dcy+1)*3+(dcx+1), src cell = dst cell + (dcx,dcy)).

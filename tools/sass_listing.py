@@ -1,6 +1,7 @@
 """writes profiles/sass_{l1_build,conv_b2}.txt: SASS of the two hot kernels (cuobjdump of the in-tree .so) preceded by an
 instruction histogram (the mnemonics that matter for the design claims: FFMA, uniform constant weight loads, LDS,
-1-D TMA bulk copies UBLKCP + mbarrier SYNCS, no tensor-core HGMMA/HMMA on the graph path)."""
+1-D TMA bulk copies UBLKCP + mbarrier SYNCS, the 3xTF32 HMMA of conv_b2's phase 2).  conv_b2 = the PLAIN tensor-core instance
+the headline runs."""
 import collections
 import re
 import subprocess
@@ -11,7 +12,7 @@ ROOT = Path(__file__).resolve().parents[1]
 so = ROOT / "dagr_b200" / "libdagr_b200.so"
 txt = subprocess.run(["cuobjdump", "-sass", str(so)], capture_output=True, text=True).stdout
 funcs = re.split(r"(?=\t\tFunction : )", txt)
-want = {"l1_build": "_Z10k_l1_buildILi1536ELi5E", "conv_b2": "_Z12k_l1_conv_b2I17dagr_l1b_params_tLi2ELb0E"}
+want = {"l1_build": "_Z10k_l1_buildILi1536ELi5E", "conv_b2": "_Z12k_l1_conv_b2I17dagr_l1b_params_tLi2ELb0ELb0ELb1ELb1E"}
 for tag, prefix in want.items():
     body = next(f for f in funcs if f.lstrip().startswith("Function : " + prefix))
     hist = collections.Counter()
