@@ -9,6 +9,7 @@
 // neighbours are written to the column-major ELL and folded into conv_block1.conv_block1 on the fly
 // (their features are (polarity, x/W, y/H): no gather at all).
 // Voxels whose neighbourhood does not fit the staging buffer fall back to probing global memory.
+#include <type_traits>
 #include "common.cuh"
 
 // Two instances of the per-voxel routine (template parameters CAP = staged neighbourhood records, THREADS = CTA size):
@@ -32,19 +33,23 @@ struct BLTile {
     int run_start[3], run_off[3], run_len[3];
     int smin, smax;              // slice (t / delta_t) range of the voxel's own events
     int unsorted;                // some pixel's records are not time-sorted -> no time bucketing
+    int bucketed;                // the bucket ranges are in use (kept here, not in a register live through the event loop)
     int maxidx;                  // newest arrival index among the events this launch must process (-1: none)
 };
 
-__host__ __device__ __forceinline__ size_t bl_acc_offset(const dagr_geom_t &g, int cap, int threads)
+__host__ __device__ __forceinline__ size_t bl_acc_offset(const dagr_geom_t &g, int cap)
 {
     const size_t TW = g.CW + 2 * g.r, TH = g.CH + 2 * g.r, TP = TW * TH;
-    const size_t o = (size_t)cap * 12 + TP * 4 + (TW + TH) * 4 + TP * BL_NB * 2 + (size_t)g.ncell * 4 + (size_t)threads * 2 + (TW + TH);
+    const size_t o = (size_t)(2 * g.r + 1) * 32 + (size_t)cap * 12 + TP * 4 + (TW + TH) * 4 + TP * BL_NB * 2 + (size_t)g.ncell * 4;
     return (o + 15) / 16 * 16;
 }
+// The occupancy masks are built only for the ring walk and s_order only serves the cell walk, so the two share one region.
+// The cell walk runs when a tile side exceeds 32 px or r > 8; then TWmax + THmax >= 33 and the masks' region is the larger one.
 static size_t bl_smem_bytes(const dagr_geom_t *g, int cap, int threads)
 {
     const size_t TW = g->CW + 2 * g->r, TH = g->CH + 2 * g->r;
-    return bl_acc_offset(*g, cap, threads) + (size_t)(DAGR_ELL - 1) * threads * 4 + (size_t)BL_NB * (TW + TH) * 4 + 16;
+    const size_t occ = (size_t)BL_NB * (TW + TH) * 4, order = (size_t)threads * 2;
+    return bl_acc_offset(*g, cap) + (size_t)(DAGR_ELL - 1) * threads * 4 + (occ > order ? occ : order) + 16;
 }
 
 #define BL_R1 96                 // spiral cells walked one-thread-per-event before unsaturated events are handed
@@ -115,7 +120,7 @@ __device__ __forceinline__ uint32_t bl_lds16(uint32_t a) { uint32_t v; asm volat
 __device__ __forceinline__ int bl_lds16s(uint32_t a) { int v; asm volatile("{ .reg .s16 t; ld.shared.s16 t, [%1]; cvt.s32.s16 %0, t; }" : "=r"(v) : "r"(a) : "memory"); return v; }
 __device__ __forceinline__ int2 bl_lds64(uint32_t a) { int2 v; asm volatile("ld.shared.v2.s32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a) : "memory"); return v; }
 #ifndef BL_FAST_TABLES
-#define BL_FAST_TABLES 1            // exact reciprocal division + 32-bit shared addressing in the occupancy scan (faster in an A/B)
+#define BL_FAST_TABLES 1            // exact reciprocal division for the time buckets (faster in an A/B)
 #endif
 // t / d for 0 <= t < 2^24 through a float reciprocal and one exact fix-up step (the generic 32-bit division is ~20 instructions);
 // anything else takes the plain division, so the result is always the C quotient
@@ -249,7 +254,7 @@ __device__ __forceinline__ int bl_probe_coop(const dagr_geom_t &g, int64_t N, in
 // only counted and probed from global memory), wl_hdr[1] = pop cursor of the dense kernel
 template <int CAP, int THREADS>
 __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const int32_t *__restrict__ start, const int2 *__restrict__ ti,
-                                         const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s, const float *__restrict__ tab,
+                                         const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
                                          const dagr_l1a_params_t &P, const int do_conv, const int min_idx, const int32_t *__restrict__ flags,
                                          int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask,
                                          float *__restrict__ xa, const int cell, unsigned char *smem_raw, BLTile &T, uint32_t &s_mask,
@@ -261,20 +266,23 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
     if (p1 == p0) { if (threadIdx.x == 0 && min_idx <= 0) cellmask[cell] = 0; return; }      // block-uniform
 
     // ---- shared memory carve-up -------------------------------------------------------------------
-    const int TWmax = g.CW + 2 * g.r, THmax = g.CH + 2 * g.r, TPmax = TWmax * THmax;
-    int2 *s_ti = (int2 *)smem_raw;                                      // [CAP]
+    const int TWmax = g.CW + 2 * g.r, THmax = g.CH + 2 * g.r, TPmax = TWmax * THmax, R = 2 * g.r + 1;
+    // factor tables of the slot weights (tab[c][k+3j] == tabx[dx+r][k] * taby[dy+r][j]), laid out so that a warp's lookups
+    // do not collide: wy[0..3] as one float4 per offset, wx as [3 x-slots][R] at a 4-byte stride, wy[4] apart
+    float4 *s_wy = (float4 *)smem_raw;                                  // [R]
+    float *s_wx = (float *)(s_wy + R);                                  // [3][R]
+    float *s_wy4 = s_wx + 3 * R;                                        // [R]
+    int2 *s_ti = (int2 *)(s_wy4 + R);                                   // [CAP]  (16-byte aligned: 32 R bytes of tables)
     float *s_feat = (float *)(s_ti + CAP);                              // [CAP]
     uint16_t *s_rng = (uint16_t *)(s_feat + CAP);                       // [TP][BL_NB]  lo | hi << 8   (16-byte aligned: CAP % 4 == 0)
     uint32_t *s_pbin = (uint32_t *)(s_rng + TPmax * BL_NB);             // [TP]  pos << 8 | visible count
     float *s_posx = (float *)(s_pbin + TPmax);                          // [TWmax]
     float *s_posy = s_posx + TWmax;                                     // [THmax]
-    short *s_sp = (short *)(s_posy + THmax);                     // [ncell]  dx | dy << 8
-    short *s_sp2 = s_sp + g.ncell;                                      // [ncell]  dy*TW + dx
-    uint16_t *s_order = (uint16_t *)(s_sp2 + g.ncell);                  // [THREADS]
-    uint32_t *s_acc = (uint32_t *)(smem_raw + bl_acc_offset(g, CAP, THREADS));   // [K-1][THREADS]  record << 10 | cell
-    uint32_t *s_occ_r = s_acc + (DAGR_ELL - 1) * THREADS;               // [BL_NB][THmax] row occupancy bitmasks
-    unsigned char *s_colv = (unsigned char *)(s_order + THREADS);       // [TWmax]
-    unsigned char *s_rowv = s_colv + TWmax;                             // [THmax]
+    uint16_t *s_sp = (uint16_t *)(s_posy + THmax);                      // [ncell]  (dx + r) | (dy + r) << 5
+    short *s_sp2 = (short *)(s_sp + g.ncell);                           // [ncell]  dy*TW + dx
+    uint32_t *s_acc = (uint32_t *)(smem_raw + bl_acc_offset(g, CAP));   // [K-1][THREADS]  record << 10 | cell
+    uint32_t *s_occ_r = s_acc + (DAGR_ELL - 1) * THREADS;               // [BL_NB][THmax] row occupancy bitmasks (ring walk)
+    uint16_t *s_order = (uint16_t *)s_occ_r;                            // [THREADS]  (cell walk; see bl_smem_bytes)
 
     const int dtw = max(g.dt_us, 1);
     const float dtw_inv = 1.0f / (float)dtw;
@@ -296,6 +304,7 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
     }
     __syncthreads();
     const int TW = T.TW, TH = T.TH, TP = TW * TH;
+    const bool use_rings = TW <= 32 && TH <= 32 && g.r <= 8;            // block-uniform (a ring = 8d <= 64 mask bits)
     uint32_t *s_occ_c = s_occ_r + BL_NB * TH;                           // [BL_NB][TW] column occupancy bitmasks
     const int total = T.run_off[2] + T.run_len[2];
     const bool staged = total <= CAP;                                   // block-uniform
@@ -310,21 +319,23 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
 
     for (int i = threadIdx.x; i < g.ncell; i += blockDim.x) {
         const int dx = g.spiral[2 * i], dy = g.spiral[2 * i + 1];
-        s_sp[i] = (short)((dx & 0xff) | (dy << 8));
+        s_sp[i] = (uint16_t)((dx + g.r) | ((dy + g.r) << 5));
         s_sp2[i] = (short)(dy * TW + dx);
     }
-    // ---- tile tables: per-pixel FIFO bin, normalised positions, voxel direction ---------------------
+    for (int i = threadIdx.x; i < R; i += blockDim.x) {
+        const float4 tx = __ldg(reinterpret_cast<const float4 *>(g.tabx) + i);
+        s_wx[i] = tx.x; s_wx[R + i] = tx.y; s_wx[2 * R + i] = tx.z;
+        s_wy[i] = __ldg(reinterpret_cast<const float4 *>(g.taby) + 2 * i);
+        s_wy4[i] = __ldg(g.taby + 8 * i + 4);
+    }
+    // ---- tile tables: per-pixel FIFO bin, normalised positions ----------------------------------------
     for (int i = threadIdx.x; i < TW; i += blockDim.x) {
         const int gx = T.X0 + i;
-        const bool in = gx >= 0 && gx < g.W;
-        s_posx[i] = in ? g.posx0[gx] : 0.f;
-        s_colv[i] = (unsigned char)(in ? (g.xkey[gx] / g.CP - cx + 1) : 1);
+        s_posx[i] = (gx >= 0 && gx < g.W) ? g.posx0[gx] : 0.f;
     }
     for (int i = threadIdx.x; i < TH; i += blockDim.x) {
         const int gy = T.Y0 + i;
-        const bool in = gy >= 0 && gy < g.H;
-        s_posy[i] = in ? g.posy0[gy] : 0.f;
-        s_rowv[i] = (unsigned char)(in ? (g.ykey[gy] / (g.nx1 * g.CP) - cy + 1) : 1);
+        s_posy[i] = (gy >= 0 && gy < g.H) ? g.posy0[gy] : 0.f;
     }
     for (int i = threadIdx.x; i < TP; i += blockDim.x) {
         const int ty = i / TW, tx = i % TW;
@@ -353,6 +364,8 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
             }
         }
     }
+    if (use_rings)
+        for (int i = threadIdx.x; i < BL_NB * TW; i += blockDim.x) s_occ_c[i] = 0;
     // slice range of the voxel's own events
     {
         int mn = 0x7fffffff, mx = -0x7fffffff, mi = -1;
@@ -370,97 +383,89 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
     // bucket(t) = clamp(t/delta_t - (smin-1), 0, NB-1); an event in bucket e needs records of buckets {e-1, e}.
     const int sbase = T.smin - 1;
     bool bucketed = staged && (T.smax - sbase) < BL_NB && (flags == nullptr || flags[0] == 0);   // block-uniform
-    const bool use_rings = TW <= 32 && TH <= 32 && g.r <= 8;            // block-uniform (a ring = 8d <= 64 mask bits)
-    for (int pass = 0; pass < 2; pass++) {
-        for (int i = threadIdx.x; i < TP; i += blockDim.x) {
-            const uint32_t pb = s_pbin[i];
-            const int vis = pb & 0xff, base = pb >> 8;
-            unsigned char cum[BL_NB + 1];
+    // the ranges of tile pixel i -> s_rng[i]; returns bit e set when bucket e's range is non-empty
+    auto pixel_ranges = [&](int i) -> uint32_t {
+        const uint32_t pb = s_pbin[i];
+        const int vis = pb & 0xff, base = pb >> 8;
+        unsigned char cum[BL_NB + 1];
 #pragma unroll
-            for (int q = 0; q <= BL_NB; q++) cum[q] = 0;
-            if (bucketed) {
-                int prev = 0;
-                for (int k = 0; k < vis; k++) {
-                    int bk = bl_div(s_ti[base + k].x, dtw, dtw_inv) - sbase;
-                    bk = min(max(bk, 0), BL_NB - 1);
-                    if (bk < prev) T.unsorted = 1;                      // benign race: any writer sets 1
-                    prev = bk;
+        for (int q = 0; q <= BL_NB; q++) cum[q] = 0;
+        if (bucketed) {
+            int prev = 0;
+            for (int k = 0; k < vis; k++) {
+                int bk = bl_div(s_ti[base + k].x, dtw, dtw_inv) - sbase;
+                bk = min(max(bk, 0), BL_NB - 1);
+                if (bk < prev) T.unsorted = 1;                          // benign race: any writer sets 1
+                prev = bk;
 #pragma unroll
-                    for (int q = 0; q <= BL_NB; q++) cum[q] += (bk < q) ? 1 : 0;
-                }
-            } else {
-#pragma unroll
-                for (int q = 1; q <= BL_NB; q++) cum[q] = (unsigned char)vis;
+                for (int q = 0; q <= BL_NB; q++) cum[q] += (bk < q) ? 1 : 0;
             }
-            // the eight (lo | hi << 8) ranges of a pixel are one 16-byte store (eight 2-byte stores at a 16-byte lane stride
-            // cost four wavefronts each)
-            static_assert(BL_NB == 8, "one uint4 per pixel");
-            uint32_t w[4];
+        } else {
 #pragma unroll
-            for (int e = 0; e < BL_NB; e += 2) {
-                const uint32_t r0 = (uint32_t)cum[e > 0 ? e - 1 : 0] | ((uint32_t)cum[e + 1] << 8);
-                const uint32_t r1 = (uint32_t)cum[e] | ((uint32_t)cum[e + 2] << 8);
-                w[e >> 1] = r0 | (r1 << 16);
-            }
-            reinterpret_cast<uint4 *>(s_rng)[i] = make_uint4(w[0], w[1], w[2], w[3]);
+            for (int q = 1; q <= BL_NB; q++) cum[q] = (unsigned char)vis;
         }
-        __syncthreads();
+        // the eight (lo | hi << 8) ranges of a pixel are one 16-byte store (eight 2-byte stores at a 16-byte lane stride
+        // cost four wavefronts each)
+        static_assert(BL_NB == 8, "one uint4 per pixel");
+        uint32_t w[4], occ = 0;
+#pragma unroll
+        for (int e = 0; e < BL_NB; e += 2) {
+            const uint32_t r0 = (uint32_t)cum[e > 0 ? e - 1 : 0] | ((uint32_t)cum[e + 1] << 8);
+            const uint32_t r1 = (uint32_t)cum[e] | ((uint32_t)cum[e + 2] << 8);
+            w[e >> 1] = r0 | (r1 << 16);
+            occ |= (cum[e + 1] > cum[e > 0 ? e - 1 : 0] ? 1u : 0u) << e;
+            occ |= (cum[e + 2] > cum[e] ? 1u : 0u) << (e + 1);
+        }
+        reinterpret_cast<uint4 *>(s_rng)[i] = make_uint4(w[0], w[1], w[2], w[3]);
+        return occ;
+    };
+    for (int pass = 0; pass < 2; pass++) {
         if (use_rings) {
-            // occupancy bitmasks for the ring walk: one thread per (bucket, tile row) / (bucket, tile column) word scans its
-            // pixels -- no atomics (one atomicOr per pixel and bucket serialised on the row word: 6x the ideal wavefronts)
-            for (int idx = threadIdx.x; idx < BL_NB * (TH + TW); idx += blockDim.x) {
-                uint32_t m = 0;
-#if BL_FAST_TABLES
-                if (idx < BL_NB * TH) {
-                    const int e = idx / TH, row = idx % TH;
-                    uint32_t a = bl_sa(s_rng) + 2u * (uint32_t)(row * TW * BL_NB + e);
-                    for (int x = 0; x < TW; x++, a += 2u * BL_NB) {
-                        const uint32_t rg = bl_lds16(a);
-                        m |= ((rg >> 8) > (rg & 0xff)) ? (1u << x) : 0u;
-                    }
-                } else {
-                    const int i2 = idx - BL_NB * TH, e = i2 / TW, col = i2 % TW;
-                    uint32_t a = bl_sa(s_rng) + 2u * (uint32_t)(col * BL_NB + e);
-                    for (int y = 0; y < TH; y++, a += 2u * BL_NB * (uint32_t)TW) {
-                        const uint32_t rg = bl_lds16(a);
-                        m |= ((rg >> 8) > (rg & 0xff)) ? (1u << y) : 0u;
-                    }
+            // the occupancy bitmasks of the ring walk come out of the same pass: one warp per tile row (TW <= 32), lane = column.
+            // A row word is one ballot per bucket; a lane ORs its column's bits over the warp's rows and adds them to the
+            // (zeroed) column words with one atomicOr per bucket -- distinct words, so the atomics do not collide.
+            const int lane = threadIdx.x & 31;
+            uint32_t colm[BL_NB];
+#pragma unroll
+            for (int e = 0; e < BL_NB; e++) colm[e] = 0;
+            for (int row = threadIdx.x >> 5; row < TH; row += blockDim.x >> 5) {      // warp-uniform
+                const uint32_t occ = lane < TW ? pixel_ranges(row * TW + lane) : 0u;
+#pragma unroll
+                for (int e = 0; e < BL_NB; e++) {
+                    const uint32_t m = __ballot_sync(0xffffffffu, (occ >> e) & 1u);
+                    if (lane == e) s_occ_r[e * TH + row] = m;
+                    colm[e] |= ((occ >> e) & 1u) << row;
                 }
-#else
-                if (idx < BL_NB * TH) {
-                    const int e = idx / TH, row = idx % TH;
-                    for (int x = 0; x < TW; x++) {
-                        const uint32_t rg = s_rng[(row * TW + x) * BL_NB + e];
-                        m |= ((rg >> 8) > (rg & 0xff)) ? (1u << x) : 0u;
-                    }
-                } else {
-                    const int i2 = idx - BL_NB * TH, e = i2 / TW, col = i2 % TW;
-                    for (int y = 0; y < TH; y++) {
-                        const uint32_t rg = s_rng[(y * TW + col) * BL_NB + e];
-                        m |= ((rg >> 8) > (rg & 0xff)) ? (1u << y) : 0u;
-                    }
-                }
-#endif
-                s_occ_r[idx] = m;                                        // s_occ_c follows s_occ_r: [BL_NB][TH] then [BL_NB][TW]
             }
+            if (lane < TW) {
+#pragma unroll
+                for (int e = 0; e < BL_NB; e++)
+                    if (colm[e]) atomicOr(&s_occ_c[e * TW + lane], colm[e]);
+            }
+        } else {
+            for (int i = threadIdx.x; i < TP; i += blockDim.x) pixel_ranges(i);
         }
         __syncthreads();
         if (!bucketed || !T.unsorted) break;                            // block-uniform
         bucketed = false;                                               // records not time-sorted: redo without buckets
+        if (use_rings) {
+            for (int i = threadIdx.x; i < BL_NB * TW; i += blockDim.x) s_occ_c[i] = 0;
+            __syncthreads();
+        }
     }
+    if (threadIdx.x == 0) T.bucketed = bucketed;                        // read after the event loop's first barrier
     // ---- thread <-> event assignment in arrival order (time-homogeneous warps) ------------------------
-    const int nown = p1 - p0;
-    const int own_off = staged ? (p0 - T.run_start[1] + T.run_off[1]) : 0;
     uint32_t mloc = 0;
-    for (int pb0 = 0; pb0 < nown; pb0 += blockDim.x) {
-        const int chunk = min((int)blockDim.x, nown - pb0);
+    for (int pb = p0; pb < p1; pb += blockDim.x) {                      // chunk = own events [pb, pb + chunk)
+        const int chunk = min((int)blockDim.x, p1 - pb);
         __syncthreads();
         // rank of each event of the chunk by arrival index (cell walk only: the ring walk does not need age-sorted warps)
         if (!use_rings && (int)threadIdx.x < chunk) {
-            const int myidx = staged ? s_ti[own_off + pb0 + threadIdx.x].y : ti[p0 + pb0 + threadIdx.x].y;
+            const int d = T.run_off[1] - T.run_start[1];               // staged position - sorted position (run 1)
+            const int myidx = staged ? s_ti[d + pb + threadIdx.x].y : ti[pb + threadIdx.x].y;
             int rank = 0;
             for (int k = 0; k < chunk; k++) {
-                const int oi = staged ? s_ti[own_off + pb0 + k].y : __ldg(&ti[p0 + pb0 + k].y);
+                const int oi = staged ? s_ti[d + pb + k].y : __ldg(&ti[pb + k].y);
                 rank += (oi < myidx) ? 1 : 0;
             }
             s_order[rank] = (uint16_t)threadIdx.x;
@@ -473,7 +478,7 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
         // cell walk (fallback): ranks dealt round-robin so that no warp is the straggler
         const int rank = use_rings ? (int)threadIdx.x : (int)(threadIdx.x & 31) * nw + (int)(threadIdx.x >> 5);
         bool active = rank < chunk;
-        const int p = p0 + pb0 + (active ? (use_rings ? rank : (int)s_order[rank]) : 0);
+        const int p = pb + (active ? (use_rings ? rank : (int)s_order[rank]) : 0);
         int x = 0, y = 0;
         int2 me = make_int2(0, 0);
         if (active) {
@@ -484,7 +489,7 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
         }
         const int tx0 = active ? x - T.X0 : g.r, ty0 = active ? y - T.Y0 : g.r;
         int eb = 0;
-        if (bucketed) eb = min(max(bl_div(me.x, dtw, dtw_inv) - sbase, 0), BL_NB - 1);
+        if (T.bucketed) eb = min(max(bl_div(me.x, dtw, dtw_inv) - sbase, 0), BL_NB - 1);
         int n;
         const int tidx0 = ty0 * TW + tx0;
         if (use_rings) {
@@ -513,44 +518,75 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
         }
         if (active) nbr[(int64_t)(DAGR_ELL - 1) * N + p] = n;
         // phase B: A_u = sum_e tab[c_e][u] * (polarity_src, x_src/W, y_src/H), converged over the ELL slots;
-        // also translates the staged record index into the global sorted position and collects the voxel mask
+        // also translates the staged record index into the global sorted position and collects the voxel mask.
+        // tab[c][k+3j] is rebuilt as wy[j] * wx[k] from the factor tables; __fmul_rn keeps the product from being contracted
+        // into the FMA that consumes it, so every weight has the bits of the [ncell][16] table (geometry.py checks the identity).
+        // A lane's table rows differ from its neighbours': one 64-byte global row per edge and lane touched ~28 L1 lines per
+        // warp-wide load, the factors are conflict-free shared-memory loads.
         const float f0 = active ? feat_s[p] : 0.f, f1 = s_posx[tx0], f2 = s_posy[ty0];
         float A[DAGR_KU][3];
         {
+            const int o = g.r;                                          // self loop: spiral cell 0, offset (0, 0)
+            const float4 wya = s_wy[o];
+            const float wy[5] = {wya.x, wya.y, wya.z, wya.w, s_wy4[o]}, wx[3] = {s_wx[o], s_wx[R + o], s_wx[2 * R + o]};
 #pragma unroll
-            for (int u = 0; u < DAGR_KU; u++) { const float t = __ldg(tab + u); A[u][0] = t * f0; A[u][1] = t * f1; A[u][2] = t * f2; }
-        }
-        const int nmax = __reduce_max_sync(0xffffffffu, n);
-        for (int q = 0; q < nmax; q++) {
-            if (q < n) {
-                int j, c;
-                if (staged) { const uint32_t a = s_acc[q * THREADS + threadIdx.x]; j = (int)(a >> 10); c = (int)(a & 0x3ff); }
-                else { j = nbr[(int64_t)q * N + p]; c = off[(int64_t)q * N + p]; }
-                const int sp = s_sp[c];
-                const int tx = tx0 + (int)(signed char)(sp & 0xff), ty = ty0 + (sp >> 8);
-                const int rr = s_rowv[ty];
-                float e0;
-                if (staged) {
-                    e0 = s_feat[j];
-                    nbr[(int64_t)q * N + p] = j - T.run_off[rr] + T.run_start[rr];
-                    off[(int64_t)q * N + p] = (uint16_t)c;
-                } else e0 = __ldg(feat_s + j);
-                const int dcx = (int)s_colv[tx] - 1, dcy = rr - 1;
-                if (dcx | dcy) mloc |= 1u << ((dcy + 1) * 3 + (dcx + 1));
-                const float e1 = s_posx[tx], e2 = s_posy[ty];
-                const float4 *tr = reinterpret_cast<const float4 *>(tab + c * DAGR_TABW);
-                const float4 t0 = __ldg(tr), t1 = __ldg(tr + 1), t2 = __ldg(tr + 2), t3 = __ldg(tr + 3);
-                const float t[DAGR_KU] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w, t2.x, t2.y, t2.z, t2.w, t3.x, t3.y, t3.z};
+            for (int jy = 0; jy < 5; jy++)
 #pragma unroll
-                for (int u = 0; u < DAGR_KU; u++) {
-                    A[u][0] = fmaf(t[u], e0, A[u][0]);
-                    A[u][1] = fmaf(t[u], e1, A[u][1]);
-                    A[u][2] = fmaf(t[u], e2, A[u][2]);
+                for (int k = 0; k < 3; k++) {
+                    const float t = __fmul_rn(wy[jy], wx[k]);
+                    A[k + 3 * jy][0] = t * f0; A[k + 3 * jy][1] = t * f1; A[k + 3 * jy][2] = t * f2;
                 }
-            }
         }
+        // tile position of spiral offset (-r, -r), x | y << 16: one register fewer through the loop (tile sides < 2^15)
+        int txy = (tx0 - g.r) | ((ty0 - g.r) << 16);
+        // the staged and the global-memory form are separate loops: one loop with both forms predicated needs more registers
+        auto edges = [&](auto staged_c) {
+            constexpr bool ST = decltype(staged_c)::value;
+            for (int q = 0; q < n; q++) {
+                const uint32_t e = (uint32_t)q * (uint32_t)N + (uint32_t)p;     // ELL index: 16 N < 2^28 (N < 2^24 checked)
+                int j, c;
+                if (ST) { const uint32_t a = s_acc[q * THREADS + threadIdx.x]; j = (int)(a >> 10); c = (int)(a & 0x3ff); }
+                else { j = nbr[e]; c = off[e]; }
+                const uint32_t sp = s_sp[c];
+                const int dxi = (int)(sp & 31u), dyi = (int)(sp >> 5);
+                const int txy_e = txy + dxi + (dyi << 16);
+                const int tx = txy_e & 0xffff, ty = txy_e >> 16;
+                // voxel row / column (0..2) of the source pixel: r is smaller than every voxel side (geometry.py), so the tile's
+                // first and last r rows / columns belong to the neighbouring voxels and the rest to this one
+                const int vr = (ty >= g.r) + (ty + g.r >= TH), vc = (tx >= g.r) + (tx + g.r >= TW);
+                float e0;
+                if (ST) {
+                    e0 = s_feat[j];
+                    nbr[e] = j - T.run_off[vr] + T.run_start[vr];
+                    off[e] = (uint16_t)c;
+                } else e0 = __ldg(feat_s + j);
+                mloc |= 1u << (vr * 3 + vc);                            // bit 4 (this voxel) is dropped below
+                const float e1 = s_posx[tx], e2 = s_posy[ty];
+                const float4 wya = s_wy[dyi];
+                const float wy[5] = {wya.x, wya.y, wya.z, wya.w, s_wy4[dyi]}, wx[3] = {s_wx[dxi], s_wx[R + dxi], s_wx[2 * R + dxi]};
+#pragma unroll
+                for (int jy = 0; jy < 5; jy++)
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+                        const int u = k + 3 * jy;
+                        const float t = __fmul_rn(wy[jy], wx[k]);
+                        A[u][0] = fmaf(t, e0, A[u][0]);
+                        A[u][1] = fmaf(t, e1, A[u][1]);
+                        A[u][2] = fmaf(t, e2, A[u][2]);
+                    }
+            }
+        };
+        if (staged) edges(std::true_type{});
+        else        edges(std::false_type{});
+
         if (!active || !do_conv) continue;
         // conv_a phase 2: out = sum_u W_u^T A_u + W_root^T x_i, BN, act  (weights in the constant bank)
+        // the root term's inputs are read again rather than kept live through phase B, which keeps the lean instance within
+        // its 72 registers; the empty asm hides that they are the values read before phase B, so the compiler neither reuses
+        // those nor forms the addresses (and keeps them) before the loop
+        int pr = p;
+        asm volatile("" : "+r"(txy), "+r"(pr));
+        const float r0 = __ldg(feat_s + pr), r1 = s_posx[(txy & 0xffff) + g.r], r2 = s_posy[(txy >> 16) + g.r];
         float o[16];
 #pragma unroll
         for (int k = 0; k < 16; k++) o[k] = 0.f;
@@ -563,9 +599,9 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
 #pragma unroll
         for (int k = 0; k < 16; k++) {
             float r = o[k];
-            r = fmaf(f0, P.root[0][k], r);
-            r = fmaf(f1, P.root[1][k], r);
-            r = fmaf(f2, P.root[2][k], r);
+            r = fmaf(r0, P.root[0][k], r);
+            r = fmaf(r1, P.root[1][k], r);
+            r = fmaf(r2, P.root[2][k], r);
             r = fmaf(r, P.scale[k], P.shift[k]);
             o[k] = P.relu ? fmaxf(r, 0.f) : r;
         }
@@ -578,7 +614,7 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
         dst[sw] = make_float4(o[8], o[9], o[10], o[11]);
         dst[sw ^ 1] = make_float4(o[12], o[13], o[14], o[15]);
     }
-    mloc = __reduce_or_sync(0xffffffffu, mloc);
+    mloc = __reduce_or_sync(0xffffffffu, mloc) & ~(1u << 4);
     if ((threadIdx.x & 31) == 0 && mloc) atomicOr(&s_mask, mloc);
     __syncthreads();
     if (threadIdx.x == 0) cellmask[cell] = (min_idx > 0 ? cellmask[cell] : 0u) | s_mask;
@@ -589,7 +625,7 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
 template <int CAP, int MIN_CTAS>
 __global__ void __launch_bounds__(BL_THREADS, MIN_CTAS)
 k_l1_build(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const int2 *__restrict__ ti,
-           const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s, const float *__restrict__ tab,
+           const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
            const __grid_constant__ dagr_l1a_params_t P, const int do_conv, const int min_idx, const int32_t *__restrict__ flags,
            int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask, float *__restrict__ xa,
            int32_t *__restrict__ wl_hdr, int32_t *__restrict__ wl_ids, const int defer)
@@ -597,14 +633,14 @@ k_l1_build(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, co
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ BLTile T;
     __shared__ uint32_t s_mask;
-    bl_voxel<CAP, BL_THREADS>(g, N, start, ti, xyb, feat_s, tab, P, do_conv, min_idx, flags, nbr, off, cellmask, xa,
+    bl_voxel<CAP, BL_THREADS>(g, N, start, ti, xyb, feat_s, P, do_conv, min_idx, flags, nbr, off, cellmask, xa,
                               (int)blockIdx.x, smem_raw, T, s_mask, wl_hdr, wl_ids, defer);
 }
 
 // dense voxels: persistent CTAs (one per SM) pop voxel ids from the work list the regular kernel filled
 __global__ void __launch_bounds__(BL_THREADS_BIG, 1)
 k_l1_build_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const int2 *__restrict__ ti,
-                 const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s, const float *__restrict__ tab,
+                 const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
                  const __grid_constant__ dagr_l1a_params_t P, const int do_conv, const int min_idx, const int32_t *__restrict__ flags,
                  int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask, float *__restrict__ xa,
                  int32_t *__restrict__ wl_hdr, const int32_t *__restrict__ wl_ids)
@@ -620,7 +656,7 @@ k_l1_build_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ sta
         __syncthreads();
         const int i = s_next;
         if (i >= count) break;
-        bl_voxel<BL_CAP_BIG, BL_THREADS_BIG>(g, N, start, ti, xyb, feat_s, tab, P, do_conv, min_idx, flags, nbr, off, cellmask, xa,
+        bl_voxel<BL_CAP_BIG, BL_THREADS_BIG>(g, N, start, ti, xyb, feat_s, P, do_conv, min_idx, flags, nbr, off, cellmask, xa,
                                              wl_ids[i], smem_raw, T, s_mask, nullptr, nullptr, 0);
     }
 }
@@ -631,6 +667,7 @@ extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *sta
                              uint32_t *cellmask, float *xa, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
 {
     DAGR_CHECK_ARG(g, "null argument");
+    (void)tab;                                                          // the slot weights come from g->tabx / g->taby
     static const dagr_l1a_params_t zero_params = {};
     const int do_conv = p_host != nullptr;
     if (!p_host) p_host = &zero_params;
@@ -643,13 +680,13 @@ extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *sta
         const size_t smem = bl_smem_bytes(g, BL_CAP, BL_THREADS);
         auto kern = k_l1_build<BL_CAP, 4>;
         DAGR_CUDA(dagr_allow_smem(kern, smem, true));
-        kern<<<cells, BL_THREADS, smem, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, tab, *p_host, do_conv, min_idx,
+        kern<<<cells, BL_THREADS, smem, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, do_conv, min_idx,
                                                                 flags, nbr, off, cellmask, xa, wl_hdr, wl_ids, 1);
     } else {
         const size_t smem = bl_smem_bytes(g, BL_CAP_LEAN, BL_THREADS);
         auto kern = k_l1_build<BL_CAP_LEAN, 5>;
         DAGR_CUDA(dagr_allow_smem(kern, smem, true));
-        kern<<<cells, BL_THREADS, smem, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, tab, *p_host, do_conv, min_idx,
+        kern<<<cells, BL_THREADS, smem, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, do_conv, min_idx,
                                                                 flags, nbr, off, cellmask, xa, wl_hdr, wl_ids, 0);
     }
     DAGR_CHECK_LAUNCH();
@@ -662,7 +699,7 @@ extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *sta
             DAGR_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
         }
         DAGR_CUDA(dagr_allow_smem(k_l1_build_dense, smem_big));
-        k_l1_build_dense<<<n_sm, BL_THREADS_BIG, smem_big, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, tab,
+        k_l1_build_dense<<<n_sm, BL_THREADS_BIG, smem_big, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s,
                                                                                     *p_host, do_conv, min_idx, flags, nbr, off,
                                                                                     cellmask, xa, wl_hdr, wl_ids);
         DAGR_CHECK_LAUNCH();

@@ -143,7 +143,9 @@ int dagr_graph_search(const dagr_geom_t *g, int64_t N, const int32_t *start, con
  * cell-major order), probes the spiral entirely on chip, writes the ELL adjacency + cellmask exactly like
  * dagr_graph_search and applies conv_block1.conv_block1 (SplineConv 3->16 + BN + act, see dagr_l1_conv_a)
  * to the neighbours as they are found -> xa (half-major [2][N][8]).  cellmask needs no zeroing for this
- * entry point.  With p_host == NULL only the adjacency / cellmask are produced (image path). */
+ * entry point.  With p_host == NULL only the adjacency / cellmask are produced (image path).  The per-edge slot
+ * weights come from the per-axis factor tables g->tabx / g->taby; `tab` is not read by this kernel any more (kept in
+ * the signature for ABI stability, may be NULL). */
 struct dagr_l1a_params_s;
 int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
                   const uint32_t *xyb, const float *feat_s, const float *tab,
