@@ -83,6 +83,8 @@ _SIGS = {
     "dagr_graph_sort": (C.c_int, [C.POINTER(Geom), p, p, p, i64, p, p, p, p, p, p, p, p, p, p, p]),
     "dagr_graph_sort_ring": (C.c_int, [C.POINTER(Geom), p, p, p, i64, p, p, p, p, p, p, p, p, p, p, p, p]),
     "dagr_stream_push": (C.c_int, [p, p, p, p, p, i64, C.c_int, C.c_int, p]),
+    "dagr_stream_push_multi": (C.c_int, [p, p, p, p, p, i64, C.c_int, C.c_int, p]),
+    "dagr_graph_sort_rings": (C.c_int, [C.POINTER(Geom), p, p, p, i64, C.c_int, p, p, p, p, p, p, p, p, p, p, p, p]),
     "dagr_graph_search": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p]),
     "dagr_l1_build": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, C.POINTER(L1AParams), p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
     "dagr_xa_permute": (C.c_int, [i64, p, C.c_int, p, p, C.c_int, p]),

@@ -145,7 +145,7 @@ class Engine:
         self._out_slot = {}
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
-    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
+    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
                      dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
                      dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1)
@@ -506,16 +506,21 @@ class Engine:
     @torch.no_grad()
     def forward_events(self, batch_i32: torch.Tensor, pos_i32: torch.Tensor, feat: torch.Tensor, B: int,
                        W: int, H: int, image_feats=None, image_outs=None, stream_state=None, n_old: int = 0, ring=None,
-                       image_event=None):
+                       image_event=None, ring_streams=None):
         """batch int32[N], pos int32[N,3], feat fp32[N] (polarity) on CUDA -> decoded [B, A, 5+nc].
 
         ring = device control block (int32[8], dagr_graph_sort_ring): the three inputs are ring buffers of N = capacity
         slots whose live window {head, count} is only known on the device; every launch then covers the capacity, nothing
-        depends on a host-side count and the whole call can sit inside one captured CUDA graph (dagr_b200.streaming)."""
+        depends on a host-side count and the whole call can sit inside one captured CUDA graph (dagr_b200.streaming).
+        ring_streams = S: `ring` is the int32[S+1][8] block of S rings of N / S slots each (dagr_graph_sort_rings), stream s
+        being sample s of B = S."""
         for n, t in (("batch", batch_i32), ("pos", pos_i32), ("x", feat)):
             _lib.require_cuda(t, n)
         dev = pos_i32.device
         N = int(batch_i32.shape[0])
+        if ring_streams is not None and (ring is None or int(ring_streams) != int(B) or N % int(ring_streams)):
+            raise ValueError(f"ring_streams={ring_streams} needs a ring control block, B == ring_streams and N a multiple of it "
+                             f"(B={B}, N={N})")
         geom = self.geometry(W, H, B, dev)
         pk = self.pack(geom, dev)
         ws = self.workspace(geom, N, dev)
@@ -553,7 +558,12 @@ class Engine:
         wl_hdr = self._zs(ws, "wl_hdr", torch.int32)
         defer = self._dense_policy(ws, wl_hdr, ring is not None or stream_state is not None)
         # ---- event level ---------------------------------------------------------------------
-        if ring is not None:
+        if ring is not None and ring_streams is not None:
+            self._run("graph_sort", lib.dagr_graph_sort_rings, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), N // ring_streams,
+                      int(ring_streams), _lib.ptr(ring), _lib.ptr(ws["key"]), _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]),
+                      _lib.ptr(ws["blocksums"]), _lib.ptr(ws["start"]), _lib.ptr(ws["perm"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
+                      _lib.ptr(ws["feat_s"]), _lib.ptr(flags), st)
+        elif ring is not None:
             self._run("graph_sort", lib.dagr_graph_sort_ring, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), N, _lib.ptr(ring),
                       _lib.ptr(ws["key"]), _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]), _lib.ptr(ws["blocksums"]), _lib.ptr(ws["start"]),
                       _lib.ptr(ws["perm"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(flags), st)

@@ -15,6 +15,10 @@ How a step works (everything on the device, ONE CUDA graph replay per chunk, no 
                --> coarse stack, head, NMS    fixed-shape launches
                --D2H--> pinned detections
 
+MultiStreamDetector runs S such streams (S cameras) as the S samples of ONE step: S rings, a packed stage, and
+dagr_stream_push_multi / dagr_graph_sort_rings in place of the single-ring calls; everything below the sort already
+works on a batch.  The step is still one CUDA graph replay.
+
 Why the event level is recomputed over the window instead of patched: evicting an event changes the neighbour lists of
 every node it fed (the K cap admits the next candidate of the spiral), i.e. of the window's oldest 10 ms -- and their
 activations feed the next 10 ms.  At 50 k live events the per-voxel kernels take ~0.1 ms for the WHOLE window
@@ -32,30 +36,41 @@ import torch
 from . import _lib
 
 
-class StreamingDetector:
-    """det = StreamingDetector(model, window_us=50_000); det.push(x, y, t, p) -> list with one dict(boxes, scores, labels)."""
+RING_CTL = 8                          # ints per stream in a control block (DAGR_RING_CTL)
+MAX_STREAMS = 127                     # dagr_stream_push_multi: 1 <= S <= 127
+MAX_RING_SLOTS = 1 << 24              # S * capacity < 2^24: sorted positions are packed in 24 bits
 
-    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
-        if model.backbone.use_image:
-            raise NotImplementedError("streaming mode drives the events-only model")
+
+def _pow2_at_least(n: int) -> int:
+    cap = 1
+    while cap < n:
+        cap <<= 1
+    return cap
+
+
+class _RingDetector:
+    """What StreamingDetector and MultiStreamDetector share: the device rings of `streams` x `cap` slots, a pinned stage
+    and its device copy, and the step itself -- H2D of the stage, push, forward over the live windows, NMS, D2H of the
+    detections and of the control block.  The first two steps run eagerly (they allocate every buffer of the step); the
+    second is followed by one capture, and every later step is one replay of that CUDA graph."""
+
+    def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device):
         self.model, self.eng = model, model.engine
         self.lib = self.eng.lib
         self.W, self.H = int(model.width), int(model.height)
         self.window_us, self.max_chunk = int(window_us), int(max_chunk)
-        cap = 1
-        while cap < capacity:
-            cap <<= 1
-        self.cap = cap
+        self.cap = _pow2_at_least(capacity)
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("dagr_b200: streaming needs a CUDA device (no CPU fallback)")
         self.dev = dev
-        self.batch = torch.zeros(cap, dtype=torch.int32, device=dev)
-        self.pos = torch.zeros((cap, 3), dtype=torch.int32, device=dev)
-        self.feat = torch.zeros(cap, dtype=torch.float32, device=dev)
-        self.ctl = torch.zeros(8, dtype=torch.int32, device=dev)
-        self.stage_h = torch.zeros(4 + 4 * self.max_chunk, dtype=torch.int32).pin_memory()
-        self.stage_d = torch.zeros(4 + 4 * self.max_chunk, dtype=torch.int32, device=dev)
+        n = streams * self.cap
+        self.batch = torch.zeros(n, dtype=torch.int32, device=dev)
+        self.pos = torch.zeros((n, 3), dtype=torch.int32, device=dev)
+        self.feat = torch.zeros(n, dtype=torch.float32, device=dev)
+        nstage = 4 * streams + 4 * streams * self.max_chunk
+        self.stage_h = torch.zeros(nstage, dtype=torch.int32).pin_memory()
+        self.stage_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
         self._stage_np = self.stage_h.numpy()
         self.stream = torch.cuda.Stream(device=dev)
         self.graph = None
@@ -63,49 +78,26 @@ class StreamingDetector:
         self._done = None
         self._warm = 0
 
-    # ------------------------------------------------------------------------------------------------------------
-    def reset(self):
-        if self._done is not None:
-            self._done.synchronize()
-        self.ctl.zero_()
+    def _push(self):
+        raise NotImplementedError
 
     def _enqueue(self):
         """one streaming step on the current stream (eager or under capture)."""
         m, eng = self.model, self.eng
         self.stage_d.copy_(self.stage_h, non_blocking=True)
-        _lib.check(self.lib.dagr_stream_push(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
-                                             _lib.ptr(self.feat), self.cap, self.max_chunk, 0, _lib.stream_ptr()), "stream_push")
+        self._push()
         eng.launches += 2
-        dec = eng.forward_events(self.batch, self.pos, self.feat, 1, self.W, self.H, ring=self.ctl)
+        dec = eng.forward_events(self.batch, self.pos, self.feat, self._B, self.W, self.H, ring=self.ctl, ring_streams=self._ring_streams)
         det, ndet = eng.postprocess(dec, m.conf_threshold, m.nms_threshold, self.W, self.H)
         if self._res_h is None:
             self._res_h = (torch.empty(det.shape, dtype=det.dtype).pin_memory(), torch.empty(ndet.shape, dtype=ndet.dtype).pin_memory(),
-                           torch.empty(8, dtype=torch.int32).pin_memory())
+                           torch.empty(self.ctl.shape, dtype=torch.int32).pin_memory())
         self._res_h[0].copy_(det, non_blocking=True)
         self._res_h[1].copy_(ndet, non_blocking=True)
         self._res_h[2].copy_(self.ctl, non_blocking=True)
 
-    def _fill_stage(self, x, y, t, p, t_end):
-        n = int(len(t))
-        if n > self.max_chunk:
-            raise ValueError(f"chunk of {n} events exceeds max_chunk={self.max_chunk}")
-        st = self._stage_np
-        st[0] = n
-        st[1] = int(t_end) - self.window_us
-        if n:
-            ev = st[4:4 + 4 * n].reshape(n, 4)
-            ev[:, 0] = x; ev[:, 1] = y; ev[:, 2] = t; ev[:, 3] = p
-
-    @torch.no_grad()
-    def submit(self, x, y, t, p, t_end=None):
-        """enqueue one chunk (host arrays: pixel x, y, timestamp t in us (int32 range, non-decreasing across pushes),
-        polarity -1/+1).  `t_end` = end of the chunk's time slice (default: its last timestamp); events older than
-        t_end - window_us leave the live window.  Returns immediately; `result()` blocks on the step."""
-        if self._done is not None:
-            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
-        if t_end is None:
-            t_end = int(t[-1]) if len(t) else int(self._stage_np[1]) + self.window_us
-        self._fill_stage(np.asarray(x), np.asarray(y), np.asarray(t), np.asarray(p), t_end)
+    def _step(self):
+        """enqueue one step (the stage is filled) on the detector's stream behind the caller's stream."""
         cur = torch.cuda.current_stream(self.dev)
         with torch.cuda.stream(self.stream):
             self.stream.wait_stream(cur)
@@ -130,13 +122,73 @@ class StreamingDetector:
             ev.record(self.stream)
         self._done = ev
 
+    def _dets(self, s: int):
+        det_h, ndet_h, _ = self._res_h
+        n = int(ndet_h[s])
+        d = det_h[s, :n]
+        return dict(boxes=d[:, :4].clone(), scores=d[:, 4].clone(), labels=d[:, 5].long())
+
+    def _state(self, s: int):
+        self._done.synchronize()
+        c = self._res_h[2][RING_CTL * s:RING_CTL * (s + 1)]
+        return dict(head=int(c[0]), live=int(c[1]), evicted=int(c[2]), appended=int(c[3]), overflow=bool(c[4]))
+
+    def _live(self, s: int):
+        self._done.synchronize()
+        torch.cuda.synchronize(self.dev)
+        head, n = int(self.ctl[RING_CTL * s]), int(self.ctl[RING_CTL * s + 1])
+        idx = s * self.cap + ((head + torch.arange(n, device=self.dev)) & (self.cap - 1))
+        return self.pos[idx], self.feat[idx]
+
+
+class StreamingDetector(_RingDetector):
+    """det = StreamingDetector(model, window_us=50_000); det.push(x, y, t, p) -> list with one dict(boxes, scores, labels)."""
+
+    _B, _ring_streams = 1, None
+
+    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+        if model.backbone.use_image:
+            raise NotImplementedError("streaming mode drives the events-only model")
+        self._setup(model, 1, window_us, max_chunk, capacity, device)
+        self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
+
+    # ------------------------------------------------------------------------------------------------------------
+    def reset(self):
+        if self._done is not None:
+            self._done.synchronize()
+        self.ctl.zero_()
+
+    def _push(self):
+        _lib.check(self.lib.dagr_stream_push(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
+                                             _lib.ptr(self.feat), self.cap, self.max_chunk, 0, _lib.stream_ptr()), "stream_push")
+
+    def _fill_stage(self, x, y, t, p, t_end):
+        n = int(len(t))
+        if n > self.max_chunk:
+            raise ValueError(f"chunk of {n} events exceeds max_chunk={self.max_chunk}")
+        st = self._stage_np
+        st[0] = n
+        st[1] = int(t_end) - self.window_us
+        if n:
+            ev = st[4:4 + 4 * n].reshape(n, 4)
+            ev[:, 0] = x; ev[:, 1] = y; ev[:, 2] = t; ev[:, 3] = p
+
+    @torch.no_grad()
+    def submit(self, x, y, t, p, t_end=None):
+        """enqueue one chunk (host arrays: pixel x, y, timestamp t in us (int32 range, non-decreasing across pushes),
+        polarity -1/+1).  `t_end` = end of the chunk's time slice (default: its last timestamp); events older than
+        t_end - window_us leave the live window.  Returns immediately; `result()` blocks on the step."""
+        if self._done is not None:
+            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
+        if t_end is None:
+            t_end = int(t[-1]) if len(t) else int(self._stage_np[1]) + self.window_us
+        self._fill_stage(np.asarray(x), np.asarray(y), np.asarray(t), np.asarray(p), t_end)
+        self._step()
+
     def result(self):
         """detections of the last submitted chunk: [dict(boxes f32[n,4] xyxy px, scores f32[n], labels i64[n])] (host tensors)."""
         self._done.synchronize()
-        det_h, ndet_h, _ = self._res_h
-        n = int(ndet_h[0])
-        d = det_h[0, :n]
-        return [dict(boxes=d[:, :4].clone(), scores=d[:, 4].clone(), labels=d[:, 5].long())]
+        return [self._dets(0)]
 
     def push(self, x, y, t, p, t_end=None):
         self.submit(x, y, t, p, t_end)
@@ -145,17 +197,123 @@ class StreamingDetector:
     @property
     def window_state(self):
         """(head slot, live events, evicted by the last step, appended by the last step, overflow flag) of the last finished step."""
-        self._done.synchronize()
-        c = self._res_h[2]
-        return dict(head=int(c[0]), live=int(c[1]), evicted=int(c[2]), appended=int(c[3]), overflow=bool(c[4]))
+        return self._state(0)
 
     def live_window(self):
         """(pos int32[n,3], polarity f32[n]) of the live window in arrival order (host sync; for tests)."""
+        return self._live(0)
+
+
+def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int):
+    """write the packed multi-stream stage of dagr_stream_push_multi into the int32 array `stage` (>= 4*S + 4*S*max_chunk
+    entries): header [S][4] = {n_new, t_cut, event offset, 0}, then the (x, y, t, polarity) rows of all streams back to back.
+    chunks[s] = (x, y, t, p) host arrays or None (no events).  Returns the per-stream event counts."""
+    S = len(chunks)
+    ns = [0 if c is None else len(c[2]) for c in chunks]
+    for s, n in enumerate(ns):
+        if n > max_chunk:
+            raise ValueError(f"stream {s}: chunk of {n} events exceeds max_chunk={max_chunk}")
+    if len(stage) < 4 * S + 4 * S * max_chunk:
+        raise ValueError(f"stage of {len(stage)} ints is smaller than 4*S + 4*S*max_chunk = {4 * S + 4 * S * max_chunk}")
+    hdr = stage[:4 * S].reshape(S, 4)
+    ev = stage[4 * S:4 * S + 4 * S * max_chunk].reshape(S * max_chunk, 4)
+    o = 0
+    for s, (c, n) in enumerate(zip(chunks, ns)):
+        hdr[s] = (n, int(t_cut[s]), o, 0)
+        if n:
+            x, y, t, p = c
+            e = ev[o:o + n]
+            e[:, 0] = x; e[:, 1] = y; e[:, 2] = t; e[:, 3] = p
+        o += n
+    return ns
+
+
+class MultiStreamDetector(_RingDetector):
+    """S independent event cameras on one GPU: det = MultiStreamDetector(model, streams=S, window_us=50_000);
+    det.push([(x, y, t, p) or None per stream]) -> S dicts(boxes, scores, labels).
+
+    Stream s is sample s of one batched step: its events sit in ring s (`capacity` slots), its window is evicted by its own
+    t_cut, and all S windows go through one sort, one event level, one coarse stack and one NMS -- the whole step is one
+    CUDA graph replay.  Each stream's detections are those of a StreamingDetector fed the same chunks, and those of the
+    synchronous forward over its live window.  All streams share the model (and so its W x H); each keeps its own time base,
+    and timestamps only need to be non-decreasing within a stream.  One step advances every stream: a stream with nothing
+    new passes None or an empty chunk."""
+
+    def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+        if model.backbone.use_image:
+            raise NotImplementedError("streaming mode drives the events-only model")
+        S = int(streams)
+        if not 1 <= S <= MAX_STREAMS:
+            raise ValueError(f"streams={streams}: 1 <= streams <= {MAX_STREAMS}")
+        cap = _pow2_at_least(capacity)
+        if S * cap >= MAX_RING_SLOTS:
+            raise ValueError(f"streams * capacity = {S} * {cap} must be < 2^24 (sorted positions are packed in 24 bits)")
+        if not 1 <= int(max_chunk) <= cap:
+            raise ValueError(f"max_chunk={max_chunk} must be in [1, capacity={cap}]")
+        self.S = self._B = self._ring_streams = S
+        self._setup(model, S, window_us, max_chunk, cap, device)
+        self.ctl = torch.zeros((S + 1) * RING_CTL, dtype=torch.int32, device=self.dev)
+        self.stage_bytes = 4 * self.stage_h.numel()
+
+    def _push(self):
+        _lib.check(self.lib.dagr_stream_push_multi(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
+                                                   _lib.ptr(self.feat), self.cap, self.S, self.max_chunk, _lib.stream_ptr()),
+                   "stream_push_multi")
+
+    def reset(self, stream=None):
+        """forget the live window of one stream (the others keep theirs) or of all streams."""
+        if self._done is not None:
+            self._done.synchronize()
+        if stream is None:
+            self.ctl.zero_()
+        else:
+            s = int(stream)
+            if not 0 <= s < self.S:
+                raise IndexError(f"stream {stream} out of range [0, {self.S})")
+            self.ctl[RING_CTL * s:RING_CTL * (s + 1)].zero_()
+
+    @torch.no_grad()
+    def submit(self, chunks, t_end=None):
+        """enqueue one step: chunks[s] = (x, y, t, p) host arrays of stream s (as StreamingDetector.submit) or None.
+        t_end[s] = end of stream s's time slice (None, or t_end=None: its last timestamp, or for an empty chunk the previous
+        end).  Returns immediately; `result()` blocks on the step."""
+        S = self.S
+        if len(chunks) != S:
+            raise ValueError(f"{len(chunks)} chunks for {S} streams")
+        if t_end is not None and len(t_end) != S:
+            raise ValueError(f"{len(t_end)} t_end values for {S} streams")
+        cs = [None if c is None or len(c[2]) == 0 else tuple(np.asarray(a) for a in c) for c in chunks]
+        for s, c in enumerate(cs):
+            if c is not None and len(c[2]) > self.max_chunk:
+                raise ValueError(f"stream {s}: chunk of {len(c[2])} events exceeds max_chunk={self.max_chunk}")
+        if self._done is not None:
+            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
+        hdr = self._stage_np[:4 * S].reshape(S, 4)
+        t_cut = []
+        for s, c in enumerate(cs):
+            te = None if t_end is None else t_end[s]
+            if te is None:
+                te = int(c[2][-1]) if c is not None else int(hdr[s, 1]) + self.window_us
+            t_cut.append(int(te) - self.window_us)
+        pack_stage(self._stage_np, cs, t_cut, self.max_chunk)
+        self._step()
+
+    def result(self):
+        """detections of the last step, one dict(boxes f32[n,4] xyxy px, scores f32[n], labels i64[n]) per stream (host tensors)."""
         self._done.synchronize()
-        torch.cuda.synchronize(self.dev)
-        head, n = int(self.ctl[0]), int(self.ctl[1])
-        idx = (head + torch.arange(n, device=self.dev)) & (self.cap - 1)
-        return self.pos[idx], self.feat[idx]
+        return [self._dets(s) for s in range(self.S)]
+
+    def push(self, chunks, t_end=None):
+        self.submit(chunks, t_end)
+        return self.result()
+
+    def window_state(self, s: int):
+        """stream s after the last finished step: head slot, live events, evicted / appended by the step, sticky overflow flag."""
+        return self._state(s)
+
+    def live_window(self, s: int):
+        """(pos int32[n,3], polarity f32[n]) of stream s's live window in arrival order (host sync; for tests)."""
+        return self._live(s)
 
 
 def synth_stream(rate_ev_s: int, seconds: float, width: int, height: int, seed: int = 99, kind: str = "uniform"):
@@ -222,3 +380,66 @@ def stream_benchmark(dev, size="l", width=640, height=480, rate_ev_s=1_000_000, 
                      "wall clock from submit() to the detections being readable on the host, chunks submitted back to back "
                      "(sustained_mev_s = events / busy time: how much faster than the 1 Mevents/s feed the loop runs); Python's cyclic garbage "
                      "collector is paused during the timed loop")
+
+
+def multistream_benchmark(dev, streams, size="l", width=640, height=480, rate_ev_s=1_000_000, chunk_us=1000, window_us=50_000,
+                          seconds=2.0, kind="uniform", model=None, capacity=1 << 17):
+    """config 5 with S cameras on ONE GPU: S independent synthetic streams (seeds 99, 100, ...) at `rate_ev_s` each, all
+    advanced by one MultiStreamDetector step per chunk period.  Latency mode as in stream_benchmark: a step is submitted,
+    the detections of all S streams are awaited on the host, then the next step is submitted."""
+    from .model.dagr import DAGR
+    from .utils.args import default_args
+    S = int(streams)
+    if model is None:
+        from tests.helpers import randomize_bn
+        torch.manual_seed(0)
+        model = randomize_bn(DAGR(default_args(size, batch_size=1), height=height, width=width).eval()).to(dev)
+    total_s = seconds + window_us * 1e-6 + 0.02
+    evs_s = [synth_stream(rate_ev_s, total_s, width, height, seed=99 + s, kind=kind) for s in range(S)]
+    det = MultiStreamDetector(model, streams=S, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)),
+                              capacity=capacity)
+    grid = np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us)
+    bounds = [np.searchsorted(e[2], grid) for e in evs_s]
+    nchunks = len(grid) - 1
+    lat, dev_ms, evs = [], [], []
+    warm = int(window_us / chunk_us) + 20                                # fill the live windows first (+ graph capture)
+    import gc
+    gc_was = gc.isenabled()
+    gc.collect()
+    gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
+    for k in range(nchunks):
+        chunks = []
+        for (x, y, t, p), bd in zip(evs_s, bounds):
+            a, b = int(bd[k]), int(bd[k + 1])
+            chunks.append((x[a:b], y[a:b], t[a:b], p[a:b]))
+        t_end = [(k + 1) * chunk_us] * S
+        if k >= warm:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0 = time.perf_counter()
+            e0.record(det.stream)
+            det.submit(chunks, t_end)
+            e1.record(det.stream)
+            det.result()
+            lat.append((time.perf_counter() - t0) * 1e3)
+            dev_ms.append(e0.elapsed_time(e1))
+            evs.append(sum(len(c[2]) for c in chunks))
+        else:
+            det.push(chunks, t_end)
+    if gc_was:
+        gc.enable()
+    st = [det.window_state(s) for s in range(S)]
+    lat_s, dev_s = sorted(lat), sorted(dev_ms)
+    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
+    busy = sum(lat) * 1e-3
+    return dict(model=f"dagr-{size}", streams=S, kind=kind, stream_rate_mev_s=rate_ev_s / 1e6, chunk_us=chunk_us, window_us=window_us,
+                stream_seconds=len(lat) * chunk_us * 1e-6, steps=len(lat), events_per_step=float(np.mean(evs)),
+                stage_bytes=det.stage_bytes, live_events=[x["live"] for x in st], overflow=[x["overflow"] for x in st],
+                latency_ms=dict(p50=q(lat_s, 0.5), p90=q(lat_s, 0.9), p99=q(lat_s, 0.99), max=lat_s[-1]),
+                device_ms=dict(p50=q(dev_s, 0.5), p99=q(dev_s, 0.99)),
+                sustained_mev_s=sum(evs) / busy / 1e6, realtime=bool(q(lat_s, 0.99) * 1e3 <= chunk_us),
+                realtime_margin=chunk_us / (q(lat_s, 0.5) * 1e3),
+                note=f"{S} independent streams on one GPU, one MultiStreamDetector step per chunk period: H2D of the packed stage "
+                     "(fixed size), per-stream eviction + append into S device rings, one batched forward over the S live windows, "
+                     "NMS, D2H of the detections -- one CUDA graph replay; latency = host wall clock from submit() until the "
+                     "detections of all streams are readable on the host; sustained_mev_s = events of all streams / busy time; "
+                     "Python's cyclic garbage collector is paused during the timed loop")

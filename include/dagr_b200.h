@@ -32,6 +32,7 @@ extern "C" {
 #define DAGR_ELL 16            /* neighbour slots per node (K-1 = 15 used, slot 15 = degree) */
 #define DAGR_KU  15            /* spline kernel slots reachable at the event level (3 x 5)   */
 #define DAGR_TABW 16           /* row stride (floats) of the offset->slot-weight table       */
+#define DAGR_RING_CTL 8        /* ints per stream in a streaming control block (ctl)          */
 
 int         dagr_abi_version(void);
 const char *dagr_last_error(void);
@@ -133,6 +134,27 @@ int dagr_graph_sort_ring(const dagr_geom_t *g, const int32_t *batch, const int32
                          int32_t *flags, void *stream);
 int dagr_stream_push(int32_t *ctl, const int32_t *stage, int32_t *batch, int32_t *pos, float *feat, int64_t capacity,
                      int max_chunk, int sample, void *stream);
+
+/* Multi-stream form: S independent event streams (cameras) become the S samples of one step.  Ring s owns slots
+ * [s*capacity, (s+1)*capacity) of batch/pos/feat (S*capacity slots in all); `capacity` is the per-stream ring size.
+ *   ctl   i32[S+1][8] on the DEVICE, zero-initialised.  Block s = {head slot inside ring s, live count, evicted by the last
+ *         push, appended by the last push, sticky overflow flag, kept count, offset of the stream's window in the compact
+ *         stream-major order, 0}; block S = {total live count, 0...}.  Zeroing block s resets stream s alone.
+ *   stage i32[4*S + 4*S*max_chunk] on the device: header [S][4] = {n_new, t_cut, event offset, 0}, then the (x, y, t,
+ *         polarity +-1) events of all streams back to back; stream s's n_new events start at event `offset`.
+ *   dagr_stream_push_multi : per stream, evicts the prefix with t < t_cut and appends its chunk (batch = s); then writes the
+ *         window offsets (exclusive scan of the live counts) and the total.  Two launches, grids independent of the counts.
+ *   dagr_graph_sort_rings  : dagr_graph_sort over the S live windows read in the compact order c < total: stream s's i-th
+ *         live event has arrival index c = offset_s + i.  Outputs as dagr_graph_sort with B = S; downstream kernels take
+ *         N = S*capacity.  dagr_graph_sort_ring is this sort with S = 1 and a single i32[8] block.
+ * Limits (DAGR_E_ARG before anything is launched): no null pointer (flags may be NULL), 1 <= S <= 127, capacity a power of
+ * two, S*capacity < 2^24 (sorted positions are packed in 24 bits), 1 <= max_chunk <= capacity, and for the sort S == g->B. */
+int dagr_stream_push_multi(int32_t *ctl, const int32_t *stage, int32_t *batch, int32_t *pos, float *feat, int64_t capacity,
+                           int streams, int max_chunk, void *stream);
+int dagr_graph_sort_rings(const dagr_geom_t *g, const int32_t *batch, const int32_t *pos, const float *feat,
+                          int64_t capacity, int streams, const int32_t *ctl, int32_t *key, int32_t *tmp, int32_t *count,
+                          int32_t *blocksums, int32_t *start, int32_t *perm, int32_t *ti, uint32_t *xyb, float *feat_s,
+                          int32_t *flags, void *stream);
 
 int dagr_graph_search(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
                       const uint32_t *xyb, int32_t *nbr, uint16_t *off, uint32_t *cellmask,
