@@ -52,15 +52,18 @@ __device__ __forceinline__ float bilin_sample(const float *__restrict__ img, int
 // x0[chunk][p][8] = the 16 image channels sampled at the event (two 8-channel chunks); the two 16-byte halves of a row are
 // swapped when XA_SWZ(p), like xa, so that the staged conv kernel (conv_l1.cu) reads both with the same row addressing.
 // (polarity, x/W, y/H) -- the other three inputs of conv_block1.conv_block1 -- need no gather and are handled by the probe kernel.
-__global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
+// live = start of the sort (or NULL): only positions p < start[g.NK] (the live total) are sampled.  In ring mode N is the ring
+// capacity and the sorted positions at or beyond the live total hold stale or never-written xyb words, whose x / y would index
+// past posx0 / posy0; the rows they would fill are never read (conv_a_image, conv_b and voxel_sample_max walk the voxels'
+// [start[cell], start[cell+1]) ranges, which lie below the total), so they are simply skipped.  live == NULL: the bound is N.
+__global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ live, const uint32_t *__restrict__ xyb,
                               const float *__restrict__ img0, int h, int w, float *__restrict__ x0)
 {
     // 4 threads per node: thread q computes image channels 4q..4q+3 = one 16-byte chunk of a row
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t p = t >> 2;
     const int q = (int)(t & 3);
-    if (p >= N) return;
-    (void)feat_s;
+    if (p >= (live != nullptr ? min((int64_t)__ldg(live + g.NK), N) : N)) return;
     const uint32_t wd = xyb[p];
     const int x = wd & 0xfff, y = (wd >> 12) & 0xfff, b = wd >> 24;
     const float px = g.posx0[x], py = g.posy0[y];
@@ -75,8 +78,21 @@ __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const uint32_t *__
 extern "C" int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s, const float *img0,
                                 int h, int w, float *x0, void *stream)
 {
+    (void)feat_s;
     if (N <= 0) return DAGR_OK;
-    k_l1_x0_image<<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, xyb, feat_s, img0, h, w, x0);
+    k_l1_x0_image<<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, nullptr, xyb, img0, h, w, x0);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_l1_x0_image_live(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                                     const float *img0, int h, int w, float *x0, void *stream)
+{
+    (void)feat_s;
+    DAGR_CHECK_ARG(g && start && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    if (N == 0) return DAGR_OK;
+    k_l1_x0_image<<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

@@ -145,7 +145,7 @@ class Engine:
         self._out_slot = {}
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
-    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
+    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
                      dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
                      dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1)
@@ -584,8 +584,14 @@ class Engine:
             f0 = image_feats[0]
             x0 = self._buf(ws, "x0img", (2 * max(N, 1) * 8,), torch.float32, dev)
             skipv = self._buf(ws, "skipv", (max(N, 1), 16), torch.float32, dev)
-            self._run("l1_x0_image", lib.dagr_l1_x0_image, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(f0),
-                      int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
+            if ring is not None:
+                # N = ring capacity: positions behind the live total hold stale xyb words, so the launch is bounded by the
+                # total the sort wrote (start[NK]); the synchronous path keeps the unbounded form (N is the live count there)
+                self._run("l1_x0_image", lib.dagr_l1_x0_image_live, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
+                          _lib.ptr(f0), int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
+            else:
+                self._run("l1_x0_image", lib.dagr_l1_x0_image, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(f0),
+                          int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
             self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
                       _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off),
                       C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),

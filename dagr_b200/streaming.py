@@ -19,6 +19,9 @@ MultiStreamDetector runs S such streams (S cameras) as the S samples of ONE step
 dagr_stream_push_multi / dagr_graph_sort_rings in place of the single-ring calls; everything below the sort already
 works on a batch.  The step is still one CUDA graph replay.
 
+FusionStreamingDetector streams the hybrid (image + events) model: a camera frame runs through the image trunk once, into one
+of two frame slots, and every chunk's step (one replay of that slot's graph) reads the newest frame whose trunk has finished.
+
 Why the event level is recomputed over the window instead of patched: evicting an event changes the neighbour lists of
 every node it fed (the K cap admits the next candidate of the spiral), i.e. of the window's oldest 10 ms -- and their
 activations feed the next 10 ms.  At 50 k live events the per-voxel kernels take ~0.1 ms for the WHOLE window
@@ -52,7 +55,9 @@ class _RingDetector:
     """What StreamingDetector and MultiStreamDetector share: the device rings of `streams` x `cap` slots, a pinned stage
     and its device copy, and the step itself -- H2D of the stage, push, forward over the live windows, NMS, D2H of the
     detections and of the control block.  The first two steps run eagerly (they allocate every buffer of the step); the
-    second is followed by one capture, and every later step is one replay of that CUDA graph."""
+    second is followed by one capture, and every later step is one replay of that CUDA graph.  A detector whose steps read
+    different buffers (FusionStreamingDetector's two frame slots) keeps one graph per _graph_key(); a key first used after
+    the warm-up is captured right after its first (eager) step."""
 
     def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device):
         self.model, self.eng = model, model.engine
@@ -73,10 +78,23 @@ class _RingDetector:
         self.stage_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
         self._stage_np = self.stage_h.numpy()
         self.stream = torch.cuda.Stream(device=dev)
-        self.graph = None
+        self.graphs = {}                      # _graph_key() -> captured step
         self._res_h = None
         self._done = None
         self._warm = 0
+
+    @property
+    def graph(self):
+        """the captured step (None until the second step has run)."""
+        return self.graphs.get(0)
+
+    def _graph_key(self):
+        """which captured step the next step replays (a step graph bakes in every pointer it reads)."""
+        return 0
+
+    def _image_inputs(self):
+        """(image_feats, image_outs) of the next step: None for the events-only model."""
+        return None, None
 
     def _push(self):
         raise NotImplementedError
@@ -87,7 +105,9 @@ class _RingDetector:
         self.stage_d.copy_(self.stage_h, non_blocking=True)
         self._push()
         eng.launches += 2
-        dec = eng.forward_events(self.batch, self.pos, self.feat, self._B, self.W, self.H, ring=self.ctl, ring_streams=self._ring_streams)
+        feats, outs = self._image_inputs()
+        dec = eng.forward_events(self.batch, self.pos, self.feat, self._B, self.W, self.H, image_feats=feats, image_outs=outs,
+                                 ring=self.ctl, ring_streams=self._ring_streams)
         det, ndet = eng.postprocess(dec, m.conf_threshold, m.nms_threshold, self.W, self.H)
         if self._res_h is None:
             self._res_h = (torch.empty(det.shape, dtype=det.dtype).pin_memory(), torch.empty(ndet.shape, dtype=ndet.dtype).pin_memory(),
@@ -99,10 +119,12 @@ class _RingDetector:
     def _step(self):
         """enqueue one step (the stage is filled) on the detector's stream behind the caller's stream."""
         cur = torch.cuda.current_stream(self.dev)
+        key = self._graph_key()
         with torch.cuda.stream(self.stream):
             self.stream.wait_stream(cur)
-            if self.graph is not None:
-                self.graph.replay()
+            graph = self.graphs.get(key)
+            if graph is not None:
+                graph.replay()
                 self.eng.launches += self._graph_launches
             else:
                 l0 = self.eng.launches
@@ -117,7 +139,7 @@ class _RingDetector:
                         self._enqueue()
                     self.eng.launches -= self._graph_launches          # capture enqueues nothing
                     self.ctl.copy_(saved)                              # (the captured step did not run)
-                    self.graph = g
+                    self.graphs[key] = g
             ev = torch.cuda.Event()
             ev.record(self.stream)
         self._done = ev
@@ -202,6 +224,149 @@ class StreamingDetector(_RingDetector):
     def live_window(self):
         """(pos int32[n,3], polarity f32[n]) of the live window in arrival order (host sync; for tests)."""
         return self._live(0)
+
+
+class FusionStreamingDetector(StreamingDetector):
+    """Streaming detection with the hybrid (image + events) model: camera frames at frame rate, event chunks in between.
+
+        det = FusionStreamingDetector(model, window_us=50_000)
+        fid = det.set_frame(image_u8)          # u8 [3,H,W] or [1,3,H,W], host or device -> frame id 0, 1, 2, ...
+        det.push(x, y, t, p)                   # as StreamingDetector: one CUDA graph replay per chunk
+
+    A frame runs through the model's own ImageBranch (ResNet trunk + CNN head, the captured graphs that model(data)
+    replays) once, on the branch's side stream, and its five feature maps and CNN head maps are copied into one of two frame
+    slots owned by the detector.  Each slot has its own captured step graph, so a step is still one replay.
+
+    Which frame a step uses: the newest frame whose trunk has finished when the chunk is submitted (a non-blocking event
+    query).  Chunks keep flowing on the previous frame while the next frame's trunk runs; sync_frame() blocks until the
+    pending frame is usable, so the next step uses it.  The first step waits for the first frame.  After every step the
+    detections equal model(data) over the live window with the image of the frame that frame_state reports.
+
+    Two hazards are ordered on the device: a slot is overwritten only after the last step that read it (the copy waits for
+    that step), and the branch's static output buffers are overwritten (by the next frame or a model(data) call) only after
+    the copy out of them (the branch stream waits for the copy)."""
+
+    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+        if not model.backbone.use_image:
+            raise ValueError("FusionStreamingDetector drives an image-fusion model (backbone.use_image); "
+                             "stream an events-only model with StreamingDetector")
+        if model.head.no_events:
+            raise NotImplementedError("--no_events: the model has no event path to stream")
+        self._setup(model, 1, window_us, max_chunk, capacity, device)
+        self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
+        self.frame_stream = torch.cuda.Stream(device=self.dev)
+        self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
+        self._reader = [None, None]           # per slot: done-event of the last step that read it
+        self._cur = None                      # slot of the newest usable frame
+        self._cur_frame = None                # (id, t_us) of that frame
+        self._pending = None                  # frame whose trunk may still run: dict(slot, id, t_us, ready, trunk)
+        self._step_frame = (None, None)       # (id, t_us) of the frame the last submitted step used
+        self._overlapped = False              # the last submitted step ran while a newer frame's trunk was in flight
+        self._nframes = 0
+        self._img_h = self._h2d = None
+
+    # ------------------------------------------------------------------------------------------------------------
+    def _check_frame(self, image):
+        if not isinstance(image, torch.Tensor):
+            image = torch.from_numpy(np.ascontiguousarray(image))
+        if image.dtype != torch.uint8:
+            raise ValueError(f"frame dtype {image.dtype}: expected uint8 (raw camera pixels)")
+        if image.dim() == 4 and image.shape[0] == 1:
+            image = image[0]
+        if image.dim() != 3 or tuple(image.shape) != (3, self.H, self.W):
+            raise ValueError(f"frame of shape {tuple(image.shape)}: expected [3, {self.H}, {self.W}] or [1, 3, {self.H}, {self.W}]")
+        return image.unsqueeze(0)
+
+    def _promote(self):
+        pend, self._pending = self._pending, None
+        self.stream.wait_event(pend["ready"])                         # no-op once it completed; orders the very first frame
+        self._cur, self._cur_frame = pend["slot"], (pend["id"], pend["t_us"])
+
+    @torch.no_grad()
+    def set_frame(self, image, t_us=None):
+        """start a new frame: the trunk runs on the device, this returns without waiting for it.  `image` u8 [3,H,W] or
+        [1,3,H,W] (host or device); `t_us` is the caller's timestamp of the frame, reported back by frame_state.
+        Returns the frame id (0, 1, 2, ...).  A frame still pending is waited for and becomes current first."""
+        from .model.image_branch import ImageBranch
+        img = self._check_frame(image)
+        self.sync_frame()
+        slot = 0 if self._cur is None else 1 - self._cur
+        m, fs = self.model, self.frame_stream
+        if m._image_branch is None:
+            m._image_branch = ImageBranch(m)
+        br = m._image_branch
+        cur = torch.cuda.current_stream(self.dev)
+        if img.is_cuda:
+            x = img.to(self.dev).float() / 255.0                       # on the caller's stream, ordered with its writes
+        elif self._img_h is None:
+            self._img_h = torch.empty(img.shape, dtype=torch.uint8).pin_memory()
+        with torch.cuda.stream(fs):
+            fs.wait_stream(cur)
+            if not img.is_cuda:
+                if self._h2d is not None:
+                    self._h2d.synchronize()                            # the previous frame's upload has left the pinned stage
+                self._img_h.copy_(img)
+                x = self._img_h.to(self.dev, non_blocking=True).float() / 255.0   # as format_data
+                self._h2d = torch.cuda.Event()
+                self._h2d.record(fs)
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record(fs)
+            feats, outs, (_, ev2) = br.run(x, use_graph=m.image_graph)
+            x.record_stream(fs)
+            x.record_stream(br.stream)
+            fs.wait_event(ev2)
+            t1.record(fs)
+            if self._slots is None:
+                self._slots = [([torch.empty_like(f) for f in feats], {k: [torch.empty_like(t) for t in v] for k, v in outs.items()})
+                               for _ in range(2)]
+            if self._reader[slot] is not None:
+                fs.wait_event(self._reader[slot])                     # the last step that read this slot is done
+            dst_f, dst_o = self._slots[slot]
+            for d, s in zip(dst_f, feats):
+                d.copy_(s)
+            for k, v in outs.items():
+                for d, s in zip(dst_o[k], v):
+                    d.copy_(s)
+            ready = torch.cuda.Event()
+            ready.record(fs)
+        br.stream.wait_event(ready)                                   # the branch's static outputs outlive the copy
+        fid = self._nframes
+        self._nframes += 1
+        self._pending = dict(slot=slot, id=fid, t_us=t_us, ready=ready, trunk=(t0, t1))
+        return fid
+
+    def sync_frame(self):
+        """block until the pending frame (if any) is usable; the next step uses it."""
+        if self._pending is not None:
+            self._pending["ready"].synchronize()
+            self._promote()
+
+    def _graph_key(self):
+        return self._cur
+
+    def _image_inputs(self):
+        return self._slots[self._cur]
+
+    @torch.no_grad()
+    def submit(self, x, y, t, p, t_end=None):
+        """as StreamingDetector.submit; the step uses the newest frame whose trunk has finished (see the class docstring)."""
+        if self._pending is not None and (self._cur is None or self._pending["ready"].query()):
+            self._promote()
+        if self._cur is None:
+            raise RuntimeError("FusionStreamingDetector: set_frame() must be called before the first chunk")
+        self._overlapped = self._pending is not None
+        super().submit(x, y, t, p, t_end)
+        self._reader[self._cur] = self._done
+        self._step_frame = self._cur_frame
+
+    @property
+    def frame_state(self):
+        """dict(frame=id of the frame the last finished step used, t_us=its timestamp, pending=id of a frame not yet in use
+        or None)."""
+        if self._done is not None:
+            self._done.synchronize()
+        fid, t_us = self._step_frame
+        return dict(frame=fid, t_us=t_us, pending=None if self._pending is None else self._pending["id"])
 
 
 def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int):
@@ -443,3 +608,94 @@ def multistream_benchmark(dev, streams, size="l", width=640, height=480, rate_ev
                      "NMS, D2H of the detections -- one CUDA graph replay; latency = host wall clock from submit() until the "
                      "detections of all streams are readable on the host; sustained_mev_s = events of all streams / busy time; "
                      "Python's cyclic garbage collector is paused during the timed loop")
+
+
+def fusion_stream_benchmark(dev, size="s", img_net="resnet50", width=640, height=480, rate_ev_s=1_000_000, chunk_us=1000,
+                            window_us=50_000, seconds=2.0, frame_us=50_000, sync_frames=False, kind="uniform", model=None,
+                            step_priority=0):
+    """config 3's hybrid model on config 5's stream: one event stream in `chunk_us` chunks and a new camera frame every
+    `frame_us` of stream time, through FusionStreamingDetector.  Latency mode as in stream_benchmark (a chunk is submitted,
+    its detections are awaited, then the next one); frames are set between two chunks, followed by sync_frame() when
+    `sync_frames`.  Frames are seeded random u8 images on the host (the trunk's cost does not depend on the pixels).
+    step_priority < 0 runs the steps on a higher-priority stream than the trunk's (an experiment: does it shield the chunks?)."""
+    from .model.dagr import DAGR
+    from .utils.args import default_args
+    if model is None:
+        from tests.helpers import randomize_bn
+        torch.manual_seed(0)
+        model = randomize_bn(DAGR(default_args(size, batch_size=1, use_image=True, img_net=img_net), height=height, width=width).eval()).to(dev)
+    total_s = seconds + window_us * 1e-6 + 0.02
+    x, y, t, p = synth_stream(rate_ev_s, total_s, width, height, kind=kind)
+    g = torch.Generator().manual_seed(0)
+    frames = [torch.randint(0, 256, (3, height, width), generator=g, dtype=torch.uint8) for _ in range(4)]
+    det = FusionStreamingDetector(model, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)))
+    if step_priority:
+        det.stream = torch.cuda.Stream(device=det.dev, priority=step_priority)      # before the first step: captures inherit it
+    bounds = np.searchsorted(t, np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us))
+    nchunks = len(bounds) - 1
+    lat, dev_ms, evs, overlapped, set_ms, trunk, first_use = [], [], [], [], [], [], []
+    waiting = {}                                                         # frame id -> host time of its set_frame
+    warm = int(window_us / chunk_us) + 20                                # fill the live window first (+ both graph captures)
+    import gc
+    gc_was = gc.isenabled()
+    gc.collect()
+    gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
+    for k in range(nchunks):
+        a, b = int(bounds[k]), int(bounds[k + 1])
+        t_end = (k + 1) * chunk_us
+        if (k * chunk_us) % frame_us == 0:                              # the camera delivers a frame at stream time k * chunk_us
+            ts = time.perf_counter()
+            fid = det.set_frame(frames[(k * chunk_us // frame_us) % len(frames)], t_us=k * chunk_us)
+            tr = det._pending["trunk"]
+            if sync_frames:
+                det.sync_frame()
+            if k >= warm:
+                set_ms.append((time.perf_counter() - ts) * 1e3)
+                trunk.append(tr)
+                waiting[fid] = ts
+        if k >= warm:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0 = time.perf_counter()
+            e0.record(det.stream)
+            det.submit(x[a:b], y[a:b], t[a:b], p[a:b], t_end)
+            e1.record(det.stream)
+            det.result()
+            t1 = time.perf_counter()
+            lat.append((t1 - t0) * 1e3)
+            dev_ms.append(e0.elapsed_time(e1))
+            evs.append(b - a)
+            overlapped.append(det._overlapped)
+            fid = det._step_frame[0]
+            if fid in waiting:
+                first_use.append((t1 - waiting.pop(fid)) * 1e3)
+        else:
+            det.push(x[a:b], y[a:b], t[a:b], p[a:b], t_end)
+    if gc_was:
+        gc.enable()
+    torch.cuda.synchronize(dev)
+    trunk_ms = [a.elapsed_time(b) for a, b in trunk]
+    st = det.window_state
+    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
+
+    def dist(v):
+        v = sorted(v)
+        return dict(n=len(v), p50=q(v, 0.5), p99=q(v, 0.99), max=v[-1]) if v else dict(n=0)
+
+    busy = sum(lat) * 1e-3
+    return dict(model=f"dagr-{size} + {img_net}", width=width, height=height, stream_rate_mev_s=rate_ev_s / 1e6, chunk_us=chunk_us,
+                window_us=window_us, frame_us=frame_us, sync_frames=bool(sync_frames), step_priority=step_priority, stream_seconds=len(lat) * chunk_us * 1e-6,
+                chunks=len(lat), frames=len(trunk_ms), events_per_chunk=float(np.mean(evs)), live_events=st["live"], overflow=st["overflow"],
+                latency_ms=dist(lat), latency_ms_trunk_in_flight=dist([v for v, o in zip(lat, overlapped) if o]),
+                latency_ms_no_trunk=dist([v for v, o in zip(lat, overlapped) if not o]),
+                device_ms=dist(dev_ms), trunk_device_ms=dist(trunk_ms), set_frame_host_ms=dist(set_ms),
+                frame_to_first_use_ms=dist(first_use), sustained_mev_s=sum(evs) / busy / 1e6,
+                note="one hybrid stream on one GPU: every chunk is one CUDA graph replay of the step of the current frame slot; every "
+                     "frame_us of stream time a host u8 frame goes through the ResNet trunk + CNN head (captured ImageBranch graphs) on "
+                     "a side stream and is copied into the free slot.  latency = host wall clock from submit() to the detections on the "
+                     "host; *_trunk_in_flight = chunks submitted while a newer frame's trunk had not finished (they use the previous "
+                     "frame); device_ms = CUDA events around the step on the detector's stream; trunk_device_ms = CUDA events around "
+                     "the branch on the frame stream; set_frame_host_ms = host time of set_frame (+ sync_frame when sync_frames); "
+                     "frame_to_first_use_ms = host time from set_frame until the detections of the first step using that frame are on "
+                     "the host; chunks are submitted back to back, faster than the real 1 ms period, so frames arrive every "
+                     "frame_us / chunk_us chunks rather than every frame_us of wall time; Python's cyclic garbage collector is paused "
+                     "during the timed loop")

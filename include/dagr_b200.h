@@ -193,6 +193,12 @@ int dagr_xa_permute(int64_t N, const int32_t *perm, int n_old, float *xa_sorted,
  * sampling follows net.py:193-221 (grid_sample, align_corners=True, batch as depth). */
 int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
                      const float *img0 /*[B,16,h,w]*/, int h, int w, float *x0, void *stream);
+/* Same kernel and results, bounded by the live total start[g->NK] that the sort wrote (device data): sorted positions at or
+ * beyond it are not read.  This is the form for the ring sorts, where N is the ring capacity and the positions behind the
+ * live window hold stale or never-written xyb words.  feat_s is not read and may be NULL; any other null pointer, or N outside
+ * [0, 2^31), returns DAGR_E_ARG with a message before anything is launched. */
+int dagr_l1_x0_image_live(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                          const float *img0 /*[B,16,h,w]*/, int h, int w, float *x0, void *stream);
 
 typedef struct {
     float w[DAGR_KU][24][16];     /* slot-major spline weights, input channels padded 19 -> 24 */
