@@ -15,9 +15,27 @@ appending events never changes the inputs of an existing node.  Consequently
 The reference's correctness criterion is kept and tightened: after any number of steps the outputs equal the
 dense forward over all events seen so far (evaluate_flops.py:139-147 uses 1e-3; tests use 1e-5).
 
+Image fusion (--use_image)
+--------------------------
+The frame is fixed between re-seeds, as in the reference's criterion (evaluate_flops.py:13-14 hands the same image to
+both halves).  The model's own ImageBranch (the captured trunk + CNN head graphs that model(data) replays) runs once per
+frame; its feature maps and CNN head maps are copied into buffers owned by the wrapper.  Per step, with a fixed frame:
+  * x0 (the 16 conv1 samples at every event) is resampled for ALL events -- a pure function of (event, frame), O(N) like
+    the sort, and a new node's conv reads its older neighbours' rows;
+  * conv_block1.conv_block1 convolves only the new nodes (old rows are gathered from arrival storage, as above);
+  * the 64-channel samples concatenated before pool1 keep a per-voxel running max (StreamState.imgmax): only new events
+    are sampled, voxels without new events copy their running max;
+  * the coarse levels are recomputed densely with the cached layer2..4 taps and CNN head maps.
+Frame rules (one policy): the first step after reset() needs chunk.image (formatted fp32 [B,3,H,W], as format_data makes
+it), else ValueError before any device work.  Later, a chunk without an image, with the frame tensor itself or with an
+equal one (torch.equal, one sync) is an incremental step; a different image is a new frame: the trunk runs on it, the
+running state is re-seeded and the step is one full pass over every event seen so far with the new frame (the rebuild
+evict_older_than does).  evict_older_than rebuilds with the current frame.
+
 Limits (documented, SURVEY H7): append-only between reset()s -- evicting old events changes the inputs of the
 nodes they fed, which needs a re-probe of those nodes; `evict_older_than` therefore rebuilds the live window
-with one dense pass.  Events-only model (no image fusion) in streaming mode.
+with one dense pass.  --no_events models have no event path and are refused; so is pooling_aggr: mean (the running
+per-voxel aggregate is a max, as in the reference's async pooling).
 """
 from __future__ import annotations
 
@@ -33,15 +51,19 @@ class StreamState:
         self.xa_arr = None        # f32[cap,16]  conv_block1.conv_block1 activations in arrival order
         self.voxmax = None        # f32[cells,16] running per-voxel channel max (pool1)
         self.cellmask = None      # i32[cells]   running coarse in-edge mask of pool1 voxels
+        self.imgmax = None        # f32[cells,C] running per-voxel max of the image samples before pool1 (image fusion only)
         self.n = 0
         self._geom_id = None
 
-    def ensure(self, geom, N, dev):
+    def ensure(self, geom, N, dev, img_channels: int = 0):
         if self._geom_id != (geom.W, geom.H, geom.B, geom.r):
             self.voxmax = torch.full((geom.cells1, 16), float("-inf"), dtype=torch.float32, device=dev)
             self.cellmask = torch.zeros(geom.cells1, dtype=torch.int32, device=dev)
+            self.imgmax = None
             self._geom_id = (geom.W, geom.H, geom.B, geom.r)
             self.cap = 0
+        if img_channels and (self.imgmax is None or self.imgmax.shape[1] != img_channels):
+            self.imgmax = torch.full((geom.cells1, img_channels), float("-inf"), dtype=torch.float32, device=dev)
         if N > self.cap:
             cap = max(int(N * 1.5), 4096)
             new = torch.empty((cap, 16), dtype=torch.float32, device=dev)
@@ -54,26 +76,79 @@ class StreamState:
         if self.voxmax is not None:
             self.voxmax.fill_(float("-inf"))
             self.cellmask.zero_()
+        if self.imgmax is not None:
+            self.imgmax.fill_(float("-inf"))
 
 
 class AsyncDAGR:
-    """stateful wrapper: `step(chunk)` appends events and returns the detections for everything seen so far."""
+    """stateful wrapper: `step(chunk)` appends events and returns the detections for everything seen so far.  With an
+    image-fusion model the chunk also carries the frame (see the module docstring for the frame rules)."""
 
     def __init__(self, model):
-        if model.backbone.use_image:
-            raise NotImplementedError("streaming mode supports the events-only model")
+        if model.head.no_events:
+            raise NotImplementedError("--no_events: the model has no event path to update incrementally")
         self.model = model
+        self.use_image = bool(model.backbone.use_image)
         self.state = StreamState()
         self._batch = self._pos = self._feat = None
         self._hb = self._hp = self._hf = None
         self._n = 0
         self.B = self.W = self.H = None
+        self._image = None                  # the frame: the caller's tensor (identity test) and a copy (content test)
+        self._image_copy = None
+        self._feats = self._outs = None     # the frame's feature maps / CNN head maps, copied out of the branch's graph buffers
+        self.frames = 0                     # frames run through the trunk since construction
 
     def reset(self):
         self.state.reset()
         self._batch = self._pos = self._feat = None
         self._hb = self._hp = self._hf = None
         self._n = 0
+        self._image = self._image_copy = None
+
+    def _new_frame(self, image):
+        """run the frame through the model's own ImageBranch and copy its outputs into buffers of this wrapper: the branch's
+        outputs are static graph buffers that the next model(data) overwrites."""
+        from .model.image_branch import ImageBranch
+        m = self.model
+        if m._image_branch is None:
+            m._image_branch = ImageBranch(m)
+        br = m._image_branch
+        cur = torch.cuda.current_stream(image.device)
+        feats, outs, (_, ev2) = br.run(image, use_graph=m.image_graph)
+        cur.wait_event(ev2)                                          # the copy waits for the whole branch
+        if (self._feats is None or [tuple(f.shape) for f in feats] != [tuple(f.shape) for f in self._feats]
+                or {k: [tuple(t.shape) for t in v] for k, v in outs.items()} != {k: [tuple(t.shape) for t in v] for k, v in self._outs.items()}):
+            self._feats = [torch.empty_like(f) for f in feats]
+            self._outs = {k: [torch.empty_like(t) for t in v] for k, v in outs.items()}
+        for d, s in zip(self._feats, feats):
+            d.copy_(s)
+        for k, v in outs.items():
+            for d, s in zip(self._outs[k], v):
+                d.copy_(s)
+        copied = torch.cuda.Event()
+        copied.record(cur)
+        br.stream.wait_event(copied)                                 # the branch's buffers outlive the copy
+        self._image, self._image_copy = image, image.clone()
+        self.frames += 1
+
+    def _frame_inputs(self, chunk, B):
+        """apply the frame rules to chunk.image -> (image_feats, image_outs, new_frame)."""
+        img = getattr(chunk, "image", None)
+        if img is not None and (img.dim() != 4 or int(img.shape[0]) != B or int(img.shape[1]) != 3 or not img.is_floating_point()):
+            raise ValueError(f"chunk.image of shape {tuple(img.shape)} and dtype {img.dtype}: expected a formatted float "
+                             f"[{B}, 3, H, W] frame (format_data)")
+        if self._image is None:
+            if img is None:
+                raise ValueError("the first step after reset() of an image-fusion model needs chunk.image (the stream's frame)")
+        elif img is None or img is self._image:
+            return self._feats, self._outs, False
+        else:
+            img = img.to(self._image_copy.device)
+            if img.shape == self._image_copy.shape and torch.equal(img, self._image_copy):
+                return self._feats, self._outs, False
+        self._new_frame(img if img.is_cuda else img.to(chunk.pos.device))
+        return self._feats, self._outs, True
 
     @property
     def num_events(self):
@@ -84,8 +159,12 @@ class AsyncDAGR:
         """chunk: formatted EventBatch (same contract as DAGR.forward); events of a sample must be newer than the
         ones already seen for that sample.  Returns decoded head outputs [B, A, 5+nc]."""
         m = self.model
-        batch_i, pos_i, feat, W, H = m._prepare_events(chunk)
         B = int(batch_size or getattr(chunk, "num_graphs", 1) or 1)
+        image_feats = image_outs = None
+        new_frame = False
+        if self.use_image:
+            image_feats, image_outs, new_frame = self._frame_inputs(chunk, B)
+        batch_i, pos_i, feat, W, H = m._prepare_events(chunk)
         k = int(batch_i.shape[0])
         if self._hb is None:
             self.B, self.W, self.H = B, W, H
@@ -105,7 +184,12 @@ class AsyncDAGR:
         self._n = n0 + k
         self._batch, self._pos, self._feat = self._hb[: self._n], self._hp[: self._n], self._hf[: self._n]
         n_old = self.state.n
-        dec = m.engine.forward_events(self._batch, self._pos, self._feat, self.B, self.W, self.H, stream_state=self.state, n_old=n_old)
+        if new_frame and n_old:
+            # a new frame changes the inputs of every node: re-seed the running state with one full pass over all events
+            self.state.reset()
+            n_old = 0
+        dec = m.engine.forward_events(self._batch, self._pos, self._feat, self.B, self.W, self.H, image_feats=image_feats,
+                                      image_outs=image_outs, stream_state=self.state, n_old=n_old)
         self.state.n = self.num_events
         return dec
 
@@ -122,15 +206,16 @@ class AsyncDAGR:
 
     @torch.no_grad()
     def evict_older_than(self, t_us: int):
-        """sliding window: drop events with t < t_us and rebuild the state with one dense pass over the live window."""
+        """sliding window: drop events with t < t_us and rebuild the state with one dense pass over the live window (with
+        the current frame for an image-fusion model)."""
         if self._batch is None:
             return
         keep = self._pos[:, 2] >= int(t_us)
         self._batch, self._pos, self._feat = self._batch[keep].contiguous(), self._pos[keep].contiguous(), self._feat[keep].contiguous()
         self._hb, self._hp, self._hf, self._n = self._batch, self._pos, self._feat, int(self._batch.shape[0])
         self.state.reset()
-        dec = self.model.engine.forward_events(self._batch, self._pos, self._feat, self.B, self.W, self.H, stream_state=self.state,
-                                               n_old=0)
+        dec = self.model.engine.forward_events(self._batch, self._pos, self._feat, self.B, self.W, self.H, image_feats=self._feats,
+                                               image_outs=self._outs, stream_state=self.state, n_old=0)
         self.state.n = self.num_events
         return dec
 

@@ -686,8 +686,9 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
     // nodes and take one x-slot each (both channel halves), their partial sums are added through shared memory: a third of
     // the serial work per thread.  Block-uniform; the dense path below is unchanged.
     // (compiled into the image-fusion instance only: in the 2-chunk conv_block2 instance the extra live state costs the
-    // dense path 1.3 % and the sparse gain is small, measured)
-    const bool sparse = MODE_A && staged && nown <= 32 && min_idx <= 0;
+    // dense path 1.3 % and the sparse gain is small, measured).  Incremental steps take the same path, so that a new node gets
+    // the bits the synchronous forward gives it (the passes skip the nodes that are not active).
+    const bool sparse = MODE_A && staged && nown <= 32;
     const int lane_ = threadIdx.x & 31, wid_ = threadIdx.x >> 5;
     for (int pb0 = p0; pb0 < p1; pb0 += blockDim.x) {
         const int p = sparse ? p0 + lane_ : pb0 + threadIdx.x;
@@ -1114,6 +1115,26 @@ extern "C" int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const in
     DAGR_CHECK_ARG(wfrag, "null weight fragments (dagr_l1_tc_weights)");
     return conv_a_image<CB2_TC != 0>(g, N, start, xyb, feat_s, x0, nbr, off, p_host, (const float4 *)wfrag, xa, skipv, wl_hdr, wl_ids, defer,
                                      (cudaStream_t)stream);
+}
+
+// incremental stream step of the same instances: only nodes with arrival index ti[p].y >= min_idx are convolved, their xa rows
+// (the probe's event-channel sums) finished and their skipv rows written.  The rows of older nodes hold final activations
+// gathered from arrival storage and are not touched.  min_idx == 0 takes every node: the bits of dagr_l1_conv_a_image_tc.
+extern "C" int dagr_l1_conv_a_image_inc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                                        const float *feat_s, const float *x0, const int32_t *nbr, const uint16_t *off,
+                                        const dagr_l1img_params_t *p_host, const float *wfrag, int min_idx, float *xa, float *skipv,
+                                        int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
+{
+    DAGR_CHECK_ARG(g && start && xyb && ti && feat_s && x0 && nbr && off && p_host && wfrag && xa && skipv,
+                   "null argument (only wl_hdr / wl_ids may be NULL)");
+    DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    if (N == 0) return DAGR_OK;
+    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
+    return cb2_launch<dagr_l1img_params_t, 2, true, CB2_TC != 0>(g, N, start, xyb, (const int2 *)ti, feat_s, x0, nbr, off, p_host,
+                                                                  (const float4 *)wfrag, nullptr, min_idx, nullptr, nullptr, nullptr,
+                                                                  nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr, wl_ids, defer,
+                                                                  (cudaStream_t)stream);
 }
 
 // host-side packing of the weight fragments the tensor-core instances read (layout: see cb2_tc_kstep)

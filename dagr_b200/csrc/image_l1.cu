@@ -139,10 +139,15 @@ __device__ __forceinline__ float vs_sample(const float *__restrict__ img, const 
 // MEAN: the pooling's aggregation (pooling.py:74-77, args.pooling_aggr); max in every shipped config
 template <bool MEAN> __device__ __forceinline__ float vs_comb(float a, float b) { return MEAN ? a + b : fmaxf(a, b); }
 
-template <bool MEAN>
+// INC (incremental stream step, max only): persist f32[cells][C] holds the running per-voxel max of the samples between steps
+// (the reference's async pool1 keeps a running max of the concatenated x, max_pool.py:59-62).  min_idx > 0: only events with
+// arrival index ti[p].y >= min_idx are sampled and their max is combined with persist; a voxel without such events copies
+// persist and stages nothing.  min_idx == 0 samples every event (the bits of the plain instance) and seeds persist.
+template <bool MEAN, bool INC>
 __global__ void __launch_bounds__(VS_THREADS)
 k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
-                   const float *__restrict__ img, int C, int h, int w, float *__restrict__ xg, int ldx, int c0)
+                   const int2 *__restrict__ ti, const float *__restrict__ img, int C, int h, int w, const int min_idx,
+                   float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0)
 {
     __shared__ float s_m[VS_THREADS / 32][128];
     __shared__ __align__(16) float s_patch[VS_SMEM_FLOATS];
@@ -152,9 +157,31 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
     const int p0 = start[(int64_t)cell * g.CP], p1 = start[(int64_t)(cell + 1) * g.CP];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     if (p1 == p0) {                                                       // block-uniform
-        for (int c = threadIdx.x; c < C; c += blockDim.x) xg[(int64_t)cell * ldx + c0 + c] = 0.f;
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+            xg[(int64_t)cell * ldx + c0 + c] = 0.f;
+            if (INC && min_idx <= 0) persist[(int64_t)cell * C + c] = -INFINITY;
+        }
         return;
     }
+    if (INC && min_idx > 0) {
+        bool any = false;
+        for (int p = p0 + (int)threadIdx.x; p < p1 && !any; p += blockDim.x) any = __ldg(&ti[p].y) >= min_idx;
+        if (!__syncthreads_or(any)) {                                     // nothing new in this voxel: keep its running max
+            for (int c = threadIdx.x; c < C; c += blockDim.x) xg[(int64_t)cell * ldx + c0 + c] = persist[(int64_t)cell * C + c];
+            return;
+        }
+    }
+    // the events sampled in this launch (INC: the new ones)
+    auto take = [&](int p) { return !INC || min_idx <= 0 || __ldg(&ti[p].y) >= min_idx; };
+    // the voxel's result for channel c: INC combines it with the running max and stores it back
+    auto finish = [&](int c, float v) {
+        if (INC) {
+            float *pc = persist + (int64_t)cell * C + c;
+            if (min_idx > 0) v = fmaxf(v, *pc);
+            *pc = v;
+        }
+        xg[(int64_t)cell * ldx + c0 + c] = v;
+    };
     // window of the map this voxel's pixels can touch: the sample coordinates are monotone in x / y, so the corner
     // pixels bound it (same arithmetic as the per-event set-up)
     const Bilin lo = bilin_setup(g.posx0[g.vx0[cx]], g.posy0[g.vy0[cy]], b, (float)g.W, (float)g.H, g.B, h, w);
@@ -181,7 +208,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
         for (int k = 0; k < 8; k++) m[k] = MEAN ? 0.f : -INFINITY;
         for (int pb = p0 + wid * epw; pb < p1; pb += (VS_THREADS / 32) * epw) {
             const int p = pb + sub;
-            if (p < p1) {
+            if (p < p1 && take(p)) {
                 const uint32_t wd = xyb[p];
                 const int x = wd & 0xfff, y = (wd >> 12) & 0xfff;
                 const Bilin q = bilin_setup(g.posx0[x], g.posy0[y], b, (float)g.W, (float)g.H, g.B, h, w);
@@ -228,7 +255,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
         for (int c = threadIdx.x; c < C; c += blockDim.x) {
             float v = s_mm[c];
             for (int w2 = 1; w2 < VS_THREADS / 32; w2++) v = vs_comb<MEAN>(v, s_mm[w2 * 128 + c]);
-            xg[(int64_t)cell * ldx + c0 + c] = MEAN ? __fdiv_rn(v, (float)(p1 - p0)) : v;
+            finish(c, MEAN ? __fdiv_rn(v, (float)(p1 - p0)) : v);
         }
         return;
     }
@@ -236,6 +263,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
         const float ident = MEAN ? 0.f : -INFINITY;
         float m[4] = {ident, ident, ident, ident};
         for (int p = p0 + wid; p < p1; p += VS_THREADS / 32) {
+            if (!take(p)) continue;
             const uint32_t wd = xyb[p];
             const int x = wd & 0xfff, y = (wd >> 12) & 0xfff;
             const Bilin bl = bilin_setup(g.posx0[x], g.posy0[y], b, (float)g.W, (float)g.H, g.B, h, w);
@@ -254,7 +282,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
         if (c < C) {
             float v = s_m[0][threadIdx.x];
             for (int w2 = 1; w2 < VS_THREADS / 32; w2++) v = vs_comb<MEAN>(v, s_m[w2][threadIdx.x]);
-            xg[(int64_t)cell * ldx + c0 + c] = MEAN ? __fdiv_rn(v, (float)(p1 - p0)) : v;
+            finish(c, MEAN ? __fdiv_rn(v, (float)(p1 - p0)) : v);
         }
         __syncthreads();
     }
@@ -265,8 +293,26 @@ extern "C" int dagr_voxel_sample_max(const dagr_geom_t *g, int64_t N, const int3
 {
     (void)N;
     const int cells = g->B * g->ny1 * g->nx1;
-    if (pool_mean) k_voxel_sample_max<true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, img, C, h, w, xg, ldx, c0);
-    else           k_voxel_sample_max<false><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, img, C, h, w, xg, ldx, c0);
+    if (pool_mean) k_voxel_sample_max<true, false><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
+                                                                                                 nullptr, xg, ldx, c0);
+    else           k_voxel_sample_max<false, false><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
+                                                                                                  nullptr, xg, ldx, c0);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_voxel_sample_max_inc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                                         const float *img, int C, int h, int w, int min_idx, float *persist, float *xg, int ldx, int c0,
+                                         int pool_mean, void *stream)
+{
+    DAGR_CHECK_ARG(g && start && xyb && ti && img && persist && xg, "null argument");
+    DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
+    DAGR_CHECK_ARG(!pool_mean, "pool_mean: the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
+    const int cells = g->B * g->ny1 * g->nx1;
+    k_voxel_sample_max<false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, (const int2 *)ti, img, C, h, w, min_idx,
+                                                                                   persist, xg, ldx, c0);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

@@ -146,6 +146,7 @@ class Engine:
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
     _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
+                     dagr_l1_conv_a_image_inc=2, dagr_voxel_sample_max_inc=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
                      dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
                      dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1)
@@ -548,10 +549,9 @@ class Engine:
         min_idx, persist = 0, None
         if stream_state is not None:
             # incremental step: the first n_old arrival indices were processed before; only newer events get
-            # their edges / activations computed (the causal graph never changes an old node's inputs)
-            if image_feats is not None:
-                raise NotImplementedError("streaming updates are implemented for the events-only model")
-            stream_state.ensure(geom, N, dev)
+            # their edges / activations computed (the causal graph never changes an old node's inputs).  With image fusion
+            # the frame is the same for every step between two re-seeds (dagr_b200.asynchronous)
+            stream_state.ensure(geom, N, dev, img_channels=int(image_feats[1].shape[1]) if image_feats is not None else 0)
             cellmask, persist, min_idx = stream_state.cellmask, stream_state.voxmax, int(n_old)
         poolmax = self._zs(ws, "poolmax", torch.int32)
         flags = self._zs(ws, "flags", torch.int32)
@@ -574,10 +574,13 @@ class Engine:
                       _lib.ptr(ws["feat_s"]), _lib.ptr(flags), st)
         use_image = image_feats is not None
         if use_image:
+            if stream_state is not None and min_idx > 0:
+                self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
+                          _lib.ptr(stream_state.xa_arr), 0, st)
             # adjacency + the (polarity, x, y) part of conv_block1.conv_block1, which runs on [polarity, 16 image samples, x, y]
             # (net.py:117-126); the image channels follow in dagr_l1_conv_a_image
             self._run("l1_build", lib.dagr_l1_build, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), _lib.ptr(geom.d_tab1), C.byref(pk["l1a_img"]), _lib.ptr(flags), 0, _lib.ptr(nbr), _lib.ptr(off),
+                      _lib.ptr(ws["feat_s"]), _lib.ptr(geom.d_tab1), C.byref(pk["l1a_img"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr), _lib.ptr(off),
                       _lib.ptr(cellmask), _lib.ptr(ws["xa"]), _lib.ptr(wl_hdr), _lib.ptr(self._zs(ws, "wl_build", torch.int32)), defer[0], st)
             if image_event is not None:                       # stage 1 of the image branch ran on a side stream next to sort + probe
                 torch.cuda.current_stream().wait_event(image_event[0])
@@ -590,12 +593,22 @@ class Engine:
                 self._run("l1_x0_image", lib.dagr_l1_x0_image_live, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
                           _lib.ptr(f0), int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
             else:
+                # incremental steps resample every node too: a new node's conv reads the x0 rows of its older neighbours
                 self._run("l1_x0_image", lib.dagr_l1_x0_image, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(f0),
                           int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
-            self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
-                      _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off),
-                      C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
-                      _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
+            if stream_state is not None:
+                # only the new nodes are convolved; the xa rows of the older ones are final and stay as gathered
+                self._run("l1_conv_a_image_inc", lib.dagr_l1_conv_a_image_inc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                          _lib.ptr(ws["ti"]), _lib.ptr(ws["feat_s"]), _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off), C.byref(pk["l1img"]),
+                          _lib.ptr(pk["l1img_wfrag"]), min_idx, _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
+                          _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
+                self._run("xa_scatter", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
+                          _lib.ptr(stream_state.xa_arr), 1, st)
+            else:
+                self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
+                          _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off),
+                          C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
+                          _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
         elif self.fused_build or stream_state is not None:
             if min_idx > 0:
                 self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
@@ -627,7 +640,12 @@ class Engine:
                       _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy), _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1,
                       _lib.ptr(wl_hdr[4:]), _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
             self._dense_report(ws, wl_hdr)
-            if use_image:                                     # sampling_skip before pool1 (net.py:128-131)
+            if use_image and stream_state is not None:        # running per-voxel max of the samples, new events only
+                f1 = image_feats[1]
+                self._run("voxel_sample_max_inc", lib.dagr_voxel_sample_max_inc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                          _lib.ptr(ws["ti"]), _lib.ptr(f1), int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), min_idx,
+                          _lib.ptr(stream_state.imgmax), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
+            elif use_image:                                   # sampling_skip before pool1 (net.py:128-131)
                 f1 = image_feats[1]
                 self._run("voxel_sample_max", lib.dagr_voxel_sample_max, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
                           int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)

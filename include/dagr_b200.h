@@ -316,6 +316,27 @@ int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const int32_t *star
                             const float *x0, const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host,
                             const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
 
+/* ---- incremental stream steps with image fusion (a13 with use_image) ----
+ * dagr_l1_conv_a_image_inc: dagr_l1_conv_a_image_tc for an append-only stream step.  Only nodes whose arrival index
+ * ti[p].y (int32[N][2] from the sort) is >= min_idx are convolved: their xa rows (the probe's event-channel sums, as
+ * dagr_l1_build with the same min_idx left them) are finished and their skipv rows written.  The xa rows of older nodes hold
+ * the final activations gathered from arrival storage (dagr_xa_permute) and are left untouched, skipv rows of older nodes
+ * are not written.  x0 must hold the samples of EVERY node (a new node's conv reads its older neighbours' x0).  min_idx = 0
+ * gives the bits of dagr_l1_conv_a_image_tc.
+ * dagr_voxel_sample_max_inc: dagr_voxel_sample_max (max only) with a running per-voxel max persist f32[cells][C] across
+ * steps.  min_idx = 0 samples every event, seeds persist (-inf for empty voxels) and gives the bits of dagr_voxel_sample_max;
+ * min_idx > 0 samples only the events with arrival index >= min_idx and combines their max with persist; a voxel without
+ * such events copies persist to xg and stages nothing.
+ * Both return DAGR_E_ARG with a message before launching anything on a null pointer (wl_hdr / wl_ids may be NULL), a
+ * negative min_idx, N outside [0, 2^31), c0 + C > ldx or pool_mean != 0 (the stream's running aggregate is a max). */
+int dagr_l1_conv_a_image_inc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                             const float *feat_s, const float *x0, const int32_t *nbr, const uint16_t *off,
+                             const dagr_l1img_params_t *p_host, const float *wfrag, int min_idx, float *xa, float *skipv,
+                             int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
+int dagr_voxel_sample_max_inc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                              const float *img /*[B,C,h,w]*/, int C, int h, int w, int min_idx, float *persist, float *xg, int ldx,
+                              int c0, int pool_mean, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Coarse levels live on dense voxel grids [B, ny, nx]: per cell  valid, pixel position, features,
  * and an 8-neighbour in-edge mask (bit (dcy+1)*3+(dcx+1), src cell = dst cell + (dcx,dcy)).
