@@ -90,8 +90,11 @@ _SIGS = {
     "dagr_xa_permute": (C.c_int, [i64, p, C.c_int, p, p, C.c_int, p]),
     "dagr_l1_x0_image": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, p, p]),
     "dagr_l1_x0_image_live": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, p, p]),
+    "dagr_l1_x0_image_planes": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, p, p]),
     "dagr_l1_conv_a_image": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1ImgParams), p, p, p, p, C.c_int, p]),
     "dagr_voxel_sample_max": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, C.c_int, C.c_int, p]),
+    "dagr_voxel_sample_max_planes": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p, C.c_int,
+                                               C.c_int, C.c_int, p]),
     "dagr_graph_export": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, p, i64, p]),
     "dagr_l1_conv_a": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, C.POINTER(L1AParams), p, p]),
     "dagr_l1_conv_b_pool": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1BParams), p, p, p]),
@@ -114,9 +117,13 @@ _SIGS = {
     "dagr_grid_to_dense": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, C.c_int, p, p, p]),
     "dagr_head_decode": (C.c_int, [p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p]),
     "dagr_head_finish": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, p, C.c_int, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p]),
+    "dagr_head_finish_planes": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, p, C.c_int, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.c_int, p, C.c_int, p, p]),
     "dagr_postprocess_nms": (C.c_int, [p, C.c_int, C.c_int, C.c_int, f32, f32, C.c_int, C.c_int, C.c_int, p, p, p]),
     "dagr_sample_features": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p,
                                        C.c_int, C.c_int, p]),
+    "dagr_sample_features_planes": (C.c_int, [p, C.c_int, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p,
+                                              C.c_int, C.c_int, p]),
     "dagr_masked_lin": (C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p]),
     "dagr_masked_inplace_bn": (C.c_int, [p, i64, p, p, p, p, p, p, C.c_int, f32, p]),
     "dagr_masked_isdiff": (C.c_int, [p, i64, p, p, C.c_int, f32, f32, p]),

@@ -676,24 +676,27 @@ extern "C" int dagr_head_decode(const float *reg, const float *obj, const float 
 //   reg/obj/cls = (valid ? conv output : 0) + CNN map;  xy = (reg_xy + grid) * stride, wh = exp(reg_wh) * stride,
 //   sigmoid(obj), sigmoid(cls)  -> out[b, a0 + cell, 5 + nc]
 // (the separate to_dense + head_decode launches, 8 per forward, remain for callers that want the dense maps)
+// PLANES: the CNN maps add_* are plane arrays [pl.n][C][ny][nx] and sample b reads plane img_plane(pl, b).
+template <bool PLANES>
 __global__ void k_head_finish(const dagr_grid_t gr, const int32_t *__restrict__ cnt, const float *__restrict__ cls, int ldc,
                               const float *__restrict__ regobj, int ldr, const float *__restrict__ add_cls,
                               const float *__restrict__ add_reg, const float *__restrict__ add_obj, int nc, float stride, int a0,
-                              int A, float *__restrict__ out)
+                              int A, float *__restrict__ out, const ImgPlanes pl)
 {
     const int per = gr.ny * gr.nx;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= gr.B * per) return;
     const int b = i / per, a = i % per, gy = a / gr.nx, gx = a % gr.nx;
+    const int bm = PLANES ? img_plane(pl, b) : b;                          // batch index of the CNN maps
     const bool valid = cnt[i] > 0;
     float r[5];
 #pragma unroll
     for (int c = 0; c < 5; c++) r[c] = valid ? regobj[(int64_t)i * ldr + c] : 0.f;
     if (add_reg) {
 #pragma unroll
-        for (int c = 0; c < 4; c++) r[c] += add_reg[((int64_t)b * 4 + c) * per + a];
+        for (int c = 0; c < 4; c++) r[c] += add_reg[((int64_t)bm * 4 + c) * per + a];
     }
-    if (add_obj) r[4] += add_obj[(int64_t)b * per + a];
+    if (add_obj) r[4] += add_obj[(int64_t)bm * per + a];
     float *o = out + ((int64_t)b * A + a0 + a) * (5 + nc);
     o[0] = (r[0] + (float)gx) * stride;
     o[1] = (r[1] + (float)gy) * stride;
@@ -702,7 +705,7 @@ __global__ void k_head_finish(const dagr_grid_t gr, const int32_t *__restrict__ 
     o[4] = 1.f / (1.f + expf(-r[4]));
     for (int c = 0; c < nc; c++) {
         float v = valid ? cls[(int64_t)i * ldc + c] : 0.f;
-        if (add_cls) v += add_cls[((int64_t)b * nc + c) * per + a];
+        if (add_cls) v += add_cls[((int64_t)bm * nc + c) * per + a];
         o[5 + c] = 1.f / (1.f + expf(-v));
     }
 }
@@ -713,8 +716,24 @@ extern "C" int dagr_head_finish(const dagr_grid_t *gr, const int32_t *cnt, const
 {
     DAGR_CHECK_ARG(gr && cls && regobj && ldc >= nc && ldr >= 5, "bad argument");
     const int n = gr->B * gr->ny * gr->nx;
-    k_head_finish<<<dagr_div_up(n, 128), 128, 0, (cudaStream_t)stream>>>(*gr, cnt, cls, ldc, regobj, ldr, add_cls, add_reg, add_obj, nc,
-                                                                       (float)stride, a0, A, out);
+    k_head_finish<false><<<dagr_div_up(n, 128), 128, 0, (cudaStream_t)stream>>>(*gr, cnt, cls, ldc, regobj, ldr, add_cls, add_reg, add_obj,
+                                                                              nc, (float)stride, a0, A, out, ImgPlanes{});
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_head_finish_planes(const dagr_grid_t *gr, const int32_t *cnt, const float *cls, int ldc, const float *regobj,
+                                       int ldr, const float *add_cls, const float *add_reg, const float *add_obj, int nc, int stride,
+                                       int a0, int A, int nplanes, const int32_t *plane, int plane_stride, float *out, void *stream)
+{
+    DAGR_CHECK_ARG(gr && cnt && cls && regobj && add_cls && add_reg && add_obj && plane && out, "null argument");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(ldc >= nc && ldr >= 5, "row strides ldc >= nc and ldr >= 5");
+    const int n = gr->B * gr->ny * gr->nx;
+    k_head_finish<true><<<dagr_div_up(n, 128), 128, 0, (cudaStream_t)stream>>>(*gr, cnt, cls, ldc, regobj, ldr, add_cls, add_reg, add_obj,
+                                                                             nc, (float)stride, a0, A, out,
+                                                                             ImgPlanes{plane, plane_stride, nplanes});
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }
@@ -829,20 +848,24 @@ extern "C" int dagr_postprocess_nms(const float *pred, int B, int A, int nc, flo
 
 // ------------------------------------------------------------------------------------------------
 // a8 sample_features: 3-D bilinear grid_sample, align_corners=True, zero padding (net.py:193-221)
+// PLANES: img_in is a plane array [pl.n][C][h][w]; node i samples plane img_plane(pl, bidx[i]) as a batch of one.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_sample_features(const float *__restrict__ img, int Bi, int C, int h, int w,
+template <bool PLANES>
+__global__ void k_sample_features(const float *__restrict__ img_in, int Bi_in, int C, int h, int w,
                                   const float *__restrict__ posx, const float *__restrict__ posy,
                                   const int32_t *__restrict__ bidx, int64_t n, float width, float height,
-                                  float *__restrict__ out, int ldo, int c0)
+                                  float *__restrict__ out, int ldo, int c0, const ImgPlanes pl)
 {
     const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (i >= n) return;
+    const int Bi = PLANES ? 1 : Bi_in;
+    const float *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, bidx[i]) * C * h * w : img_in;
     // normalise exactly as _sample_features does, then unnormalise as grid_sample(align_corners=True)
     float gx = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posx[i], width)), width - 1.f), 1.f);
     float gy = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posy[i], height)), height - 1.f), 1.f);
     const float bs = (float)(Bi > 1 ? Bi : 2);
-    float gz = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, (float)bidx[i]), bs - 1.f), 1.f);
+    float gz = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, PLANES ? 0.f : (float)bidx[i]), bs - 1.f), 1.f);
     const float ix = __fmul_rn(__fmul_rn(__fadd_rn(gx, 1.f), 0.5f), (float)(w - 1));
     const float iy = __fmul_rn(__fmul_rn(__fadd_rn(gy, 1.f), 0.5f), (float)(h - 1));
     const float iz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.f), 0.5f), (float)(Bi - 1));
@@ -879,8 +902,24 @@ extern "C" int dagr_sample_features(const float *img, int Bi, int C, int h, int 
                                     void *stream)
 {
     if (n <= 0) return DAGR_OK;
-    k_sample_features<<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, Bi, C, h, w, posx, posy, bidx, n,
-                                                                         (float)width, (float)height, out, ldo, c0);
+    k_sample_features<false><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, Bi, C, h, w, posx, posy, bidx, n,
+                                                                                (float)width, (float)height, out, ldo, c0, ImgPlanes{});
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_sample_features_planes(const float *img, int nplanes, const int32_t *plane, int plane_stride, int C, int h, int w,
+                                           const float *posx, const float *posy, const int32_t *bidx, int64_t n, int width, int height,
+                                           float *out, int ldo, int c0, void *stream)
+{
+    DAGR_CHECK_ARG(img && posx && posy && bidx && out && plane, "null argument");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
+    if (n == 0) return DAGR_OK;
+    k_sample_features<true><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, 1, C, h, w, posx, posy, bidx, n, (float)width,
+                                                                               (float)height, out, ldo, c0,
+                                                                               ImgPlanes{plane, plane_stride, nplanes});
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

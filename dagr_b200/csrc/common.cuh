@@ -37,6 +37,19 @@ template <class K> static inline cudaError_t dagr_allow_smem(K kernel, size_t by
 
 static inline int dagr_div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// Plane mode of the image kernels (several hybrid cameras as the samples of one step): the image is a plane array
+// [n][C][h][w] and sample b reads plane plane[b * stride] alone, sampled as a batch of one (b = 0, Bi = 1: the depth
+// coordinate is exactly 0), i.e. with the bits of that sample in a B = 1 forward.  The plane table is device data that the
+// launch cannot check, so a value outside [0, n) is clamped (it selects a wrong plane, never memory outside the array).
+struct ImgPlanes {
+    const int32_t *plane;
+    int stride, n;
+};
+__device__ __forceinline__ int img_plane(const ImgPlanes &pl, int b)
+{
+    return min(max(__ldg(pl.plane + (int64_t)b * pl.stride), 0), pl.n - 1);
+}
+
 // exclusive prefix sum of n ints (graph.cu); blocksums: int[dagr_scan_blocks(n) + 2]; the grand total is left in
 // blocksums[dagr_scan_blocks(n)]
 int scan_exclusive(const int *in, int *out, int64_t n, int *blocksums, cudaStream_t st);

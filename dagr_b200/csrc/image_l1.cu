@@ -56,8 +56,10 @@ __device__ __forceinline__ float bilin_sample(const float *__restrict__ img, int
 // capacity and the sorted positions at or beyond the live total hold stale or never-written xyb words, whose x / y would index
 // past posx0 / posy0; the rows they would fill are never read (conv_a_image, conv_b and voxel_sample_max walk the voxels'
 // [start[cell], start[cell+1]) ranges, which lie below the total), so they are simply skipped.  live == NULL: the bound is N.
+// PLANES: img0 is a plane array [pl.n][16][h][w] and the event of sample b samples plane img_plane(pl, b) as a batch of one.
+template <bool PLANES>
 __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ live, const uint32_t *__restrict__ xyb,
-                              const float *__restrict__ img0, int h, int w, float *__restrict__ x0)
+                              const float *__restrict__ img0, int h, int w, float *__restrict__ x0, const ImgPlanes pl)
 {
     // 4 threads per node: thread q computes image channels 4q..4q+3 = one 16-byte chunk of a row
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -67,10 +69,12 @@ __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__r
     const uint32_t wd = xyb[p];
     const int x = wd & 0xfff, y = (wd >> 12) & 0xfff, b = wd >> 24;
     const float px = g.posx0[x], py = g.posy0[y];
-    const Bilin bl = bilin_setup(px, py, b, (float)g.W, (float)g.H, g.B, h, w);
+    const int Bi = PLANES ? 1 : g.B;
+    const float *img = PLANES ? img0 + (int64_t)img_plane(pl, b) * 16 * h * w : img0;
+    const Bilin bl = bilin_setup(px, py, PLANES ? 0 : b, (float)g.W, (float)g.H, Bi, h, w);
     float f[4];
 #pragma unroll
-    for (int k = 0; k < 4; k++) f[k] = bilin_sample(img0, g.B, 16, h, w, 4 * q + k, bl);
+    for (int k = 0; k < 4; k++) f[k] = bilin_sample(img, Bi, 16, h, w, 4 * q + k, bl);
     float4 *dst = reinterpret_cast<float4 *>(x0 + ((int64_t)(q >> 1) * N + p) * 8);
     dst[(q & 1) ^ XA_SWZ(p)] = make_float4(f[0], f[1], f[2], f[3]);
 }
@@ -80,7 +84,7 @@ extern "C" int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t 
 {
     (void)feat_s;
     if (N <= 0) return DAGR_OK;
-    k_l1_x0_image<<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, nullptr, xyb, img0, h, w, x0);
+    k_l1_x0_image<false><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, nullptr, xyb, img0, h, w, x0, ImgPlanes{});
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }
@@ -92,7 +96,23 @@ extern "C" int dagr_l1_x0_image_live(const dagr_geom_t *g, int64_t N, const int3
     DAGR_CHECK_ARG(g && start && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
     if (N == 0) return DAGR_OK;
-    k_l1_x0_image<<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0);
+    k_l1_x0_image<false><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0, ImgPlanes{});
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                                       const float *img0, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *x0,
+                                       void *stream)
+{
+    (void)feat_s;
+    DAGR_CHECK_ARG(g && start && xyb && img0 && plane && x0, "null argument (only feat_s may be NULL)");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    if (N == 0) return DAGR_OK;
+    k_l1_x0_image<true><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0,
+                                                                                 ImgPlanes{plane, plane_stride, nplanes});
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }
@@ -143,11 +163,13 @@ template <bool MEAN> __device__ __forceinline__ float vs_comb(float a, float b) 
 // (the reference's async pool1 keeps a running max of the concatenated x, max_pool.py:59-62).  min_idx > 0: only events with
 // arrival index ti[p].y >= min_idx are sampled and their max is combined with persist; a voxel without such events copies
 // persist and stages nothing.  min_idx == 0 samples every event (the bits of the plain instance) and seeds persist.
-template <bool MEAN, bool INC>
+// PLANES: img is a plane array [pl.n][C][h][w]; a voxel of sample b samples plane img_plane(pl, b) as a batch of one, so its
+// window is staged from that one plane (pz = 1).
+template <bool MEAN, bool INC, bool PLANES = false>
 __global__ void __launch_bounds__(VS_THREADS)
 k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
-                   const int2 *__restrict__ ti, const float *__restrict__ img, int C, int h, int w, const int min_idx,
-                   float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0)
+                   const int2 *__restrict__ ti, const float *__restrict__ img_in, int C, int h, int w, const int min_idx,
+                   float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0, const ImgPlanes pl = ImgPlanes{})
 {
     __shared__ float s_m[VS_THREADS / 32][128];
     __shared__ __align__(16) float s_patch[VS_SMEM_FLOATS];
@@ -182,12 +204,15 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
         }
         xg[(int64_t)cell * ldx + c0 + c] = v;
     };
+    // the sampled batch: sample b of the g.B planes of img, or (PLANES) the one plane of sample b as a batch of one (its depth
+    // coordinate and batch size are spelled out at each use below: a local copy of g.B changes the plain instances' allocation)
+    const float *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, b) * C * h * w : img_in;
     // window of the map this voxel's pixels can touch: the sample coordinates are monotone in x / y, so the corner
     // pixels bound it (same arithmetic as the per-event set-up)
-    const Bilin lo = bilin_setup(g.posx0[g.vx0[cx]], g.posy0[g.vy0[cy]], b, (float)g.W, (float)g.H, g.B, h, w);
-    const Bilin hi = bilin_setup(g.posx0[g.vx0[cx + 1] - 1], g.posy0[g.vy0[cy + 1] - 1], b, (float)g.W, (float)g.H, g.B, h, w);
+    const Bilin lo = bilin_setup(g.posx0[g.vx0[cx]], g.posy0[g.vy0[cy]], PLANES ? 0 : b, (float)g.W, (float)g.H, PLANES ? 1 : g.B, h, w);
+    const Bilin hi = bilin_setup(g.posx0[g.vx0[cx + 1] - 1], g.posy0[g.vy0[cy + 1] - 1], PLANES ? 0 : b, (float)g.W, (float)g.H, PLANES ? 1 : g.B, h, w);
     const int xb = max(lo.x0, 0), yb = max(lo.y0, 0), zb = max(lo.z0, 0);
-    const int xe = min(hi.x0 + 1, w - 1), ye = min(hi.y0 + 1, h - 1), ze = min(lo.z0 + 1, g.B - 1);
+    const int xe = min(hi.x0 + 1, w - 1), ye = min(hi.y0 + 1, h - 1), ze = min(lo.z0 + 1, (PLANES ? 1 : g.B) - 1);
     const int pw = xe - xb + 1, ph = ye - yb + 1, pz = ze - zb + 1;
     const bool staged = pw > 0 && ph > 0 && pz > 0 && (int64_t)pz * ph * pw * C <= VS_SMEM_FLOATS;   // block-uniform
     if (staged) {
@@ -211,7 +236,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
             if (p < p1 && take(p)) {
                 const uint32_t wd = xyb[p];
                 const int x = wd & 0xfff, y = (wd >> 12) & 0xfff;
-                const Bilin q = bilin_setup(g.posx0[x], g.posy0[y], b, (float)g.W, (float)g.H, g.B, h, w);
+                const Bilin q = bilin_setup(g.posx0[x], g.posy0[y], PLANES ? 0 : b, (float)g.W, (float)g.H, PLANES ? 1 : g.B, h, w);
                 float acc[8];
 #pragma unroll
                 for (int k = 0; k < 8; k++) acc[k] = 0.f;
@@ -219,7 +244,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
                 for (int dz = 0; dz < 2; dz++) {
                     const int z = q.z0 + dz;
                     const float wz = dz ? q.tz : 1.f - q.tz;
-                    if (z < 0 || z >= g.B) continue;
+                    if (z < 0 || z >= (PLANES ? 1 : g.B)) continue;
 #pragma unroll
                     for (int dy = 0; dy < 2; dy++) {
                         const int yy = q.y0 + dy;
@@ -266,13 +291,13 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
             if (!take(p)) continue;
             const uint32_t wd = xyb[p];
             const int x = wd & 0xfff, y = (wd >> 12) & 0xfff;
-            const Bilin bl = bilin_setup(g.posx0[x], g.posy0[y], b, (float)g.W, (float)g.H, g.B, h, w);
+            const Bilin bl = bilin_setup(g.posx0[x], g.posy0[y], PLANES ? 0 : b, (float)g.W, (float)g.H, PLANES ? 1 : g.B, h, w);
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int c = cb + lane + 32 * k;
                 if (c < C)
-                    m[k] = vs_comb<MEAN>(m[k], staged ? vs_sample<true>(img, s_patch, g.B, C, h, w, c, bl, zb, yb, xb, ph, pw)
-                                                      : vs_sample<false>(img, s_patch, g.B, C, h, w, c, bl, zb, yb, xb, ph, pw));
+                    m[k] = vs_comb<MEAN>(m[k], staged ? vs_sample<true>(img, s_patch, PLANES ? 1 : g.B, C, h, w, c, bl, zb, yb, xb, ph, pw)
+                                                      : vs_sample<false>(img, s_patch, PLANES ? 1 : g.B, C, h, w, c, bl, zb, yb, xb, ph, pw));
             }
         }
 #pragma unroll
@@ -313,6 +338,25 @@ extern "C" int dagr_voxel_sample_max_inc(const dagr_geom_t *g, int64_t N, const 
     const int cells = g->B * g->ny1 * g->nx1;
     k_voxel_sample_max<false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, (const int2 *)ti, img, C, h, w, min_idx,
                                                                                    persist, xg, ldx, c0);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_voxel_sample_max_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *img,
+                                            int C, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *xg, int ldx,
+                                            int c0, int pool_mean, void *stream)
+{
+    DAGR_CHECK_ARG(g && start && xyb && img && plane && xg, "null argument");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
+    const int cells = g->B * g->ny1 * g->nx1;
+    const ImgPlanes pl{plane, plane_stride, nplanes};
+    if (pool_mean) k_voxel_sample_max<true, false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w,
+                                                                                                      0, nullptr, xg, ldx, c0, pl);
+    else           k_voxel_sample_max<false, false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h,
+                                                                                                       w, 0, nullptr, xg, ldx, c0, pl);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

@@ -147,6 +147,7 @@ class Engine:
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
     _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_l1_conv_a_image_inc=2, dagr_voxel_sample_max_inc=1,
+                     dagr_l1_x0_image_planes=1, dagr_voxel_sample_max_planes=1, dagr_sample_features_planes=1, dagr_head_finish_planes=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
                      dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
                      dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1)
@@ -487,8 +488,9 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def _append_image(self, geom, lv, gs, o, feat, ws, st, dev):
-        """sampling_skip on a voxel grid (net.py:141-142 etc.): [o | bilinear samples of `feat` at the nodes]."""
+    def _append_image(self, geom, lv, gs, o, feat, ws, st, dev, planes=None):
+        """sampling_skip on a voxel grid (net.py:141-142 etc.): [o | bilinear samples of `feat` at the nodes].
+        planes = (plane table, stride): `feat` is a plane array and sample b samples its plane alone (forward_events)."""
         cells, Cc, Cf = gs.cells, o.shape[1], int(feat.shape[1])
         xcat = self._buf(ws, f"xcat{lv}", (cells, Cc + Cf), torch.float32, dev)
         xcat[:, :Cc] = o
@@ -499,6 +501,11 @@ class Engine:
         if key not in ws:
             per = geom.levels[lv].nx * geom.levels[lv].ny
             ws[key] = (torch.arange(cells, device=dev) // per).int()
+        if planes is not None:
+            self._run("sample_features", self.lib.dagr_sample_features_planes, _lib.ptr(feat), int(feat.shape[0]), _lib.ptr(planes[0]),
+                      int(planes[1]), Cf, int(feat.shape[2]), int(feat.shape[3]), _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells,
+                      geom.W, geom.H, _lib.ptr(xcat), Cc + Cf, Cc, st)
+            return xcat
         self._run("sample_features", self.lib.dagr_sample_features, _lib.ptr(feat), int(feat.shape[0]), Cf, int(feat.shape[2]),
                   int(feat.shape[3]), _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells, geom.W, geom.H, _lib.ptr(xcat),
                   Cc + Cf, Cc, st)
@@ -507,14 +514,18 @@ class Engine:
     @torch.no_grad()
     def forward_events(self, batch_i32: torch.Tensor, pos_i32: torch.Tensor, feat: torch.Tensor, B: int,
                        W: int, H: int, image_feats=None, image_outs=None, stream_state=None, n_old: int = 0, ring=None,
-                       image_event=None, ring_streams=None):
+                       image_event=None, ring_streams=None, image_planes=None):
         """batch int32[N], pos int32[N,3], feat fp32[N] (polarity) on CUDA -> decoded [B, A, 5+nc].
 
         ring = device control block (int32[8], dagr_graph_sort_ring): the three inputs are ring buffers of N = capacity
         slots whose live window {head, count} is only known on the device; every launch then covers the capacity, nothing
         depends on a host-side count and the whole call can sit inside one captured CUDA graph (dagr_b200.streaming).
         ring_streams = S: `ring` is the int32[S+1][8] block of S rings of N / S slots each (dagr_graph_sort_rings), stream s
-        being sample s of B = S."""
+        being sample s of B = S.
+        image_planes = (plane table int32 on the device, stride), with ring_streams and image fusion: image_feats / image_outs
+        are plane arrays [P, C, h, w] and sample b reads plane table[b * stride] alone, sampled as a batch of one (the
+        *_planes kernels), so each stream gets the bits of a B = 1 forward with its own frame.  The table may be device
+        data written inside the step (the stage header, dagr_b200.streaming.FusionMultiStreamDetector)."""
         for n, t in (("batch", batch_i32), ("pos", pos_i32), ("x", feat)):
             _lib.require_cuda(t, n)
         dev = pos_i32.device
@@ -522,6 +533,13 @@ class Engine:
         if ring_streams is not None and (ring is None or int(ring_streams) != int(B) or N % int(ring_streams)):
             raise ValueError(f"ring_streams={ring_streams} needs a ring control block, B == ring_streams and N a multiple of it "
                              f"(B={B}, N={N})")
+        if image_planes is not None:
+            if ring_streams is None or image_feats is None or image_outs is None:
+                raise ValueError("image_planes selects per-stream frames of a multi-ring step: it needs ring_streams, image_feats "
+                                 "and image_outs")
+            if self.keep_node_features:
+                raise ValueError("keep_node_features: the dense head maps (dagr_grid_to_dense) have no plane mode")
+            plane_tab, plane_stride = image_planes
         geom = self.geometry(W, H, B, dev)
         pk = self.pack(geom, dev)
         ws = self.workspace(geom, N, dev)
@@ -587,7 +605,11 @@ class Engine:
             f0 = image_feats[0]
             x0 = self._buf(ws, "x0img", (2 * max(N, 1) * 8,), torch.float32, dev)
             skipv = self._buf(ws, "skipv", (max(N, 1), 16), torch.float32, dev)
-            if ring is not None:
+            if image_planes is not None:
+                self._run("l1_x0_image", lib.dagr_l1_x0_image_planes, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
+                          _lib.ptr(f0), int(f0.shape[2]), int(f0.shape[3]), int(f0.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
+                          _lib.ptr(x0), st)
+            elif ring is not None:
                 # N = ring capacity: positions behind the live total hold stale xyb words, so the launch is bounded by the
                 # total the sort wrote (start[NK]); the synchronous path keeps the unbounded form (N is the live count there)
                 self._run("l1_x0_image", lib.dagr_l1_x0_image_live, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
@@ -645,6 +667,11 @@ class Engine:
                 self._run("voxel_sample_max_inc", lib.dagr_voxel_sample_max_inc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
                           _lib.ptr(ws["ti"]), _lib.ptr(f1), int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), min_idx,
                           _lib.ptr(stream_state.imgmax), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
+            elif image_planes is not None:
+                f1 = image_feats[1]
+                self._run("voxel_sample_max", lib.dagr_voxel_sample_max_planes, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
+                          int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), int(f1.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
+                          _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
             elif use_image:                                   # sampling_skip before pool1 (net.py:128-131)
                 f1 = image_feats[1]
                 self._run("voxel_sample_max", lib.dagr_voxel_sample_max, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
@@ -671,7 +698,7 @@ class Engine:
             lay = pk["layers"]
             inter = {}
             def cat_img(lv, gs, o, k):
-                return self._append_image(geom, lv, gs, o, image_feats[k], ws, st, dev) if use_image else o
+                return self._append_image(geom, lv, gs, o, image_feats[k], ws, st, dev, image_planes) if use_image else o
 
             _, _, o2 = self._layer(geom, 0, g1, lay[0], ws, "layer2", st, dev)
             if use_image and image_event is not None:         # layer2..4 taps + CNN head maps (stage 2 of the image branch)
@@ -705,6 +732,12 @@ class Engine:
                 for name in ("cls", "reg", "obj"):
                     adds[name] = image_outs[name + "_output"][k].float().contiguous() if image_outs is not None else None
                 stride = model.backbone.strides[k]
+                if image_planes is not None:
+                    self._run("head_finish", lib.dagr_head_finish_planes, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(ocls), nc,
+                              _lib.ptr(oro), 5, _lib.ptr(adds["cls"]), _lib.ptr(adds["reg"]), _lib.ptr(adds["obj"]), nc, int(stride), a0, A,
+                              int(adds["cls"].shape[0]), _lib.ptr(plane_tab), int(plane_stride), _lib.ptr(out), st)
+                    dense_all[k] = {}
+                    return
                 self._run("head_finish", lib.dagr_head_finish, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(ocls), nc, _lib.ptr(oro), 5,
                           _lib.ptr(adds["cls"]), _lib.ptr(adds["reg"]), _lib.ptr(adds["obj"]), nc, int(stride), a0, A, _lib.ptr(out), st)
                 dense = {}

@@ -21,6 +21,8 @@ works on a batch.  The step is still one CUDA graph replay.
 
 FusionStreamingDetector streams the hybrid (image + events) model: a camera frame runs through the image trunk once, into one
 of two frame slots, and every chunk's step (one replay of that slot's graph) reads the newest frame whose trunk has finished.
+FusionMultiStreamDetector does the same for S hybrid cameras in one step: the frame slots of all cameras are planes of one
+array, and each camera's plane travels in its stage header, so one graph serves every combination of slots.
 
 Why the event level is recomputed over the window instead of patched: evicting an event changes the neighbour lists of
 every node it fed (the K cap admits the next candidate of the spiral), i.e. of the window's oldest 10 ms -- and their
@@ -96,6 +98,10 @@ class _RingDetector:
         """(image_feats, image_outs) of the next step: None for the events-only model."""
         return None, None
 
+    def _image_planes(self):
+        """(plane table, stride) when image_feats / image_outs are per-stream plane arrays (forward_events), else None."""
+        return None
+
     def _push(self):
         raise NotImplementedError
 
@@ -107,7 +113,7 @@ class _RingDetector:
         eng.launches += 2
         feats, outs = self._image_inputs()
         dec = eng.forward_events(self.batch, self.pos, self.feat, self._B, self.W, self.H, image_feats=feats, image_outs=outs,
-                                 ring=self.ctl, ring_streams=self._ring_streams)
+                                 ring=self.ctl, ring_streams=self._ring_streams, image_planes=self._image_planes())
         det, ndet = eng.postprocess(dec, m.conf_threshold, m.nms_threshold, self.W, self.H)
         if self._res_h is None:
             self._res_h = (torch.empty(det.shape, dtype=det.dtype).pin_memory(), torch.empty(ndet.shape, dtype=ndet.dtype).pin_memory(),
@@ -226,89 +232,80 @@ class StreamingDetector(_RingDetector):
         return self._live(0)
 
 
-class FusionStreamingDetector(StreamingDetector):
-    """Streaming detection with the hybrid (image + events) model: camera frames at frame rate, event chunks in between.
+def _check_fusion_model(model, name: str, events_only_class: str):
+    if not model.backbone.use_image:
+        raise ValueError(f"{name} drives an image-fusion model (backbone.use_image); "
+                         f"stream an events-only model with {events_only_class}")
+    if model.head.no_events:
+        raise NotImplementedError("--no_events: the model has no event path to stream")
 
-        det = FusionStreamingDetector(model, window_us=50_000)
-        fid = det.set_frame(image_u8)          # u8 [3,H,W] or [1,3,H,W], host or device -> frame id 0, 1, 2, ...
-        det.push(x, y, t, p)                   # as StreamingDetector: one CUDA graph replay per chunk
 
-    A frame runs through the model's own ImageBranch (ResNet trunk + CNN head, the captured graphs that model(data)
-    replays) once, on the branch's side stream, and its five feature maps and CNN head maps are copied into one of two frame
-    slots owned by the detector.  Each slot has its own captured step graph, so a step is still one replay.
+class _CameraFrames:
+    """The frames of one hybrid camera, for the fusion detectors: two frame slots, the frame pending in the trunk, the frame
+    in use, and the done-event of the last step that read each slot.
 
-    Which frame a step uses: the newest frame whose trunk has finished when the chunk is submitted (a non-blocking event
-    query).  Chunks keep flowing on the previous frame while the next frame's trunk runs; sync_frame() blocks until the
-    pending frame is usable, so the next step uses it.  The first step waits for the first frame.  After every step the
-    detections equal model(data) over the live window with the image of the frame that frame_state reports.
+    set() runs a frame through the model's own ImageBranch (ResNet trunk + CNN head, the captured graphs that model(data)
+    replays) on the detector's frame stream and copies its five feature maps and CNN head maps into the slot the steps do
+    not use; `slot_dst(slot, feats, outs)` names the destination tensors of a slot (allocating them on first use).  Two
+    hazards are ordered on the device: the copy into a slot waits for the last step that read that slot, and the branch's
+    static output buffers are overwritten (by the next frame or a model(data) call) only after the copy out of them."""
 
-    Two hazards are ordered on the device: a slot is overwritten only after the last step that read it (the copy waits for
-    that step), and the branch's static output buffers are overwritten (by the next frame or a model(data) call) only after
-    the copy out of them (the branch stream waits for the copy)."""
+    def __init__(self, det, slot_dst):
+        self.det, self.slot_dst = det, slot_dst
+        self.reader = [None, None]            # per slot: done-event of the last step that read it
+        self.cur = None                       # slot of the newest usable frame
+        self.cur_frame = None                 # (id, t_us) of that frame
+        self.pending = None                   # frame whose trunk may still run: dict(slot, id, t_us, ready, trunk)
+        self.step_frame = (None, None)        # (id, t_us) of the frame the last submitted step used
+        self.nframes = 0
+        self.img_h = self.h2d = None
 
-    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
-        if not model.backbone.use_image:
-            raise ValueError("FusionStreamingDetector drives an image-fusion model (backbone.use_image); "
-                             "stream an events-only model with StreamingDetector")
-        if model.head.no_events:
-            raise NotImplementedError("--no_events: the model has no event path to stream")
-        self._setup(model, 1, window_us, max_chunk, capacity, device)
-        self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
-        self.frame_stream = torch.cuda.Stream(device=self.dev)
-        self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
-        self._reader = [None, None]           # per slot: done-event of the last step that read it
-        self._cur = None                      # slot of the newest usable frame
-        self._cur_frame = None                # (id, t_us) of that frame
-        self._pending = None                  # frame whose trunk may still run: dict(slot, id, t_us, ready, trunk)
-        self._step_frame = (None, None)       # (id, t_us) of the frame the last submitted step used
-        self._overlapped = False              # the last submitted step ran while a newer frame's trunk was in flight
-        self._nframes = 0
-        self._img_h = self._h2d = None
-
-    # ------------------------------------------------------------------------------------------------------------
-    def _check_frame(self, image):
+    def check(self, image):
+        d = self.det
         if not isinstance(image, torch.Tensor):
             image = torch.from_numpy(np.ascontiguousarray(image))
         if image.dtype != torch.uint8:
             raise ValueError(f"frame dtype {image.dtype}: expected uint8 (raw camera pixels)")
         if image.dim() == 4 and image.shape[0] == 1:
             image = image[0]
-        if image.dim() != 3 or tuple(image.shape) != (3, self.H, self.W):
-            raise ValueError(f"frame of shape {tuple(image.shape)}: expected [3, {self.H}, {self.W}] or [1, 3, {self.H}, {self.W}]")
+        if image.dim() != 3 or tuple(image.shape) != (3, d.H, d.W):
+            raise ValueError(f"frame of shape {tuple(image.shape)}: expected [3, {d.H}, {d.W}] or [1, 3, {d.H}, {d.W}]")
         return image.unsqueeze(0)
 
-    def _promote(self):
-        pend, self._pending = self._pending, None
-        self.stream.wait_event(pend["ready"])                         # no-op once it completed; orders the very first frame
-        self._cur, self._cur_frame = pend["slot"], (pend["id"], pend["t_us"])
+    def promote(self):
+        pend, self.pending = self.pending, None
+        self.det.stream.wait_event(pend["ready"])                     # no-op once it completed; orders the very first frame
+        self.cur, self.cur_frame = pend["slot"], (pend["id"], pend["t_us"])
 
-    @torch.no_grad()
-    def set_frame(self, image, t_us=None):
-        """start a new frame: the trunk runs on the device, this returns without waiting for it.  `image` u8 [3,H,W] or
-        [1,3,H,W] (host or device); `t_us` is the caller's timestamp of the frame, reported back by frame_state.
-        Returns the frame id (0, 1, 2, ...).  A frame still pending is waited for and becomes current first."""
+    def sync(self):
+        if self.pending is not None:
+            self.pending["ready"].synchronize()
+            self.promote()
+
+    def set(self, image, t_us):
         from .model.image_branch import ImageBranch
-        img = self._check_frame(image)
-        self.sync_frame()
-        slot = 0 if self._cur is None else 1 - self._cur
-        m, fs = self.model, self.frame_stream
+        det = self.det
+        img = self.check(image)
+        self.sync()
+        slot = 0 if self.cur is None else 1 - self.cur
+        m, fs = det.model, det.frame_stream
         if m._image_branch is None:
             m._image_branch = ImageBranch(m)
         br = m._image_branch
-        cur = torch.cuda.current_stream(self.dev)
+        cur = torch.cuda.current_stream(det.dev)
         if img.is_cuda:
-            x = img.to(self.dev).float() / 255.0                       # on the caller's stream, ordered with its writes
-        elif self._img_h is None:
-            self._img_h = torch.empty(img.shape, dtype=torch.uint8).pin_memory()
+            x = img.to(det.dev).float() / 255.0                        # on the caller's stream, ordered with its writes
+        elif self.img_h is None:
+            self.img_h = torch.empty(img.shape, dtype=torch.uint8).pin_memory()
         with torch.cuda.stream(fs):
             fs.wait_stream(cur)
             if not img.is_cuda:
-                if self._h2d is not None:
-                    self._h2d.synchronize()                            # the previous frame's upload has left the pinned stage
-                self._img_h.copy_(img)
-                x = self._img_h.to(self.dev, non_blocking=True).float() / 255.0   # as format_data
-                self._h2d = torch.cuda.Event()
-                self._h2d.record(fs)
+                if self.h2d is not None:
+                    self.h2d.synchronize()                             # the previous frame's upload has left the pinned stage
+                self.img_h.copy_(img)
+                x = self.img_h.to(det.dev, non_blocking=True).float() / 255.0    # as format_data
+                self.h2d = torch.cuda.Event()
+                self.h2d.record(fs)
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record(fs)
             feats, outs, (_, ev2) = br.run(x, use_graph=m.image_graph)
@@ -316,12 +313,9 @@ class FusionStreamingDetector(StreamingDetector):
             x.record_stream(br.stream)
             fs.wait_event(ev2)
             t1.record(fs)
-            if self._slots is None:
-                self._slots = [([torch.empty_like(f) for f in feats], {k: [torch.empty_like(t) for t in v] for k, v in outs.items()})
-                               for _ in range(2)]
-            if self._reader[slot] is not None:
-                fs.wait_event(self._reader[slot])                     # the last step that read this slot is done
-            dst_f, dst_o = self._slots[slot]
+            if self.reader[slot] is not None:
+                fs.wait_event(self.reader[slot])                      # the last step that read this slot is done
+            dst_f, dst_o = self.slot_dst(slot, feats, outs)
             for d, s in zip(dst_f, feats):
                 d.copy_(s)
             for k, v in outs.items():
@@ -330,34 +324,89 @@ class FusionStreamingDetector(StreamingDetector):
             ready = torch.cuda.Event()
             ready.record(fs)
         br.stream.wait_event(ready)                                   # the branch's static outputs outlive the copy
-        fid = self._nframes
-        self._nframes += 1
-        self._pending = dict(slot=slot, id=fid, t_us=t_us, ready=ready, trunk=(t0, t1))
+        fid = self.nframes
+        self.nframes += 1
+        self.pending = dict(slot=slot, id=fid, t_us=t_us, ready=ready, trunk=(t0, t1))
         return fid
+
+    def take_newest(self):
+        """before a step: the newest frame whose trunk has finished becomes current (a non-blocking query; the first frame is
+        taken whatever its state, the step waits for it on the device).  Returns whether a newer frame is still in flight."""
+        if self.pending is not None and (self.cur is None or self.pending["ready"].query()):
+            self.promote()
+        return self.pending is not None
+
+    def stepped(self, done):
+        """after a step was enqueued: it reads the current slot until `done`."""
+        self.reader[self.cur] = done
+        self.step_frame = self.cur_frame
+
+    def state(self):
+        fid, t_us = self.step_frame
+        return dict(frame=fid, t_us=t_us, pending=None if self.pending is None else self.pending["id"])
+
+
+class FusionStreamingDetector(StreamingDetector):
+    """Streaming detection with the hybrid (image + events) model: camera frames at frame rate, event chunks in between.
+
+        det = FusionStreamingDetector(model, window_us=50_000)
+        fid = det.set_frame(image_u8)          # u8 [3,H,W] or [1,3,H,W], host or device -> frame id 0, 1, 2, ...
+        det.push(x, y, t, p)                   # as StreamingDetector: one CUDA graph replay per chunk
+
+    A frame runs through the model's own ImageBranch (ResNet trunk + CNN head, the captured graphs that model(data)
+    replays) once, on a side stream, and its five feature maps and CNN head maps are copied into one of two frame slots
+    owned by the detector (_CameraFrames).  Each slot has its own captured step graph, so a step is still one replay.
+
+    Which frame a step uses: the newest frame whose trunk has finished when the chunk is submitted (a non-blocking event
+    query).  Chunks keep flowing on the previous frame while the next frame's trunk runs; sync_frame() blocks until the
+    pending frame is usable, so the next step uses it.  The first step waits for the first frame.  After every step the
+    detections equal model(data) over the live window with the image of the frame that frame_state reports."""
+
+    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+        _check_fusion_model(model, "FusionStreamingDetector", "StreamingDetector")
+        self._setup(model, 1, window_us, max_chunk, capacity, device)
+        self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
+        self.frame_stream = torch.cuda.Stream(device=self.dev)
+        self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
+        self._cam = _CameraFrames(self, self._slot_dst)
+        self._overlapped = False              # the last submitted step ran while a newer frame's trunk was in flight
+
+    def _slot_dst(self, slot, feats, outs):
+        if self._slots is None:
+            self._slots = [([torch.empty_like(f) for f in feats], {k: [torch.empty_like(t) for t in v] for k, v in outs.items()})
+                           for _ in range(2)]
+        return self._slots[slot]
+
+    @property
+    def _cur(self):
+        return self._cam.cur
+
+    # ------------------------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def set_frame(self, image, t_us=None):
+        """start a new frame: the trunk runs on the device, this returns without waiting for it.  `image` u8 [3,H,W] or
+        [1,3,H,W] (host or device); `t_us` is the caller's timestamp of the frame, reported back by frame_state.
+        Returns the frame id (0, 1, 2, ...).  A frame still pending is waited for and becomes current first."""
+        return self._cam.set(image, t_us)
 
     def sync_frame(self):
         """block until the pending frame (if any) is usable; the next step uses it."""
-        if self._pending is not None:
-            self._pending["ready"].synchronize()
-            self._promote()
+        self._cam.sync()
 
     def _graph_key(self):
-        return self._cur
+        return self._cam.cur
 
     def _image_inputs(self):
-        return self._slots[self._cur]
+        return self._slots[self._cam.cur]
 
     @torch.no_grad()
     def submit(self, x, y, t, p, t_end=None):
         """as StreamingDetector.submit; the step uses the newest frame whose trunk has finished (see the class docstring)."""
-        if self._pending is not None and (self._cur is None or self._pending["ready"].query()):
-            self._promote()
-        if self._cur is None:
+        self._overlapped = self._cam.take_newest()
+        if self._cam.cur is None:
             raise RuntimeError("FusionStreamingDetector: set_frame() must be called before the first chunk")
-        self._overlapped = self._pending is not None
         super().submit(x, y, t, p, t_end)
-        self._reader[self._cur] = self._done
-        self._step_frame = self._cur_frame
+        self._cam.stepped(self._done)
 
     @property
     def frame_state(self):
@@ -365,14 +414,15 @@ class FusionStreamingDetector(StreamingDetector):
         or None)."""
         if self._done is not None:
             self._done.synchronize()
-        fid, t_us = self._step_frame
-        return dict(frame=fid, t_us=t_us, pending=None if self._pending is None else self._pending["id"])
+        return self._cam.state()
 
 
-def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int):
+def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int, planes=None):
     """write the packed multi-stream stage of dagr_stream_push_multi into the int32 array `stage` (>= 4*S + 4*S*max_chunk
-    entries): header [S][4] = {n_new, t_cut, event offset, 0}, then the (x, y, t, polarity) rows of all streams back to back.
-    chunks[s] = (x, y, t, p) host arrays or None (no events).  Returns the per-stream event counts."""
+    entries): header [S][4] = {n_new, t_cut, event offset, plane}, then the (x, y, t, polarity) rows of all streams back to
+    back.  chunks[s] = (x, y, t, p) host arrays or None (no events).  planes[s] = the frame plane stream s's step reads (image
+    fusion, read by the *_planes kernels; the push ignores the word), 0 when `planes` is None.  Returns the per-stream event
+    counts."""
     S = len(chunks)
     ns = [0 if c is None else len(c[2]) for c in chunks]
     for s, n in enumerate(ns):
@@ -384,7 +434,7 @@ def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int):
     ev = stage[4 * S:4 * S + 4 * S * max_chunk].reshape(S * max_chunk, 4)
     o = 0
     for s, (c, n) in enumerate(zip(chunks, ns)):
-        hdr[s] = (n, int(t_cut[s]), o, 0)
+        hdr[s] = (n, int(t_cut[s]), o, 0 if planes is None else int(planes[s]))
         if n:
             x, y, t, p = c
             e = ev[o:o + n]
@@ -407,6 +457,9 @@ class MultiStreamDetector(_RingDetector):
     def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
         if model.backbone.use_image:
             raise NotImplementedError("streaming mode drives the events-only model")
+        self._setup_streams(model, streams, window_us, max_chunk, capacity, device)
+
+    def _setup_streams(self, model, streams, window_us, max_chunk, capacity, device):
         S = int(streams)
         if not 1 <= S <= MAX_STREAMS:
             raise ValueError(f"streams={streams}: 1 <= streams <= {MAX_STREAMS}")
@@ -460,7 +513,7 @@ class MultiStreamDetector(_RingDetector):
             if te is None:
                 te = int(c[2][-1]) if c is not None else int(hdr[s, 1]) + self.window_us
             t_cut.append(int(te) - self.window_us)
-        pack_stage(self._stage_np, cs, t_cut, self.max_chunk)
+        pack_stage(self._stage_np, cs, t_cut, self.max_chunk, planes=self._stage_planes())
         self._step()
 
     def result(self):
@@ -479,6 +532,97 @@ class MultiStreamDetector(_RingDetector):
     def live_window(self, s: int):
         """(pos int32[n,3], polarity f32[n]) of stream s's live window in arrival order (host sync; for tests)."""
         return self._live(s)
+
+    def _stage_planes(self):
+        """word 3 of each stream's stage header: the frame plane of its step (FusionMultiStreamDetector), None for no frames."""
+        return None
+
+
+class FusionMultiStreamDetector(MultiStreamDetector):
+    """S hybrid (image + events) cameras on one GPU: MultiStreamDetector with a camera frame per stream.
+
+        det = FusionMultiStreamDetector(model, streams=S, window_us=50_000)
+        det.set_frame(s, image_u8)             # per camera, at its own frame rate -> that camera's frame id 0, 1, 2, ...
+        det.push([(x, y, t, p) or None per camera], t_end) -> S dicts(boxes, scores, labels)
+
+    Each camera's frames go through the model's own ImageBranch at B = 1, one at a time on the detector's frame stream, and
+    their feature maps and CNN head maps are copied into the camera's two frame slots (_CameraFrames, the same bookkeeping as
+    FusionStreamingDetector).  Every image tensor the step reads is one plane array [2S, C, h, w]; slot j of camera s is plane
+    2s + j.  The plane each camera's step reads travels in word 3 of its stage header, which the step copies to the device
+    anyway, and the image kernels read it there (the *_planes entry points): ONE captured step graph serves every
+    combination of slots, and the step is one replay.
+
+    Semantics: every camera's image is sampled as a batch of one.  Camera s's detections equal those of a
+    FusionStreamingDetector fed the same chunks and frames, and those of model(data) at B = 1 over its live window with the
+    frame frame_state(s) reports (the batched model(data) samples with the batch index as a third grid_sample coordinate,
+    which is not an exact integer for every sample at every B, so it would tie a camera's bits to the number of cameras).
+
+    Frame policy, per camera: a step uses the camera's newest frame whose copy has finished (a non-blocking event query);
+    a camera's first step waits on the device for its first frame; submit raises RuntimeError before any device work while
+    some camera has never had a frame.  reset() keeps the frames."""
+
+    def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+        _check_fusion_model(model, "FusionMultiStreamDetector", "MultiStreamDetector")
+        self._setup_streams(model, streams, window_us, max_chunk, capacity, device)
+        self.frame_stream = torch.cuda.Stream(device=self.dev)
+        self._planes = None                   # (image_feats, image_outs) as plane arrays [2S, ...]
+        self._cams = [_CameraFrames(self, lambda j, f, o, s=s: self._plane_dst(2 * s + j, f, o)) for s in range(self.S)]
+        self._overlapped = [False] * self.S   # per camera: the last step ran while a newer frame of it was in flight
+
+    def _plane_dst(self, k, feats, outs):
+        if self._planes is None:
+            n = 2 * self.S
+            self._planes = ([torch.empty((n,) + tuple(f.shape[1:]), dtype=f.dtype, device=self.dev) for f in feats],
+                            {key: [torch.empty((n,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev) for t in v]
+                             for key, v in outs.items()})
+        pf, po = self._planes
+        return [f[k:k + 1] for f in pf], {key: [t[k:k + 1] for t in v] for key, v in po.items()}
+
+    def _camera(self, s):
+        s = int(s)
+        if not 0 <= s < self.S:
+            raise IndexError(f"camera {s} out of range [0, {self.S})")
+        return self._cams[s]
+
+    @torch.no_grad()
+    def set_frame(self, s: int, image, t_us=None):
+        """start a new frame of camera s (see FusionStreamingDetector.set_frame): returns without waiting for the trunk;
+        returns camera s's frame id (0, 1, 2, ...).  A frame of camera s still pending is waited for and becomes current."""
+        return self._camera(s).set(image, t_us)
+
+    def sync_frame(self, s=None):
+        """block until the pending frame of camera s (of every camera when None) is usable; the next step uses it."""
+        for c in (self._cams if s is None else [self._camera(s)]):
+            c.sync()
+
+    def _image_inputs(self):
+        return self._planes
+
+    def _image_planes(self):
+        return self.stage_d[3:], 4
+
+    def _stage_planes(self):
+        return [2 * s + c.cur for s, c in enumerate(self._cams)]
+
+    @torch.no_grad()
+    def submit(self, chunks, t_end=None):
+        """as MultiStreamDetector.submit; each camera's step uses its newest frame whose copy has finished."""
+        missing = [s for s, c in enumerate(self._cams) if c.cur is None and c.pending is None]
+        if missing:
+            raise RuntimeError(f"FusionMultiStreamDetector: set_frame() must be called for every camera before the first step "
+                               f"(no frame yet: cameras {missing})")
+        self._overlapped = [c.take_newest() for c in self._cams]
+        super().submit(chunks, t_end)
+        for c in self._cams:
+            c.stepped(self._done)
+
+    def frame_state(self, s: int):
+        """camera s after the last finished step: dict(frame=id of the frame the step used, t_us=its timestamp, pending=id of a
+        frame of camera s not yet in use or None)."""
+        cam = self._camera(s)
+        if self._done is not None:
+            self._done.synchronize()
+        return cam.state()
 
 
 def synth_stream(rate_ev_s: int, seconds: float, width: int, height: int, seed: int = 99, kind: str = "uniform"):
@@ -646,7 +790,7 @@ def fusion_stream_benchmark(dev, size="s", img_net="resnet50", width=640, height
         if (k * chunk_us) % frame_us == 0:                              # the camera delivers a frame at stream time k * chunk_us
             ts = time.perf_counter()
             fid = det.set_frame(frames[(k * chunk_us // frame_us) % len(frames)], t_us=k * chunk_us)
-            tr = det._pending["trunk"]
+            tr = det._cam.pending["trunk"]
             if sync_frames:
                 det.sync_frame()
             if k >= warm:
@@ -665,7 +809,7 @@ def fusion_stream_benchmark(dev, size="s", img_net="resnet50", width=640, height
             dev_ms.append(e0.elapsed_time(e1))
             evs.append(b - a)
             overlapped.append(det._overlapped)
-            fid = det._step_frame[0]
+            fid = det._cam.step_frame[0]
             if fid in waiting:
                 first_use.append((t1 - waiting.pop(fid)) * 1e3)
         else:
@@ -699,3 +843,101 @@ def fusion_stream_benchmark(dev, size="s", img_net="resnet50", width=640, height
                      "the host; chunks are submitted back to back, faster than the real 1 ms period, so frames arrive every "
                      "frame_us / chunk_us chunks rather than every frame_us of wall time; Python's cyclic garbage collector is paused "
                      "during the timed loop")
+
+
+def fusion_multistream_benchmark(dev, streams, size="s", img_net="resnet50", width=640, height=480, rate_ev_s=1_000_000,
+                                 chunk_us=1000, window_us=50_000, seconds=2.0, frame_us=50_000, kind="uniform", model=None,
+                                 capacity=1 << 17):
+    """S hybrid cameras on ONE GPU through FusionMultiStreamDetector: S independent synthetic event streams (seeds 99, 100,
+    ...) at `rate_ev_s` each, advanced by one step per chunk period, and a new frame every `frame_us` of stream time per
+    camera, camera s's frames offset by s * frame_us / S (rounded down to the chunk grid) so that the trunks spread out.
+    Latency mode as in multistream_benchmark: a step is submitted, the detections of all S cameras are awaited, then the next
+    step is submitted; frames are set between two steps and never waited for."""
+    from .model.dagr import DAGR
+    from .utils.args import default_args
+    S = int(streams)
+    if model is None:
+        from tests.helpers import randomize_bn
+        torch.manual_seed(0)
+        model = randomize_bn(DAGR(default_args(size, batch_size=1, use_image=True, img_net=img_net), height=height, width=width).eval()).to(dev)
+    total_s = seconds + window_us * 1e-6 + 0.02
+    evs_s = [synth_stream(rate_ev_s, total_s, width, height, seed=99 + s, kind=kind) for s in range(S)]
+    g = torch.Generator().manual_seed(0)
+    frames = [torch.randint(0, 256, (3, height, width), generator=g, dtype=torch.uint8) for _ in range(4)]
+    det = FusionMultiStreamDetector(model, streams=S, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)),
+                                    capacity=capacity)
+    offset = [(s * frame_us // S) // chunk_us * chunk_us for s in range(S)]
+    grid = np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us)
+    bounds = [np.searchsorted(e[2], grid) for e in evs_s]
+    nchunks = len(grid) - 1
+    lat, dev_ms, evs, overlapped, trunk = [], [], [], [], []
+    first_use = [[] for _ in range(S)]
+    waiting = {}                                                         # (camera, frame id) -> host time of its set_frame
+    warm = int(window_us / chunk_us) + 20                                # fill the live windows first (+ graph capture)
+    for s in range(S):                                                   # every camera needs a frame before the first step
+        det.set_frame(s, frames[s % len(frames)], t_us=0)
+    import gc
+    gc_was = gc.isenabled()
+    gc.collect()
+    gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
+    for k in range(nchunks):
+        tk = k * chunk_us
+        for s in range(S):
+            if tk > offset[s] and (tk - offset[s]) % frame_us == 0:      # camera s delivers a frame at stream time tk
+                ts = time.perf_counter()
+                fid = det.set_frame(s, frames[(s + (tk - offset[s]) // frame_us) % len(frames)], t_us=tk)
+                if k >= warm:
+                    trunk.append(det._cams[s].pending["trunk"])
+                    waiting[(s, fid)] = ts
+        chunks = []
+        for (x, y, t, p), bd in zip(evs_s, bounds):
+            a, b = int(bd[k]), int(bd[k + 1])
+            chunks.append((x[a:b], y[a:b], t[a:b], p[a:b]))
+        t_end = [(k + 1) * chunk_us] * S
+        if k >= warm:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0 = time.perf_counter()
+            e0.record(det.stream)
+            det.submit(chunks, t_end)
+            e1.record(det.stream)
+            det.result()
+            t1 = time.perf_counter()
+            lat.append((t1 - t0) * 1e3)
+            dev_ms.append(e0.elapsed_time(e1))
+            evs.append(sum(len(c[2]) for c in chunks))
+            overlapped.append(any(det._overlapped))
+            for s, cam in enumerate(det._cams):
+                key = (s, cam.step_frame[0])
+                if key in waiting:
+                    first_use[s].append((t1 - waiting.pop(key)) * 1e3)
+        else:
+            det.push(chunks, t_end)
+    if gc_was:
+        gc.enable()
+    torch.cuda.synchronize(dev)
+    trunk_ms = [a.elapsed_time(b) for a, b in trunk]
+    st = [det.window_state(s) for s in range(S)]
+    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
+
+    def dist(v):
+        v = sorted(v)
+        return dict(n=len(v), p50=q(v, 0.5), p99=q(v, 0.99), max=v[-1]) if v else dict(n=0)
+
+    busy = sum(lat) * 1e-3
+    return dict(model=f"dagr-{size} + {img_net}", streams=S, width=width, height=height, stream_rate_mev_s=rate_ev_s / 1e6,
+                chunk_us=chunk_us, window_us=window_us, frame_us=frame_us, frame_offset_us=offset, stream_seconds=len(lat) * chunk_us * 1e-6,
+                steps=len(lat), frames=len(trunk_ms), events_per_step=float(np.mean(evs)), live_events=[x["live"] for x in st],
+                overflow=[x["overflow"] for x in st], graphs=len(det.graphs), latency_ms=dist(lat),
+                latency_ms_trunk_in_flight=dist([v for v, o in zip(lat, overlapped) if o]),
+                latency_ms_no_trunk=dist([v for v, o in zip(lat, overlapped) if not o]), steps_trunk_in_flight=int(sum(overlapped)),
+                device_ms=dist(dev_ms), trunk_device_ms=dist(trunk_ms), frame_to_first_use_ms=[dist(v) for v in first_use],
+                sustained_mev_s=sum(evs) / busy / 1e6,
+                note=f"{S} hybrid cameras on one GPU, one FusionMultiStreamDetector step (one CUDA graph replay) per chunk period; every "
+                     "frame_us of stream time each camera's host u8 frame goes through the ResNet trunk + CNN head at B = 1 (captured "
+                     "ImageBranch graphs) on the frame stream and is copied into the camera's free plane; latency = host wall clock "
+                     "from submit() until the detections of all cameras are on the host; *_trunk_in_flight = steps submitted while "
+                     "some camera's newer frame had not finished; device_ms = CUDA events around the step on the detector's stream; "
+                     "trunk_device_ms = CUDA events around the branch on the frame stream; frame_to_first_use_ms[s] = host time from "
+                     "set_frame of camera s until the detections of the first step using that frame are on the host; steps are "
+                     "submitted back to back, faster than the real 1 ms period, so frames arrive every frame_us / chunk_us steps "
+                     "rather than every frame_us of wall time; Python's cyclic garbage collector is paused during the timed loop")

@@ -140,8 +140,10 @@ int dagr_stream_push(int32_t *ctl, const int32_t *stage, int32_t *batch, int32_t
  *   ctl   i32[S+1][8] on the DEVICE, zero-initialised.  Block s = {head slot inside ring s, live count, evicted by the last
  *         push, appended by the last push, sticky overflow flag, kept count, offset of the stream's window in the compact
  *         stream-major order, 0}; block S = {total live count, 0...}.  Zeroing block s resets stream s alone.
- *   stage i32[4*S + 4*S*max_chunk] on the device: header [S][4] = {n_new, t_cut, event offset, 0}, then the (x, y, t,
- *         polarity +-1) events of all streams back to back; stream s's n_new events start at event `offset`.
+ *   stage i32[4*S + 4*S*max_chunk] on the device: header [S][4] = {n_new, t_cut, event offset, plane}, then the (x, y, t,
+ *         polarity +-1) events of all streams back to back; stream s's n_new events start at event `offset`.  Word 3 is the
+ *         frame plane of the stream (image fusion), ignored by the push: the *_planes entry points below read it with
+ *         plane = stage + 3, plane_stride = 4.
  *   dagr_stream_push_multi : per stream, evicts the prefix with t < t_cut and appends its chunk (batch = s); then writes the
  *         window offsets (exclusive scan of the live counts) and the total.  Two launches, grids independent of the counts.
  *   dagr_graph_sort_rings  : dagr_graph_sort over the S live windows read in the compact order c < total: stream s's i-th
@@ -427,6 +429,31 @@ int dagr_postprocess_nms(const float *pred, int B, int A, int nc, float conf_thr
 int dagr_sample_features(const float *img, int Bi, int C, int h, int w, const float *posx, const float *posy,
                          const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
                          void *stream);
+
+/* Plane mode of the image kernels (several hybrid cameras as the samples of one streaming step, each with its own frame):
+ * the image is a plane array [nplanes][C][h][w] and sample b reads plane[b * plane_stride] alone, sampled as a batch of
+ * one -- the bits a B = 1 forward gives that sample with that plane as its image (the batched forward samples with the batch
+ * index as a third grid_sample coordinate, which mixes neighbouring planes where it is not an integer).  Plane values are
+ * device data: the kernels clamp them to [0, nplanes).  Every *_planes entry point returns DAGR_E_ARG with a message before
+ * launching anything on a null pointer (feat_s may be NULL), nplanes < 1, plane_stride < 1 or N outside [0, 2^31).
+ *   dagr_l1_x0_image_planes      : dagr_l1_x0_image_live (bounded by the live total start[g->NK]) with img0 [nplanes,16,h,w].
+ *   dagr_voxel_sample_max_planes : dagr_voxel_sample_max with img [nplanes,C,h,w]; a voxel's window is staged from its one
+ *                                  plane; also refuses c0 + C > ldx.
+ *   dagr_sample_features_planes  : dagr_sample_features with img [nplanes,C,h,w]; node i samples plane[bidx[i] * stride].
+ *   dagr_head_finish_planes      : dagr_head_finish with add_* [nplanes,C,ny,nx] (all three required); the maps of sample b
+ *                                  are read at plane[b * stride]. */
+int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                            const float *img0, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *x0,
+                            void *stream);
+int dagr_voxel_sample_max_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *img, int C,
+                                 int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *xg, int ldx, int c0,
+                                 int pool_mean, void *stream);
+int dagr_sample_features_planes(const float *img, int nplanes, const int32_t *plane, int plane_stride, int C, int h, int w,
+                                const float *posx, const float *posy, const int32_t *bidx, int64_t n, int width, int height,
+                                float *out, int ldo, int c0, void *stream);
+int dagr_head_finish_planes(const dagr_grid_t *gr, const int32_t *cnt, const float *cls, int ldc, const float *regobj, int ldr,
+                            const float *add_cls, const float *add_reg, const float *add_obj, int nc, int stride, int a0, int A,
+                            int nplanes, const int32_t *plane, int plane_stride, float *out, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a14  asy_tools (src/dagr/asynchronous/asy_tools/main.cu:239-244), same argument meaning.
