@@ -21,6 +21,7 @@ ELL = 16
 KU = 15
 TABW = 16
 L1_TC_WFRAG_FLOATS = 8192               # DAGR_L1_TC_WFRAG_FLOATS
+L1A_TC_WFRAG_FLOATS = 1536              # DAGR_L1A_TC_WFRAG_FLOATS
 
 p = C.c_void_p
 i32 = C.c_int32
@@ -87,6 +88,8 @@ _SIGS = {
     "dagr_graph_sort_rings": (C.c_int, [C.POINTER(Geom), p, p, p, i64, C.c_int, p, p, p, p, p, p, p, p, p, p, p, p]),
     "dagr_graph_search": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p]),
     "dagr_l1_build": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, C.POINTER(L1AParams), p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
+    "dagr_l1a_tc_weights": (C.c_int, [C.POINTER(L1AParams), p]),
+    "dagr_l1_build_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.POINTER(L1AParams), p, p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
     "dagr_xa_permute": (C.c_int, [i64, p, C.c_int, p, p, C.c_int, p]),
     "dagr_l1_x0_image": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, p, p]),
     "dagr_l1_x0_image_live": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, p, p]),

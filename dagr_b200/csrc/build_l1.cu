@@ -250,12 +250,76 @@ __device__ __forceinline__ int bl_probe_coop(const dagr_geom_t &g, int64_t N, in
     return n;
 }
 
+// ---- conv_a phase 2 on tensor cores (TC instances, dagr_l1_build_tc) -----------------------------------------------------
+// out = [32 nodes of a warp x 48] x [48 x 16]: k = 3u + ci for the 45 slot inputs A[u][ci], k = 45 + ci for the root inputs
+// (polarity, x/W, y/H) of the node itself.  mma.sync.m16n8k8 TF32 in 3xTF32 form (common.cuh): 6 k-steps x 2 m-tiles x
+// 2 n-tiles.  On CUDA cores the product is 768 FFMA per event, each with its weight from the constant bank.
+// Every lane holds one node's row; the A fragments need other lanes' rows, which go through shared memory: per k-step the
+// warp writes its 32 x 8 block and reads it back with two ldmatrix.x4 (one per m-tile).  The block lives in the warp's own
+// columns of s_acc, rows 0..7: s_acc[q][tid] is read only by phase B of lane tid (and written by the probe of a lane of the
+// same warp), so after the warp's __syncwarp those columns are dead until the next chunk's probe, which starts behind a CTA
+// barrier.  No shared memory is added, so the lean instance keeps five CTAs per SM.
+// Layout: 16-byte chunk h (k = 4h .. 4h+3) of node row r at s_acc row 4h + (r >> 3), byte 16 (r & 7) of the warp's 128-byte
+// piece: each ldmatrix matrix (8 nodes, one chunk) is one 128-byte piece, the stores and loads are free of bank conflicts.
+// The six k-steps are one chain of 18 mma per output through fresh (zeroed) fragments, about the length of one conv_b2 pass
+// (15).  conv_b2 measured twice the largest oracle error when all its passes were chained (the tensor cores' fp32 accumulation
+// truncates); splitting this chain in two groups summed with __fadd_rn needs 16 more registers, which spilled in all three
+// instances.  An output depends only on its node's row and the fixed k order, so a node gets the same bits in every instance.
+// Weight fragments: dagr_l1a_tc_weights, float4 [k-step 0..5][lane][n-tile] = (hi b0, hi b1, lo b0, lo b1).
+#define BL_TC_KSTEPS 6
+static_assert(8 * BL_TC_KSTEPS == 3 * DAGR_KU + 3 && BL_TC_KSTEPS * 32 * 2 * 4 == DAGR_L1A_TC_WFRAG_FLOATS, "48 = 45 slot + 3 root inputs");
+
+// The lean instance runs phase B at its 72-register cap with the 45 accumulators live; phase 2 adds 16 C registers plus the
+// fragments.  So the inputs k = 38 .. 44 are parked in rows 8..14 of the lane's own s_acc column (dead as well, see above)
+// right after phase B and read back for k-steps 4 and 5.  ptxas still spills loop state around phase 2 (52 bytes stored,
+// 92 loaded per thread and chunk; 5 CTAs per SM kept).
+#define BL_TC_PARK0 38
+
+// this lane's 8 inputs of k-step s (pk: the parked inputs, read back)
+template <int s>
+__device__ __forceinline__ void bl_tc_inputs(const float (&A)[DAGR_KU][3], const float pk[3 * DAGR_KU - BL_TC_PARK0], const float rt[3],
+                                             float v[8])
+{
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int k = 8 * s + j;
+        v[j] = k < BL_TC_PARK0 ? A[k / 3][k % 3] : k < 3 * DAGR_KU ? pk[k - BL_TC_PARK0] : rt[k - 3 * DAGR_KU];
+    }
+}
+
+// c (C fragments) += [warp's 32 rows x 8] x [8 x 16] for k-step s.  xw = shared address of the warp's s_acc columns.
+// Warp-uniform.
+template <int s, int THREADS>
+__device__ __forceinline__ void bl_tc_kstep(const float v[8], uint32_t xw, const float4 *__restrict__ wfrag, float2 c[8])
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t row = xw + (lane >> 3) * (THREADS * 4) + 16 * (lane & 7);
+    __syncwarp();                                                       // the previous k-step's block has been read
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" :: "r"(row), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" :: "r"(row + 4 * THREADS * 4), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
+                 : "memory");
+    __syncwarp();
+    // matrix i = lane >> 3 of m-tile mt: nodes 16 mt + 8 (i & 1) + 0..7, chunk i >> 1
+    const uint32_t la = xw + (4 * (lane >> 4) + ((lane >> 3) & 1)) * (THREADS * 4) + 16 * (lane & 7);
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++) {
+        uint32_t r[4], ah[4], al[4];
+        ldsm_x4(la + 2 * mt * THREADS * 4, r);
+#pragma unroll
+        for (int i = 0; i < 4; i++) tf32_split(r[i], ah[i], al[i]);
+#pragma unroll
+        for (int nt = 0; nt < 2; nt++)
+            mma_3xtf32(c[4 * mt + 2 * nt], c[4 * mt + 2 * nt + 1], ah, al, __ldg(wfrag + (s * 32 + lane) * 2 + nt));
+    }
+}
+
 // work list: wl_hdr[0] = number of voxels beyond this instance's staging capacity (queued in wl_ids when `defer`, otherwise
 // only counted and probed from global memory), wl_hdr[1] = pop cursor of the dense kernel
-template <int CAP, int THREADS>
+template <int CAP, int THREADS, bool TC>
 __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const int32_t *__restrict__ start, const int2 *__restrict__ ti,
                                          const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
-                                         const dagr_l1a_params_t &P, const int do_conv, const int min_idx, const int32_t *__restrict__ flags,
+                                         const dagr_l1a_params_t &P, const float4 *__restrict__ wfrag, const int do_conv, const int min_idx,
+                                         const int32_t *__restrict__ flags,
                                          int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask,
                                          float *__restrict__ xa, const int cell, unsigned char *smem_raw, BLTile &T, uint32_t &s_mask,
                                          int32_t *__restrict__ wl_hdr, int32_t *__restrict__ wl_ids, const int defer)
@@ -579,6 +643,64 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
         if (staged) edges(std::true_type{});
         else        edges(std::false_type{});
 
+        if constexpr (TC) {
+            // the mma calls are warp-uniform: a lane without a node joins with its row (finite, and a row only reaches its
+            // own outputs) and stores nothing
+            if (!do_conv || !__any_sync(0xffffffffu, active)) continue;
+            const uint32_t xw = bl_sa(s_acc) + 4u * (threadIdx.x & ~31u);
+            float2 c[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) c[i] = make_float2(0.f, 0.f);
+            constexpr int NPK = 3 * DAGR_KU - BL_TC_PARK0;
+            const uint32_t own = bl_sa(s_acc) + 4u * threadIdx.x;
+#pragma unroll
+            for (int j = 0; j < NPK; j++) {
+                const int k = BL_TC_PARK0 + j;
+                bl_sts32(own + (8 + j) * THREADS * 4, __float_as_uint(A[k / 3][k % 3]));
+            }
+            float rt[3] = {0.f, 0.f, 0.f}, pk[NPK], v[8];
+#pragma unroll
+            for (int j = 0; j < NPK; j++) pk[j] = 0.f;
+            bl_tc_inputs<0>(A, pk, rt, v); bl_tc_kstep<0, THREADS>(v, xw, wfrag, c);
+            bl_tc_inputs<1>(A, pk, rt, v); bl_tc_kstep<1, THREADS>(v, xw, wfrag, c);
+            bl_tc_inputs<2>(A, pk, rt, v); bl_tc_kstep<2, THREADS>(v, xw, wfrag, c);
+            bl_tc_inputs<3>(A, pk, rt, v); bl_tc_kstep<3, THREADS>(v, xw, wfrag, c);
+#pragma unroll
+            for (int j = 0; j < NPK; j++) pk[j] = __uint_as_float(bl_lds32(own + (8 + j) * THREADS * 4));
+            bl_tc_inputs<4>(A, pk, rt, v); bl_tc_kstep<4, THREADS>(v, xw, wfrag, c);
+            // root inputs: read again rather than kept live through phase B (see the CUDA-core form below)
+            int pr = p;
+            asm volatile("" : "+r"(txy), "+r"(pr));
+            rt[0] = __ldg(feat_s + pr); rt[1] = s_posx[(txy & 0xffff) + g.r]; rt[2] = s_posy[(txy >> 16) + g.r];
+            bl_tc_inputs<5>(A, pk, rt, v); bl_tc_kstep<5, THREADS>(v, xw, wfrag, c);
+            // BN + act straight from the C fragments: this lane holds channels 8 nt + 2t, +1 of nodes 16 mt + g and 16 mt + g + 8,
+            // i.e. 8 bytes of the xa half-row nt (half-major [2][N][8], 16-byte chunks swizzled by XA_SWZ); the four lanes of a
+            // row write its 32 bytes
+            const int lane = threadIdx.x & 31, gq = lane >> 2, t = lane & 3;
+            const int pv = active ? p : -1;
+            float2 sc[2], sh[2];
+#pragma unroll
+            for (int nt = 0; nt < 2; nt++) {
+                sc[nt] = *reinterpret_cast<const float2 *>(&P.scale[8 * nt + 2 * t]);
+                sh[nt] = *reinterpret_cast<const float2 *>(&P.shift[8 * nt + 2 * t]);
+            }
+#pragma unroll
+            for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+                for (int hr = 0; hr < 2; hr++) {
+                    const int q = __shfl_sync(0xffffffffu, pv, 16 * mt + 8 * hr + gq);
+#pragma unroll
+                    for (int nt = 0; nt < 2; nt++) {
+                        const float2 o = c[4 * mt + 2 * nt + hr];
+                        float r0 = fmaf(o.x, sc[nt].x, sh[nt].x), r1 = fmaf(o.y, sc[nt].y, sh[nt].y);
+                        if (P.relu) { r0 = fmaxf(r0, 0.f); r1 = fmaxf(r1, 0.f); }
+                        if (q >= 0)
+                            *reinterpret_cast<float2 *>(xa + ((int64_t)nt * N + q) * 8 + (((t >> 1) ^ XA_SWZ(q)) << 2) + 2 * (t & 1)) =
+                                make_float2(r0, r1);
+                    }
+                }
+            continue;
+        }
         if (!active || !do_conv) continue;
         // conv_a phase 2: out = sum_u W_u^T A_u + W_root^T x_i, BN, act  (weights in the constant bank)
         // the root term's inputs are read again rather than kept live through phase B, which keeps the lean instance within
@@ -622,28 +744,29 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
 
 
 
-template <int CAP, int MIN_CTAS>
+template <int CAP, int MIN_CTAS, bool TC>
 __global__ void __launch_bounds__(BL_THREADS, MIN_CTAS)
 k_l1_build(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const int2 *__restrict__ ti,
            const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
-           const __grid_constant__ dagr_l1a_params_t P, const int do_conv, const int min_idx, const int32_t *__restrict__ flags,
-           int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask, float *__restrict__ xa,
-           int32_t *__restrict__ wl_hdr, int32_t *__restrict__ wl_ids, const int defer)
+           const __grid_constant__ dagr_l1a_params_t P, const float4 *__restrict__ wfrag, const int do_conv, const int min_idx,
+           const int32_t *__restrict__ flags, int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask,
+           float *__restrict__ xa, int32_t *__restrict__ wl_hdr, int32_t *__restrict__ wl_ids, const int defer)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ BLTile T;
     __shared__ uint32_t s_mask;
-    bl_voxel<CAP, BL_THREADS>(g, N, start, ti, xyb, feat_s, P, do_conv, min_idx, flags, nbr, off, cellmask, xa,
-                              (int)blockIdx.x, smem_raw, T, s_mask, wl_hdr, wl_ids, defer);
+    bl_voxel<CAP, BL_THREADS, TC>(g, N, start, ti, xyb, feat_s, P, wfrag, do_conv, min_idx, flags, nbr, off, cellmask, xa,
+                                  (int)blockIdx.x, smem_raw, T, s_mask, wl_hdr, wl_ids, defer);
 }
 
 // dense voxels: persistent CTAs (one per SM) pop voxel ids from the work list the regular kernel filled
+template <bool TC>
 __global__ void __launch_bounds__(BL_THREADS_BIG, 1)
 k_l1_build_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const int2 *__restrict__ ti,
                  const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
-                 const __grid_constant__ dagr_l1a_params_t P, const int do_conv, const int min_idx, const int32_t *__restrict__ flags,
-                 int32_t *__restrict__ nbr, uint16_t *__restrict__ off, uint32_t *__restrict__ cellmask, float *__restrict__ xa,
-                 int32_t *__restrict__ wl_hdr, const int32_t *__restrict__ wl_ids)
+                 const __grid_constant__ dagr_l1a_params_t P, const float4 *__restrict__ wfrag, const int do_conv, const int min_idx,
+                 const int32_t *__restrict__ flags, int32_t *__restrict__ nbr, uint16_t *__restrict__ off,
+                 uint32_t *__restrict__ cellmask, float *__restrict__ xa, int32_t *__restrict__ wl_hdr, const int32_t *__restrict__ wl_ids)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ BLTile T;
@@ -656,18 +779,18 @@ k_l1_build_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ sta
         __syncthreads();
         const int i = s_next;
         if (i >= count) break;
-        bl_voxel<BL_CAP_BIG, BL_THREADS_BIG>(g, N, start, ti, xyb, feat_s, P, do_conv, min_idx, flags, nbr, off, cellmask, xa,
-                                             wl_ids[i], smem_raw, T, s_mask, nullptr, nullptr, 0);
+        bl_voxel<BL_CAP_BIG, BL_THREADS_BIG, TC>(g, N, start, ti, xyb, feat_s, P, wfrag, do_conv, min_idx, flags, nbr, off, cellmask, xa,
+                                                 wl_ids[i], smem_raw, T, s_mask, nullptr, nullptr, 0);
     }
 }
 
-extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
-                             const uint32_t *xyb, const float *feat_s, const float *tab,
-                             const dagr_l1a_params_t *p_host, const int32_t *flags, int min_idx, int32_t *nbr, uint16_t *off,
-                             uint32_t *cellmask, float *xa, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
+template <bool TC>
+static int l1_build_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti, const uint32_t *xyb,
+                           const float *feat_s, const dagr_l1a_params_t *p_host, const float4 *wfrag, const int32_t *flags,
+                           int min_idx, int32_t *nbr, uint16_t *off, uint32_t *cellmask, float *xa, int32_t *wl_hdr,
+                           int32_t *wl_ids, int defer, cudaStream_t st)
 {
     DAGR_CHECK_ARG(g, "null argument");
-    (void)tab;                                                          // the slot weights come from g->tabx / g->taby
     static const dagr_l1a_params_t zero_params = {};
     const int do_conv = p_host != nullptr;
     if (!p_host) p_host = &zero_params;
@@ -678,16 +801,16 @@ extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *sta
     const bool deferring = wl_hdr != nullptr && wl_ids != nullptr && defer;
     if (deferring) {
         const size_t smem = bl_smem_bytes(g, BL_CAP, BL_THREADS);
-        auto kern = k_l1_build<BL_CAP, 4>;
+        auto kern = k_l1_build<BL_CAP, 4, TC>;
         DAGR_CUDA(dagr_allow_smem(kern, smem, true));
-        kern<<<cells, BL_THREADS, smem, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, do_conv, min_idx,
-                                                                flags, nbr, off, cellmask, xa, wl_hdr, wl_ids, 1);
+        kern<<<cells, BL_THREADS, smem, st>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, wfrag, do_conv, min_idx, flags, nbr,
+                                              off, cellmask, xa, wl_hdr, wl_ids, 1);
     } else {
         const size_t smem = bl_smem_bytes(g, BL_CAP_LEAN, BL_THREADS);
-        auto kern = k_l1_build<BL_CAP_LEAN, 5>;
+        auto kern = k_l1_build<BL_CAP_LEAN, 5, TC>;
         DAGR_CUDA(dagr_allow_smem(kern, smem, true));
-        kern<<<cells, BL_THREADS, smem, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, do_conv, min_idx,
-                                                                flags, nbr, off, cellmask, xa, wl_hdr, wl_ids, 0);
+        kern<<<cells, BL_THREADS, smem, st>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, wfrag, do_conv, min_idx, flags, nbr,
+                                              off, cellmask, xa, wl_hdr, wl_ids, 0);
     }
     DAGR_CHECK_LAUNCH();
     if (deferring) {
@@ -698,11 +821,50 @@ extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *sta
             DAGR_CUDA(cudaGetDevice(&dev));
             DAGR_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
         }
-        DAGR_CUDA(dagr_allow_smem(k_l1_build_dense, smem_big));
-        k_l1_build_dense<<<n_sm, BL_THREADS_BIG, smem_big, (cudaStream_t)stream>>>(*g, N, start, (const int2 *)ti, xyb, feat_s,
-                                                                                    *p_host, do_conv, min_idx, flags, nbr, off,
-                                                                                    cellmask, xa, wl_hdr, wl_ids);
+        auto kd = k_l1_build_dense<TC>;
+        DAGR_CUDA(dagr_allow_smem(kd, smem_big));
+        kd<<<n_sm, BL_THREADS_BIG, smem_big, st>>>(*g, N, start, (const int2 *)ti, xyb, feat_s, *p_host, wfrag, do_conv, min_idx, flags,
+                                                   nbr, off, cellmask, xa, wl_hdr, wl_ids);
         DAGR_CHECK_LAUNCH();
     }
+    return DAGR_OK;
+}
+
+extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
+                             const uint32_t *xyb, const float *feat_s, const float *tab,
+                             const dagr_l1a_params_t *p_host, const int32_t *flags, int min_idx, int32_t *nbr, uint16_t *off,
+                             uint32_t *cellmask, float *xa, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
+{
+    (void)tab;                                                          // the slot weights come from g->tabx / g->taby
+    return l1_build_launch<false>(g, N, start, ti, xyb, feat_s, p_host, nullptr, flags, min_idx, nbr, off, cellmask, xa, wl_hdr,
+                                  wl_ids, defer, (cudaStream_t)stream);
+}
+
+extern "C" int dagr_l1_build_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
+                                const uint32_t *xyb, const float *feat_s, const dagr_l1a_params_t *p_host, const float *wfrag,
+                                const int32_t *flags, int min_idx, int32_t *nbr, uint16_t *off, uint32_t *cellmask, float *xa,
+                                int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
+{
+    DAGR_CHECK_ARG(p_host && wfrag, "null params / weight fragments (dagr_l1a_tc_weights); the adjacency-only form is "
+                                    "dagr_l1_build with p_host = NULL");
+    return l1_build_launch<true>(g, N, start, ti, xyb, feat_s, p_host, (const float4 *)wfrag, flags, min_idx, nbr, off, cellmask, xa,
+                                 wl_hdr, wl_ids, defer, (cudaStream_t)stream);
+}
+
+// host-side packing of the weight fragments of the TC instances (layout: see bl_tc_kstep): B[k][n] = w[k / 3][k % 3][n] for
+// k < 45, root[k - 45][n] after that
+extern "C" int dagr_l1a_tc_weights(const dagr_l1a_params_t *p_host, float *wfrag_host)
+{
+    DAGR_CHECK_ARG(p_host && wfrag_host, "null argument");
+    auto B = [&](int k, int n) { return k < 3 * DAGR_KU ? p_host->w[k / 3][k % 3][n] : p_host->root[k - 3 * DAGR_KU][n]; };
+    for (int s = 0; s < BL_TC_KSTEPS; s++)
+        for (int lane = 0; lane < 32; lane++)
+            for (int nt = 0; nt < 2; nt++) {
+                const int gq = lane >> 2, t = lane & 3, n = 8 * nt + gq;
+                const float x0 = B(8 * s + t, n), x1 = B(8 * s + t + 4, n);
+                const float h0 = tf32_rna_host(x0), h1 = tf32_rna_host(x1);
+                float *o = wfrag_host + (((size_t)s * 32 + lane) * 2 + nt) * 4;
+                o[0] = h0; o[1] = h1; o[2] = x0 - h0; o[3] = x1 - h1;
+            }
     return DAGR_OK;
 }

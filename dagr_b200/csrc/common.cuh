@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 #include "../../include/dagr_b200.h"
 
 #ifndef __CUDA_ARCH__
@@ -74,6 +75,57 @@ __device__ __forceinline__ float dec_ordered(uint32_t e)
 // fp32 FMA on both halves of a float2: d = a*b + c, round-to-nearest on each.  Hopper has no packed fp32 FMA, so this is
 // two FFMA; the kernels keep their paired accumulator layout.
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+
+// ---- 3xTF32 on tensor cores (mma.sync.m16n8k8, used by the per-voxel conv kernels of conv_l1.cu and build_l1.cu) ----------
+// x = hi + lo with hi = cvt.rna.tf32(x) and lo = x - hi (exact); a product is summed as a_lo*b_hi + a_hi*b_lo + a_hi*b_hi,
+// relative error ~1e-6 against the fp32 sum.  Fragment order of m16n8k8 (g = lane >> 2, t = lane & 3):
+//   A (row-major 16 x 8): a0 = A[g][t], a1 = A[g+8][t], a2 = A[g][t+4], a3 = A[g+8][t+4]
+//   B (col-major 8 x 8):  b0 = B[t][g], b1 = B[t+4][g]
+//   C (16 x 8):           c01 = (C[g][2t], C[g][2t+1]), c23 = (C[g+8][2t], C[g+8][2t+1])
+// The weight fragments come split on the host, one float4 per lane and n-tile: (hi b0, hi b1, lo b0, lo b1).
+// hi is rounded with integer ops: sm_90 has no instruction for cvt.rna.tf32.f32, and ptxas expands it to a non-finite test,
+// an add, a select and a mask per value.  (x + 0x1000) & 0xffffe000 is that expansion without the test: the same bits for
+// every finite x (round to nearest, ties away from zero; a carry into the exponent is the correct rounding), and the split
+// inputs of both kernels are finite.  (A non-finite input gives a non-finite row either way.)
+__device__ __forceinline__ void tf32_split(uint32_t x, uint32_t &hi, uint32_t &lo)
+{
+    hi = (x + 0x1000u) & 0xffffe000u;
+    lo = __float_as_uint(__uint_as_float(x) - __uint_as_float(hi));
+}
+__device__ __forceinline__ void mma_tf32(float2 &c01, float2 &c23, const uint32_t a[4], uint32_t b0, uint32_t b1)
+{
+    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(c01.x), "+f"(c01.y), "+f"(c23.x), "+f"(c23.y)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// C += A B in 3xTF32, always in this order (an output element then depends only on its own A row and the k order)
+__device__ __forceinline__ void mma_3xtf32(float2 &c01, float2 &c23, const uint32_t ah[4], const uint32_t al[4], const float4 b)
+{
+    mma_tf32(c01, c23, al, __float_as_uint(b.x), __float_as_uint(b.y));
+    mma_tf32(c01, c23, ah, __float_as_uint(b.z), __float_as_uint(b.w));
+    mma_tf32(c01, c23, ah, __float_as_uint(b.x), __float_as_uint(b.y));
+}
+// ldmatrix of 32-bit elements: matrix i (8 rows of 16 bytes, row addresses from lanes 8i .. 8i+7) lands in r[i] as
+// element (row lane >> 2, column lane & 3) -- an A fragment when the four matrices are (rows 0-7 | 8-15) x (k 0-3 | 4-7)
+__device__ __forceinline__ void ldsm_x2(uint32_t saddr, uint32_t &r0, uint32_t &r1)
+{
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(saddr) : "memory");
+}
+__device__ __forceinline__ void ldsm_x4(uint32_t saddr, uint32_t r[4])
+{
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
+}
+// host side of the split: cvt.rna.tf32.f32 (nearest, ties away from zero)
+static inline float tf32_rna_host(float x)
+{
+    uint32_t u;
+    memcpy(&u, &x, 4);
+    if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & 0xffffe000u;
+    float r;
+    memcpy(&r, &u, 4);
+    return r;
+}
 
 // degree-1 open B-spline basis in 2-D (torch_spline_conv semantics): 4 (weight, slot) pairs
 // for pseudo coordinates (ax, ay); kernel_size ks per dim.

@@ -371,21 +371,8 @@ struct CB2Tile {
 #endif
 #define CB2_TC_KSTEPS 16                   // per channel half: 15 spline slots + root
 
-__device__ __forceinline__ uint32_t tf32_rna(float x)
-{
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-__device__ __forceinline__ void mma_tf32(float2 &c01, float2 &c23, const uint32_t a[4], uint32_t b0, uint32_t b1)
-{
-    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-        : "+f"(c01.x), "+f"(c01.y), "+f"(c23.x), "+f"(c23.y)
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 // o2 (C fragments) += [this warp's nodes x 8] x [8 x 16]; this lane's node contributes a[0..7], wf = this k-step's fragments
-// of this lane.  Warp-uniform call; lanes without a node pass zeros.
+// of this lane.  Warp-uniform call; lanes without a node pass zeros.  (tf32_split / mma_3xtf32 / ldsm_*: common.cuh)
 __device__ __forceinline__ void cb2_tc_kstep(float *xt, const float a[8], const float4 *__restrict__ wf, float2 o2[8])
 {
     const int lane = threadIdx.x & 31;
@@ -403,16 +390,14 @@ __device__ __forceinline__ void cb2_tc_kstep(float *xt, const float a[8], const 
             if ((lane >> 4) == mt) *reinterpret_cast<float4 *>(row) = make_float4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
             __syncwarp();
             uint32_t r0, r1;                                       // r0 = A[g][4h + t], r1 = A[g + 8][4h + t]
-            asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(ra) : "memory");
-            ah[2 * h] = tf32_rna(__uint_as_float(r0));
-            ah[2 * h + 1] = tf32_rna(__uint_as_float(r1));
-            al[2 * h] = __float_as_uint(__uint_as_float(r0) - __uint_as_float(ah[2 * h]));
-            al[2 * h + 1] = __float_as_uint(__uint_as_float(r1) - __uint_as_float(ah[2 * h + 1]));
+            ldsm_x2(ra, r0, r1);
+            tf32_split(r0, ah[2 * h], al[2 * h]);
+            tf32_split(r1, ah[2 * h + 1], al[2 * h + 1]);
         }
         // (a0, a1, a2, a3) = (A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]): the order of ah / al above
         const uint32_t fa[4] = {ah[0], ah[1], ah[2], ah[3]}, fl[4] = {al[0], al[1], al[2], al[3]};
 #pragma unroll
-        for (int nt = 0; nt < 2; nt++) {
+        for (int nt = 0; nt < 2; nt++) {                           // the 3xTF32 order of mma_3xtf32
             mma_tf32(o2[4 * mt + 2 * nt], o2[4 * mt + 2 * nt + 1], fl, bh[nt][0], bh[nt][1]);
             mma_tf32(o2[4 * mt + 2 * nt], o2[4 * mt + 2 * nt + 1], fa, bl[nt][0], bl[nt][1]);
             mma_tf32(o2[4 * mt + 2 * nt], o2[4 * mt + 2 * nt + 1], fa, bh[nt][0], bh[nt][1]);
@@ -1138,16 +1123,6 @@ extern "C" int dagr_l1_conv_a_image_inc(const dagr_geom_t *g, int64_t N, const i
 }
 
 // host-side packing of the weight fragments the tensor-core instances read (layout: see cb2_tc_kstep)
-static float tf32_rna_host(float x)
-{
-    uint32_t u;
-    memcpy(&u, &x, 4);
-    if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & 0xffffe000u;   // cvt.rna.tf32.f32: nearest, ties away from zero
-    float r;
-    memcpy(&r, &u, 4);
-    return r;
-}
-
 extern "C" int dagr_l1_tc_weights(const float *w_host, const float *root_host, int cin, float *wfrag_host)
 {
     DAGR_CHECK_ARG(w_host && root_host && wfrag_host, "null argument");

@@ -32,6 +32,14 @@ def _tc_weights(lib, params, cin: int, device) -> torch.Tensor:
     return torch.frombuffer(out, dtype=torch.float32).clone().to(device)
 
 
+def _l1a_tc_weights(lib, params, device) -> torch.Tensor:
+    """params.w / params.root of conv_block1.conv_block1's event channels in the mma fragment order of the tensor-core build
+    kernel (dagr_l1a_tc_weights)."""
+    out = (C.c_float * _lib.L1A_TC_WFRAG_FLOATS)()
+    _lib.check(lib.dagr_l1a_tc_weights(C.byref(params), C.cast(out, C.c_void_p)), "dagr_l1a_tc_weights")
+    return torch.frombuffer(out, dtype=torch.float32).clone().to(device)
+
+
 def _fill(arr, t: torch.Tensor):
     flat = t.detach().float().cpu().contiguous().view(-1)
     assert flat.numel() == len(arr), (flat.numel(), len(arr))
@@ -145,7 +153,7 @@ class Engine:
         self._out_slot = {}
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
-    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
+    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_graph_search=1, dagr_l1_build=2, dagr_l1_build_tc=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_l1_conv_a_image_inc=2, dagr_voxel_sample_max_inc=1,
                      dagr_l1_x0_image_planes=1, dagr_voxel_sample_max_planes=1, dagr_sample_features_planes=1, dagr_head_finish_planes=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
@@ -243,6 +251,7 @@ class Engine:
             pa.relu = 1
             _fill(pb.skip, cb.lin.mlp.weight.detach().cpu().t())            # [3,16]
             pk["l1a"] = pa
+            pk["l1a_wfrag"] = _l1a_tc_weights(self.lib, pa, device)
         else:
             # input channels of the layer: [polarity, 16 image samples, x, y] (net.py:117-124).  The image channels go to the
             # TMA-staged conv (rows 0..15 of the padded 24), the three event channels to the probe kernel (they need no gather)
@@ -258,6 +267,7 @@ class Engine:
             _fill(pe.scale, torch.ones(16)); _fill(pe.shift, torch.zeros(16))
             pe.relu = 0
             pk["l1a_img"] = pe
+            pk["l1a_img_wfrag"] = _l1a_tc_weights(self.lib, pe, device)
             s, b = _fold_bn(ca.norm); _fill(pi.scale, s); _fill(pi.shift, b)
             s, b = _fold_bn(cb.norm_skip); _fill(pi.sscale, s); _fill(pi.sshift, b)
             pi.relu = 1
@@ -597,8 +607,8 @@ class Engine:
                           _lib.ptr(stream_state.xa_arr), 0, st)
             # adjacency + the (polarity, x, y) part of conv_block1.conv_block1, which runs on [polarity, 16 image samples, x, y]
             # (net.py:117-126); the image channels follow in dagr_l1_conv_a_image
-            self._run("l1_build", lib.dagr_l1_build, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), _lib.ptr(geom.d_tab1), C.byref(pk["l1a_img"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr), _lib.ptr(off),
+            self._run("l1_build", lib.dagr_l1_build_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
+                      _lib.ptr(ws["feat_s"]), C.byref(pk["l1a_img"]), _lib.ptr(pk["l1a_img_wfrag"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr), _lib.ptr(off),
                       _lib.ptr(cellmask), _lib.ptr(ws["xa"]), _lib.ptr(wl_hdr), _lib.ptr(self._zs(ws, "wl_build", torch.int32)), defer[0], st)
             if image_event is not None:                       # stage 1 of the image branch ran on a side stream next to sort + probe
                 torch.cuda.current_stream().wait_event(image_event[0])
@@ -635,8 +645,8 @@ class Engine:
             if min_idx > 0:
                 self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
                           _lib.ptr(stream_state.xa_arr), 0, st)
-            self._run("l1_build", lib.dagr_l1_build, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), _lib.ptr(geom.d_tab1), C.byref(pk["l1a"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr),
+            self._run("l1_build", lib.dagr_l1_build_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
+                      _lib.ptr(ws["feat_s"]), C.byref(pk["l1a"]), _lib.ptr(pk["l1a_wfrag"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr),
                       _lib.ptr(off), _lib.ptr(cellmask), _lib.ptr(ws["xa"]), _lib.ptr(wl_hdr), _lib.ptr(self._zs(ws, "wl_build", torch.int32)),
                       defer[0], st)
             if stream_state is not None:

@@ -267,6 +267,21 @@ int dagr_l1_conv_a(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const f
                    const int32_t *nbr, const uint16_t *off, const float *tab,
                    const dagr_l1a_params_t *p_host, float *xa /*[N,16]*/, void *stream);
 
+/* Tensor-core form of dagr_l1_build (the engine's path).  Same arguments without the unused `tab`, plus `wfrag`
+ * f32[DAGR_L1A_TC_WFRAG_FLOATS] on the DEVICE: p_host->w and p_host->root as one [48][16] matrix (k = 3 u + cin for the slot
+ * weights, 45 + cin for the root) in mma fragment order, split for 3xTF32, as written by dagr_l1a_tc_weights.  conv_a's
+ * per-node product (45 slot inputs + 3 root inputs -> 16 channels) then runs as mma.sync TF32 (hi*hi + hi*lo + lo*hi, ~1e-6
+ * relative to the fp32 sums) instead of 768 fp32 FMA per event; nbr / off / cellmask are the bits of dagr_l1_build, and every
+ * node's xa row gets the same bits in every instance (lean / regular / dense, staged / global probe, any min_idx).  p_host and
+ * wfrag must not be NULL (the adjacency-only form is dagr_l1_build with p_host = NULL).  Re-run dagr_l1a_tc_weights whenever the
+ * weights change. */
+#define DAGR_L1A_TC_WFRAG_FLOATS 1536  /* 6 k-steps x 32 lanes x 2 n-tiles x 4 */
+int dagr_l1a_tc_weights(const dagr_l1a_params_t *p_host, float *wfrag_host /* f32[DAGR_L1A_TC_WFRAG_FLOATS] */);
+int dagr_l1_build_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
+                     const uint32_t *xyb, const float *feat_s, const dagr_l1a_params_t *p_host, const float *wfrag,
+                     const int32_t *flags, int min_idx, int32_t *nbr, uint16_t *off, uint32_t *cellmask, float *xa,
+                     int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
+
 /* conv_b + skip + activation, fused with pool1's per-voxel max (a9, pooling.py:74-75):
  * poolmax u32[B*ny1*nx1][16] holds order-preserving encodings (0 = empty; MUST be zero on entry).
  * x1 (optional, may be NULL) receives the per-node activations [N,16] in sorted order. */
