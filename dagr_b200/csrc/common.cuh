@@ -55,6 +55,36 @@ __device__ __forceinline__ int img_plane(const ImgPlanes &pl, int b)
 // blocksums[dagr_scan_blocks(n)]
 int scan_exclusive(const int *in, int *out, int64_t n, int *blocksums, cudaStream_t st);
 
+// exclusive prefix sum of one int per thread over the CTA (every thread must call it); *total = the CTA's sum.
+// smem: int[32] of the caller's shared memory.
+__device__ __forceinline__ int block_exclusive_scan(int v, int *total, int *smem /*[32]*/)
+{
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int incl = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        int o = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= d) incl += o;
+    }
+    if (lane == 31) smem[wid] = incl;
+    __syncthreads();
+    if (wid == 0) {
+        int w = (lane < (blockDim.x >> 5)) ? smem[lane] : 0;
+        int wi = w;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            int o = __shfl_up_sync(0xffffffffu, wi, d);
+            if (lane >= d) wi += o;
+        }
+        smem[lane] = wi - w;            // exclusive warp offsets
+        if (lane == 31) *total = wi;
+    }
+    __syncthreads();
+    int res = smem[wid] + incl - v;
+    __syncthreads();
+    return res;
+}
+
 // xa rows are stored half-major [2][N][8]; inside each 32-byte half-row the two 16-byte chunks are swapped when bit 2 of
 // the row index is set.  A staged copy of the rows (TMA keeps them contiguous) then spreads a warp's random row gathers
 // over all eight 16-byte bank groups instead of four (LDS.128 conflict degree ~3.4 -> ~2.3).

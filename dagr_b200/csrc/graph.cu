@@ -18,36 +18,8 @@
 extern "C" int64_t dagr_scan_blocks(int64_t n) { return (n + SCAN_TILE - 1) / SCAN_TILE; }
 
 // ------------------------------------------------------------------------------------------------
-// exclusive scan (int32), three small kernels.  out may alias in.
+// exclusive scan (int32), three small kernels.  out may alias in.  (block_exclusive_scan: common.cuh)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int block_exclusive_scan(int v, int *total, int *smem /*[32]*/)
-{
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    int incl = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        int o = __shfl_up_sync(0xffffffffu, incl, d);
-        if (lane >= d) incl += o;
-    }
-    if (lane == 31) smem[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        int w = (lane < (blockDim.x >> 5)) ? smem[lane] : 0;
-        int wi = w;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            int o = __shfl_up_sync(0xffffffffu, wi, d);
-            if (lane >= d) wi += o;
-        }
-        smem[lane] = wi - w;            // exclusive warp offsets
-        if (lane == 31) *total = wi;
-    }
-    __syncthreads();
-    int res = smem[wid] + incl - v;
-    __syncthreads();
-    return res;
-}
-
 __global__ void __launch_bounds__(SCAN_THREADS) k_scan_reduce(const int *__restrict__ in, int64_t n, int *__restrict__ blocksums)
 {
     __shared__ int sm[32];

@@ -45,6 +45,17 @@ __global__ void k_ds_rank(const int32_t *__restrict__ cell, const int32_t *__res
     sorted[s + r] = i;
 }
 
+// one event of one output pixel (scripts/downsample_events.py:115-122): the accumulator step of both down-samplers
+// (k_ds_walk, k_stream_ingest).  pi = the event's polarity +-1, denom = fx * fy.  Returns whether the event passes.
+__device__ __forceinline__ bool ds_step(float &acc, float pi, double denom)
+{
+    // numba: float32 array element += float64 expression  ->  sum in float64, rounded once to float32
+    acc = (float)((double)acc + (double)pi * 1.0 / denom);
+    const bool pass = fabsf(acc) >= 1.f;
+    if (pass) acc = __fsub_rn(acc, pi);
+    return pass;
+}
+
 __global__ void k_ds_walk(const int8_t *__restrict__ p, const int32_t *__restrict__ start, const int32_t *__restrict__ sorted,
                           int cells, double denom, float *__restrict__ change_map, uint8_t *__restrict__ mask)
 {
@@ -55,12 +66,7 @@ __global__ void k_ds_walk(const int8_t *__restrict__ p, const int32_t *__restric
     float acc = change_map[c];
     for (int k = s; k < e; k++) {
         const int i = sorted[k];
-        const float pi = (float)p[i];
-        // numba: float32 array element += float64 expression  ->  sum in float64, rounded once to float32
-        acc = (float)((double)acc + (double)pi * 1.0 / denom);
-        const bool pass = fabsf(acc) >= 1.f;
-        if (pass) acc = __fsub_rn(acc, pi);
-        mask[i] = pass ? 1 : 0;
+        mask[i] = ds_step(acc, (float)p[i], denom) ? 1 : 0;
     }
     change_map[c] = acc;
 }
@@ -173,6 +179,118 @@ extern "C" int dagr_ingest_events(const uint16_t *x, const uint16_t *y, const in
     k_ing_emit<<<dagr_div_up(N, 256), 256, 0, st>>>(flag, pos, N, x, y, t, p, p_is_01, (float)W, (float)H, T, tlast, sample,
                                                     batch_out, pos_out, feat_out);
     DAGR_CUDA(cudaMemcpyAsync(n_out, pos + N, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));   // total kept
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// streaming ingest: the raw sensor chunks of S cameras -> the stage of dagr_stream_push[_multi], inside a captured step.
+// One CTA per stream.  The chunk's events are sorted in shared memory by the key cell << 14 | arrival index (a bitonic
+// sort; the keys are unique, so the order is (cell, arrival), i.e. stable), then one thread per run of equal cells walks
+// its events in arrival order with ds_step, carrying that cell's accumulator in change_map.  The kept events are then
+// compacted in arrival order, cropped to y / fy < crop_h, and written as (x / fx, y / fy, t, 2p - 1) rows.  At fx = fy = 1
+// the walk is skipped: every event passes (0 + p reaches +-1) and the accumulator returns to 0, so the map stays 0.
+// Every launch dimension is a constant of the detector; the counts are read from the raw stage on the device.
+// ------------------------------------------------------------------------------------------------
+#define SI_THREADS 1024
+#define SI_IDX_BITS 14                          // arrival index bits of a sort key: DAGR_INGEST_MAX_RAW = 2^14
+#define SI_IDX_MASK ((1u << SI_IDX_BITS) - 1u)
+
+static_assert(DAGR_INGEST_MAX_RAW == (1 << SI_IDX_BITS), "the sort key holds the arrival index in SI_IDX_BITS bits");
+static_assert((int64_t)DAGR_INGEST_MAX_CELLS << SI_IDX_BITS == (1ll << 32), "the sort key is 32 bits");
+
+__global__ void __launch_bounds__(SI_THREADS) k_stream_ingest(const int32_t *__restrict__ raw, int S, int max_raw, int kcap, int fx,
+                                                              int fy, int ow, int oh, int crop_h, float *__restrict__ change_map,
+                                                              int32_t *__restrict__ stage, int max_chunk)
+{
+    extern __shared__ uint32_t si_key[];                                 // [kcap] sort keys
+    uint8_t *keep = reinterpret_cast<uint8_t *>(si_key + kcap);          // [max_raw] the down-sampler's verdict, by arrival
+    __shared__ int sm[32];
+    __shared__ int tot;
+    const int s = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    const int4 hdr = reinterpret_cast<const int4 *>(raw)[s];
+    const int n = min(max(hdr.x, 0), max_raw);
+    const int eo = min(max(hdr.z, 0), S * max_raw - n);                  // a bad offset cannot read past the stage
+    const int2 *ev = reinterpret_cast<const int2 *>(raw + 4 * S) + eo;
+    if (fx * fy > 1) {
+        float *cm = change_map + (int64_t)s * ow * oh;
+        const int np2 = n <= 1 ? n : 1 << (32 - __clz(n - 1));
+        for (int i = tid; i < np2; i += nt) {
+            uint32_t key = 0xffffffffu;                                  // padding sorts last
+            if (i < n) {
+                const uint32_t w = (uint32_t)ev[i].x;
+                // the reference would index out of bounds; clamp as k_ds_hist does
+                const int xl = min((int)(w & 0xffffu) / fx, ow - 1), yl = min((int)((w >> 16) & 0x7fffu) / fy, oh - 1);
+                key = (uint32_t)(yl * ow + xl) << SI_IDX_BITS | (uint32_t)i;
+            }
+            si_key[i] = key;
+        }
+        __syncthreads();
+        for (int k = 2; k <= np2; k <<= 1)
+            for (int j = k >> 1; j > 0; j >>= 1) {
+                for (int q = tid; q < (np2 >> 1); q += nt) {
+                    const int i = 2 * q - (q & (j - 1)), l = i + j;
+                    const uint32_t a = si_key[i], b = si_key[l];
+                    if ((a > b) == ((i & k) == 0)) { si_key[i] = b; si_key[l] = a; }
+                }
+                __syncthreads();
+            }
+        const double denom = (double)(fx * fy);
+        for (int r = tid; r < n; r += nt) {
+            const uint32_t c = si_key[r] >> SI_IDX_BITS;
+            if (r > 0 && (si_key[r - 1] >> SI_IDX_BITS) == c) continue;   // not the first event of its cell
+            float acc = cm[c];
+            int q = r;
+            do {                                                         // a hot cell is walked serially, as in the reference
+                const int i = (int)(si_key[q] & SI_IDX_MASK);
+                keep[i] = ds_step(acc, ev[i].x < 0 ? 1.f : -1.f, denom) ? 1 : 0;
+            } while (++q < n && (si_key[q] >> SI_IDX_BITS) == c);
+            cm[c] = acc;
+        }
+    } else {
+        for (int i = tid; i < n; i += nt) keep[i] = 1;
+    }
+    __syncthreads();
+    const int obase = s * max_chunk;
+    int4 *out = reinterpret_cast<int4 *>(stage + 4 * S) + obase;
+    int kept = 0;
+    for (int b0 = 0; b0 < n; b0 += nt) {                                 // stable compaction, nt events per round
+        const int i = b0 + tid;
+        int f = 0, xo = 0, yo = 0;
+        int2 e = make_int2(0, 0);
+        if (i < n) {
+            e = ev[i];
+            const uint32_t w = (uint32_t)e.x;
+            xo = (int)(w & 0xffffu) / fx;                                // (x / fx).astype(uint16), downsample_events.py:103
+            yo = (int)((w >> 16) & 0x7fffu) / fy;
+            f = keep[i] && yo < crop_h;                                  // crop, dsec_data.py:142-143
+        }
+        const int off = block_exclusive_scan(f, &tot, sm);
+        if (f) out[kept + off] = make_int4(xo, yo, e.y, e.x < 0 ? 1 : -1);
+        kept += tot;
+    }
+    if (tid == 0) reinterpret_cast<int4 *>(stage)[s] = make_int4(kept, hdr.y, obase, hdr.w);
+}
+
+extern "C" int dagr_stream_ingest(const int32_t *raw_stage, int streams, int max_raw, int fx, int fy, int out_w, int out_h, int crop_h,
+                                  float *change_map, int32_t *stage, int max_chunk, void *stream)
+{
+    DAGR_CHECK_ARG(raw_stage && change_map && stage, "null argument");
+    DAGR_CHECK_ARG(streams >= 1 && streams <= 127, "streams must be in [1, 127]");
+    DAGR_CHECK_ARG(fx >= 1 && fy >= 1, "fx and fy must be >= 1");
+    DAGR_CHECK_ARG(out_w >= 1 && out_h >= 1 && (int64_t)out_w * fx <= (1 << 16) && (int64_t)out_h * fy <= (1 << 15),
+                   "bad geometry: the raw record holds x in 16 bits and y in 15 bits (out_w * fx <= 65536, out_h * fy <= 32768)");
+    DAGR_CHECK_ARG(fx * fy == 1 || (int64_t)out_w * out_h <= DAGR_INGEST_MAX_CELLS,
+                   "more than 2^18 output cells: the sort key is cell << 14 | arrival index in 32 bits");
+    DAGR_CHECK_ARG(crop_h >= 1 && crop_h <= out_h, "crop_h must be in [1, out_h]");
+    DAGR_CHECK_ARG(max_raw >= 1 && max_raw <= DAGR_INGEST_MAX_RAW, "max_raw must be in [1, 16384] (shared-memory sort)");
+    DAGR_CHECK_ARG(max_raw <= max_chunk, "max_raw must be <= max_chunk (a stream's kept events fill its stage slot)");
+    int kcap = 1;
+    while (kcap < max_raw) kcap <<= 1;
+    const size_t smem = (size_t)kcap * sizeof(uint32_t) + (size_t)(max_raw + 15) / 16 * 16;
+    DAGR_CUDA(dagr_allow_smem(k_stream_ingest, smem));
+    k_stream_ingest<<<streams, SI_THREADS, smem, (cudaStream_t)stream>>>(raw_stage, streams, max_raw, kcap, fx, fy, out_w, out_h, crop_h,
+                                                                         change_map, stage, max_chunk);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

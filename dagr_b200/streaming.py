@@ -24,6 +24,9 @@ of two frame slots, and every chunk's step (one replay of that slot's graph) rea
 FusionMultiStreamDetector does the same for S hybrid cameras in one step: the frame slots of all cameras are planes of one
 array, and each camera's plane travels in its stage header, so one graph serves every combination of slots.
 
+With sensor=(width, height) any of the four takes the camera's raw events: dagr_stream_ingest runs the reference's 2x
+down-sampler, the crop, 2p - 1 and the time rebase in front of the push, inside the same replay (_RingDetector).
+
 Why the event level is recomputed over the window instead of patched: evicting an event changes the neighbour lists of
 every node it fed (the K cap admits the next candidate of the spiral), i.e. of the window's oldest 10 ms -- and their
 activations feed the next 10 ms.  At 50 k live events the per-voxel kernels take ~0.1 ms for the WHOLE window
@@ -44,6 +47,9 @@ from . import _lib
 RING_CTL = 8                          # ints per stream in a control block (DAGR_RING_CTL)
 MAX_STREAMS = 127                     # dagr_stream_push_multi: 1 <= S <= 127
 MAX_RING_SLOTS = 1 << 24              # S * capacity < 2^24: sorted positions are packed in 24 bits
+MAX_RAW = 16384                       # dagr_stream_ingest: raw events per stream per step (DAGR_INGEST_MAX_RAW)
+MAX_CELLS = 1 << 18                   # dagr_stream_ingest: cells of a down-sampling grid (DAGR_INGEST_MAX_CELLS)
+_I32_MIN, _I32_MAX = -(1 << 31), (1 << 31) - 1
 
 
 def _pow2_at_least(n: int) -> int:
@@ -59,14 +65,22 @@ class _RingDetector:
     detections and of the control block.  The first two steps run eagerly (they allocate every buffer of the step); the
     second is followed by one capture, and every later step is one replay of that CUDA graph.  A detector whose steps read
     different buffers (FusionStreamingDetector's two frame slots) keeps one graph per _graph_key(); a key first used after
-    the warm-up is captured right after its first (eager) step."""
+    the warm-up is captured right after its first (eager) step.
 
-    def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device):
+    Raw sensor mode (`sensor=(width, height)`): the detector takes the camera's own events and runs the reference's 2x
+    down-sampler (scripts/downsample_events.py), the crop to the model's height (dsec_data.py:142-143), the polarity 2p - 1
+    and the time rebase inside the step, as one more kernel in front of the push (dagr_stream_ingest).  The pinned stage
+    then holds the raw chunks (8 bytes per event, pack_raw_stage) and the device stage the push reads is the ingest's
+    output.  Each stream keeps its down-sampler's change map on the device and its time base (the first raw timestamp
+    after a reset) on the host."""
+
+    def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device, sensor=None, p_is_01=True):
         self.model, self.eng = model, model.engine
         self.lib = self.eng.lib
         self.W, self.H = int(model.width), int(model.height)
         self.window_us, self.max_chunk = int(window_us), int(max_chunk)
         self.cap = _pow2_at_least(capacity)
+        self._check_sensor(sensor, p_is_01)
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("dagr_b200: streaming needs a CUDA device (no CPU fallback)")
@@ -76,9 +90,21 @@ class _RingDetector:
         self.pos = torch.zeros((n, 3), dtype=torch.int32, device=dev)
         self.feat = torch.zeros(n, dtype=torch.float32, device=dev)
         nstage = 4 * streams + 4 * streams * self.max_chunk
-        self.stage_h = torch.zeros(nstage, dtype=torch.int32).pin_memory()
         self.stage_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
-        self._stage_np = self.stage_h.numpy()
+        if self.sensor is None:
+            self.stage_h = torch.zeros(nstage, dtype=torch.int32).pin_memory()
+            self._stage_np = self.stage_h.numpy()
+        else:
+            nraw = 4 * streams + 2 * streams * self.max_chunk
+            self.stage_h = torch.zeros(nraw, dtype=torch.int32).pin_memory()        # the raw stage
+            self.raw_d = torch.zeros(nraw, dtype=torch.int32, device=dev)
+            self._raw_np = self.stage_h.numpy()
+            ow, oh = self.grid
+            self._cmap = torch.zeros((streams, oh, ow), dtype=torch.float32, device=dev)
+            self._tbase = [None] * streams    # per stream: raw timestamp of rebased time 0
+            self._tend = [None] * streams     # per stream: raw t_end of its last step
+            self._nraw = [0] * streams        # per stream: raw events of the last submitted chunk
+        self._nstreams = streams
         self.stream = torch.cuda.Stream(device=dev)
         self.graphs = {}                      # _graph_key() -> captured step
         self._res_h = None
@@ -102,13 +128,48 @@ class _RingDetector:
         """(plane table, stride) when image_feats / image_outs are per-stream plane arrays (forward_events), else None."""
         return None
 
+    def _stage_planes(self):
+        """word 3 of each stream's stage header: the frame plane of its step (FusionMultiStreamDetector), None for no frames."""
+        return None
+
     def _push(self):
         raise NotImplementedError
+
+    def _check_sensor(self, sensor, p_is_01):
+        """raw sensor mode: the down-sampling factor and grid of a `sensor` = (width, height) stream for this model."""
+        self.sensor = None
+        if sensor is None:
+            if not p_is_01:
+                raise ValueError("p_is_01 describes raw sensor chunks: it needs sensor=(width, height)")
+            return
+        sw, sh = (int(v) for v in sensor)
+        scale = sw // self.W
+        if scale < 1 or sw != scale * self.W or sh < scale * self.H:
+            raise ValueError(f"sensor {sw}x{sh} for a {self.W}x{self.H} model: the sensor width must be an integer multiple "
+                             f"scale * {self.W} and the height at least scale * {self.H}")
+        ow, oh = sw // scale, sh // scale
+        if scale > 1 and ow * oh > MAX_CELLS:
+            raise ValueError(f"down-sampling grid {ow}x{oh} has more than 2^18 cells (the ingest's 32-bit sort key)")
+        if sw > 1 << 16 or sh > 1 << 15:
+            raise ValueError(f"sensor {sw}x{sh}: the raw record holds x < 2^16 and y < 2^15")
+        if not 1 <= self.max_chunk <= MAX_RAW:
+            raise ValueError(f"max_chunk={self.max_chunk}: with a sensor it bounds the raw events per stream and step, "
+                             f"1 <= max_chunk <= {MAX_RAW} (the ingest sorts a chunk in shared memory)")
+        self.sensor, self.scale, self.grid, self.p_is_01 = (sw, sh), scale, (ow, oh), bool(p_is_01)
+
+    def _ingest(self):
+        ow, oh = self.grid
+        self.eng._run("stream_ingest", self.lib.dagr_stream_ingest, _lib.ptr(self.raw_d), self._nstreams, self.max_chunk, self.scale,
+                      self.scale, ow, oh, self.H, _lib.ptr(self._cmap), _lib.ptr(self.stage_d), self.max_chunk, _lib.stream_ptr())
 
     def _enqueue(self):
         """one streaming step on the current stream (eager or under capture)."""
         m, eng = self.model, self.eng
-        self.stage_d.copy_(self.stage_h, non_blocking=True)
+        if self.sensor is None:
+            self.stage_d.copy_(self.stage_h, non_blocking=True)
+        else:
+            self.raw_d.copy_(self.stage_h, non_blocking=True)
+            self._ingest()
         self._push()
         eng.launches += 2
         feats, outs = self._image_inputs()
@@ -159,7 +220,10 @@ class _RingDetector:
     def _state(self, s: int):
         self._done.synchronize()
         c = self._res_h[2][RING_CTL * s:RING_CTL * (s + 1)]
-        return dict(head=int(c[0]), live=int(c[1]), evicted=int(c[2]), appended=int(c[3]), overflow=bool(c[4]))
+        st = dict(head=int(c[0]), live=int(c[1]), evicted=int(c[2]), appended=int(c[3]), overflow=bool(c[4]))
+        if self.sensor is not None:
+            st["raw"] = self._nraw[s]                                 # raw events of the chunk; `appended` = the kept ones
+        return st
 
     def _live(self, s: int):
         self._done.synchronize()
@@ -168,23 +232,95 @@ class _RingDetector:
         idx = s * self.cap + ((head + torch.arange(n, device=self.dev)) & (self.cap - 1))
         return self.pos[idx], self.feat[idx]
 
+    # ---- raw sensor mode ---------------------------------------------------------------------------------------------
+    def _raw_rows(self, s, c):
+        """check one raw chunk (x, y, t int64 us, p) of stream s and rebase its time; raises ValueError, touches nothing."""
+        x, y, t, p = (np.asarray(a) for a in c)
+        n = len(t)
+        if not len(x) == len(y) == len(p) == n:
+            raise ValueError(f"stream {s}: x, y, t, p of different lengths {len(x)}, {len(y)}, {n}, {len(p)}")
+        if n > self.max_chunk:
+            raise ValueError(f"stream {s}: raw chunk of {n} events exceeds max_chunk={self.max_chunk}")
+        sw, sh = self.sensor
+        if int(x.min()) < 0 or int(x.max()) >= sw or int(y.min()) < 0 or int(y.max()) >= sh:
+            raise ValueError(f"stream {s}: event coordinates outside the {sw}x{sh} sensor")
+        lo, hi = int(p.min()), int(p.max())
+        if (lo < 0 or hi > 1) if self.p_is_01 else (lo < -1 or hi > 1 or np.count_nonzero(p) != n):
+            raise ValueError(f"stream {s}: polarities must be in " + ("{0, 1} (p_is_01=True)" if self.p_is_01 else "{-1, +1} (p_is_01=False)"))
+        base = self._tbase[s] if self._tbase[s] is not None else int(t[0])
+        tr = t.astype(np.int64) - base
+        if int(tr.min()) < _I32_MIN or int(tr.max()) > _I32_MAX:
+            raise ValueError(f"stream {s}: timestamps {int(t.min())}..{int(t.max())} us leave the int32 range of the stream's time "
+                             f"base {base} us (reset the stream to start a new base)")
+        return base, (x, y, tr, p)
+
+    def _submit_raw(self, chunks, t_end):
+        """raw sensor mode: check and rebase every chunk, then fill the raw stage and step.  Nothing is touched (no device
+        work, no time base) when a chunk is refused."""
+        rows, t_cut, bases, ends = [], [], list(self._tbase), list(self._tend)
+        for s, c in enumerate(chunks):
+            row = None
+            if c is not None and len(c[2]) > 0:
+                bases[s], row = self._raw_rows(s, c)
+            rows.append(row)
+            te = None if t_end is None else t_end[s]
+            if te is None:
+                te = int(row[2][-1]) + bases[s] if row is not None else ends[s]
+            ends[s] = te
+            cut = _I32_MIN if te is None or bases[s] is None else int(te) - bases[s] - self.window_us
+            if cut > _I32_MAX:
+                raise ValueError(f"stream {s}: t_end {te} us leaves the int32 range of the stream's time base {bases[s]} us")
+            t_cut.append(max(cut, _I32_MIN))
+        if self._done is not None:
+            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
+        self._nraw = pack_raw_stage(self._raw_np, rows, t_cut, self.max_chunk, planes=self._stage_planes())
+        self._tbase, self._tend = bases, ends
+        self._step()
+
+    def _forget(self, s=None):
+        """raw sensor mode: stream s (every stream when None) starts over: zero change map, no time base."""
+        if self.sensor is None:
+            return
+        for k in (range(self._nstreams) if s is None else [s]):
+            self._cmap[k].zero_()
+            self._tbase[k] = self._tend[k] = None
+            self._nraw[k] = 0
+
+    def _change_map(self, s: int):
+        if self.sensor is None:
+            raise RuntimeError("the change map is the raw sensor mode's down-sampler state (sensor=...)")
+        if self._done is not None:
+            self._done.synchronize()
+        return self._cmap[s].cpu()
+
 
 class StreamingDetector(_RingDetector):
-    """det = StreamingDetector(model, window_us=50_000); det.push(x, y, t, p) -> list with one dict(boxes, scores, labels)."""
+    """det = StreamingDetector(model, window_us=50_000); det.push(x, y, t, p) -> list with one dict(boxes, scores, labels).
+
+    With sensor=(width, height) the chunks are the camera's raw events (x, y uint16 at the sensor's resolution, t int64 us,
+    p in {0, 1}, or +-1 with p_is_01=False), down-sampled, cropped and rebased inside the step (see _RingDetector); the
+    model's width must divide the sensor's.  max_chunk then bounds the raw events of a chunk (<= 16384)."""
 
     _B, _ring_streams = 1, None
 
-    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None, sensor=None,
+                 p_is_01: bool = True):
         if model.backbone.use_image:
             raise NotImplementedError("streaming mode drives the events-only model")
-        self._setup(model, 1, window_us, max_chunk, capacity, device)
+        self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
         self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
 
     # ------------------------------------------------------------------------------------------------------------
     def reset(self):
+        """forget the live window (raw sensor mode: and the change map and time base)."""
         if self._done is not None:
             self._done.synchronize()
         self.ctl.zero_()
+        self._forget()
+
+    def change_map(self):
+        """raw sensor mode: host copy of the down-sampler's accumulators f32[h, w] after the last step (for tests)."""
+        return self._change_map(0)
 
     def _push(self):
         _lib.check(self.lib.dagr_stream_push(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
@@ -205,7 +341,13 @@ class StreamingDetector(_RingDetector):
     def submit(self, x, y, t, p, t_end=None):
         """enqueue one chunk (host arrays: pixel x, y, timestamp t in us (int32 range, non-decreasing across pushes),
         polarity -1/+1).  `t_end` = end of the chunk's time slice (default: its last timestamp); events older than
-        t_end - window_us leave the live window.  Returns immediately; `result()` blocks on the step."""
+        t_end - window_us leave the live window.  Returns immediately; `result()` blocks on the step.
+        Raw sensor mode: x, y at the sensor's resolution, t int64 us, p in {0, 1} (or +-1, p_is_01=False), t_end in raw
+        time; a chunk over max_chunk, outside the sensor or whose rebased time leaves int32 raises ValueError before any
+        device work."""
+        if self.sensor is not None:
+            self._submit_raw([(x, y, t, p)], None if t_end is None else [t_end])
+            return
         if self._done is not None:
             self._done.synchronize()                                  # the stage / result buffers of the previous step are free
         if t_end is None:
@@ -224,7 +366,8 @@ class StreamingDetector(_RingDetector):
 
     @property
     def window_state(self):
-        """(head slot, live events, evicted by the last step, appended by the last step, overflow flag) of the last finished step."""
+        """(head slot, live events, evicted by the last step, appended by the last step, overflow flag) of the last finished step;
+        raw sensor mode adds `raw`, the raw events of the chunk (`appended` counts the kept ones)."""
         return self._state(0)
 
     def live_window(self):
@@ -362,9 +505,10 @@ class FusionStreamingDetector(StreamingDetector):
     pending frame is usable, so the next step uses it.  The first step waits for the first frame.  After every step the
     detections equal model(data) over the live window with the image of the frame that frame_state reports."""
 
-    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+    def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None, sensor=None,
+                 p_is_01: bool = True):
         _check_fusion_model(model, "FusionStreamingDetector", "StreamingDetector")
-        self._setup(model, 1, window_us, max_chunk, capacity, device)
+        self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
         self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
         self.frame_stream = torch.cuda.Stream(device=self.dev)
         self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
@@ -443,6 +587,35 @@ def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int, planes=None):
     return ns
 
 
+def pack_raw_stage(stage: np.ndarray, chunks, t_cut, max_raw: int, planes=None):
+    """write the raw stage of dagr_stream_ingest into the int32 array `stage` (>= 4*S + 2*S*max_raw entries): header [S][4] =
+    {n_raw, t_cut, event offset, plane}, then 8-byte records of all streams back to back, (x | y << 16 | (p > 0) << 31,
+    t).  chunks[s] = (x, y, t, p) host arrays or None: x < 2^16, y < 2^15, t in the stream's rebased time (int32 range),
+    p in {0, 1} or {-1, +1} (bit 31 = the event is positive, i.e. 2p - 1 = +1 or p = +1).  t_cut[s] in rebased time,
+    planes[s] as in pack_stage.  Vectorised numpy; returns the per-stream event counts."""
+    S = len(chunks)
+    ns = [0 if c is None else len(c[2]) for c in chunks]
+    for s, n in enumerate(ns):
+        if n > max_raw:
+            raise ValueError(f"stream {s}: raw chunk of {n} events exceeds max_raw={max_raw}")
+    if len(stage) < 4 * S + 2 * S * max_raw:
+        raise ValueError(f"stage of {len(stage)} ints is smaller than 4*S + 2*S*max_raw = {4 * S + 2 * S * max_raw}")
+    hdr = stage[:4 * S].reshape(S, 4)
+    ev = stage[4 * S:4 * S + 2 * S * max_raw].reshape(S * max_raw, 2)
+    o = 0
+    for s, (c, n) in enumerate(zip(chunks, ns)):
+        hdr[s] = (n, int(t_cut[s]), o, 0 if planes is None else int(planes[s]))
+        if n:
+            x, y, t, p = c
+            w = (np.asarray(x).astype(np.uint32) | np.asarray(y).astype(np.uint32) << 16
+                 | (np.asarray(p) > 0).astype(np.uint32) << 31)
+            e = ev[o:o + n]
+            e[:, 0] = w.view(np.int32)
+            e[:, 1] = np.asarray(t).astype(np.int32)
+        o += n
+    return ns
+
+
 class MultiStreamDetector(_RingDetector):
     """S independent event cameras on one GPU: det = MultiStreamDetector(model, streams=S, window_us=50_000);
     det.push([(x, y, t, p) or None per stream]) -> S dicts(boxes, scores, labels).
@@ -452,14 +625,18 @@ class MultiStreamDetector(_RingDetector):
     CUDA graph replay.  Each stream's detections are those of a StreamingDetector fed the same chunks, and those of the
     synchronous forward over its live window.  All streams share the model (and so its W x H); each keeps its own time base,
     and timestamps only need to be non-decreasing within a stream.  One step advances every stream: a stream with nothing
-    new passes None or an empty chunk."""
+    new passes None or an empty chunk.
 
-    def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+    sensor=(width, height) takes every camera's raw events, as StreamingDetector does; each camera keeps its own change map
+    and time base, and reset(s) restarts both."""
+
+    def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None,
+                 sensor=None, p_is_01: bool = True):
         if model.backbone.use_image:
             raise NotImplementedError("streaming mode drives the events-only model")
-        self._setup_streams(model, streams, window_us, max_chunk, capacity, device)
+        self._setup_streams(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
 
-    def _setup_streams(self, model, streams, window_us, max_chunk, capacity, device):
+    def _setup_streams(self, model, streams, window_us, max_chunk, capacity, device, sensor=None, p_is_01=True):
         S = int(streams)
         if not 1 <= S <= MAX_STREAMS:
             raise ValueError(f"streams={streams}: 1 <= streams <= {MAX_STREAMS}")
@@ -469,7 +646,7 @@ class MultiStreamDetector(_RingDetector):
         if not 1 <= int(max_chunk) <= cap:
             raise ValueError(f"max_chunk={max_chunk} must be in [1, capacity={cap}]")
         self.S = self._B = self._ring_streams = S
-        self._setup(model, S, window_us, max_chunk, cap, device)
+        self._setup(model, S, window_us, max_chunk, cap, device, sensor, p_is_01)
         self.ctl = torch.zeros((S + 1) * RING_CTL, dtype=torch.int32, device=self.dev)
         self.stage_bytes = 4 * self.stage_h.numel()
 
@@ -479,28 +656,39 @@ class MultiStreamDetector(_RingDetector):
                    "stream_push_multi")
 
     def reset(self, stream=None):
-        """forget the live window of one stream (the others keep theirs) or of all streams."""
+        """forget the live window of one stream (the others keep theirs) or of all streams (raw sensor mode: and its change
+        map and time base)."""
         if self._done is not None:
             self._done.synchronize()
         if stream is None:
             self.ctl.zero_()
+            self._forget()
         else:
             s = int(stream)
             if not 0 <= s < self.S:
                 raise IndexError(f"stream {stream} out of range [0, {self.S})")
             self.ctl[RING_CTL * s:RING_CTL * (s + 1)].zero_()
+            self._forget(s)
+
+    def change_map(self, s: int):
+        """raw sensor mode: host copy of stream s's down-sampler accumulators f32[h, w] after the last step (for tests)."""
+        return self._change_map(int(s))
 
     @torch.no_grad()
     def submit(self, chunks, t_end=None):
         """enqueue one step: chunks[s] = (x, y, t, p) host arrays of stream s (as StreamingDetector.submit) or None.
         t_end[s] = end of stream s's time slice (None, or t_end=None: its last timestamp, or for an empty chunk the previous
-        end).  Returns immediately; `result()` blocks on the step."""
+        end).  Returns immediately; `result()` blocks on the step.  Raw sensor mode: raw chunks and raw t_end, as
+        StreamingDetector.submit."""
         S = self.S
         if len(chunks) != S:
             raise ValueError(f"{len(chunks)} chunks for {S} streams")
         if t_end is not None and len(t_end) != S:
             raise ValueError(f"{len(t_end)} t_end values for {S} streams")
-        cs = [None if c is None or len(c[2]) == 0 else tuple(np.asarray(a) for a in c) for c in chunks]
+        if self.sensor is not None:
+            self._submit_raw(chunks, t_end)
+            return
+        cs =[None if c is None or len(c[2]) == 0 else tuple(np.asarray(a) for a in c) for c in chunks]
         for s, c in enumerate(cs):
             if c is not None and len(c[2]) > self.max_chunk:
                 raise ValueError(f"stream {s}: chunk of {len(c[2])} events exceeds max_chunk={self.max_chunk}")
@@ -533,10 +721,6 @@ class MultiStreamDetector(_RingDetector):
         """(pos int32[n,3], polarity f32[n]) of stream s's live window in arrival order (host sync; for tests)."""
         return self._live(s)
 
-    def _stage_planes(self):
-        """word 3 of each stream's stage header: the frame plane of its step (FusionMultiStreamDetector), None for no frames."""
-        return None
-
 
 class FusionMultiStreamDetector(MultiStreamDetector):
     """S hybrid (image + events) cameras on one GPU: MultiStreamDetector with a camera frame per stream.
@@ -559,11 +743,13 @@ class FusionMultiStreamDetector(MultiStreamDetector):
 
     Frame policy, per camera: a step uses the camera's newest frame whose copy has finished (a non-blocking event query);
     a camera's first step waits on the device for its first frame; submit raises RuntimeError before any device work while
-    some camera has never had a frame.  reset() keeps the frames."""
+    some camera has never had a frame.  reset() keeps the frames.  With sensor=(width, height) the event chunks are the
+    cameras' raw events (see MultiStreamDetector); frames stay at the model's resolution."""
 
-    def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None):
+    def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None,
+                 sensor=None, p_is_01: bool = True):
         _check_fusion_model(model, "FusionMultiStreamDetector", "MultiStreamDetector")
-        self._setup_streams(model, streams, window_us, max_chunk, capacity, device)
+        self._setup_streams(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
         self.frame_stream = torch.cuda.Stream(device=self.dev)
         self._planes = None                   # (image_feats, image_outs) as plane arrays [2S, ...]
         self._cams = [_CameraFrames(self, lambda j, f, o, s=s: self._plane_dst(2 * s + j, f, o)) for s in range(self.S)]

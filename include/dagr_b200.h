@@ -511,6 +511,32 @@ int dagr_ingest_events(const uint16_t *x, const uint16_t *y, const int64_t *t, c
                        int32_t *blocksums, unsigned long long *tlast, int32_t *batch_out, int32_t *pos_out,
                        float *feat_out, int32_t *n_out, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Streaming ingest: raw sensor chunks of S cameras -> the stage of dagr_stream_push / dagr_stream_push_multi, as one
+ * launch of S CTAs whose grid depends on no count (capturable in the streaming step's CUDA graph; no host sync).
+ *
+ *   raw_stage i32[4*S + 2*S*max_raw] on the DEVICE: header [S][4] = {n_raw, t_cut, event offset, plane}, then the raw
+ *         events of all streams back to back, 8 bytes each: word 0 = x | y << 16 | polarity << 31 (x < 2^16, y < 2^15,
+ *         polarity bit 1 = +1, 0 = -1), word 1 = t in the stream's rebased time (int32 us).  Stream s's n_raw events start
+ *         at event `offset`.  t_cut is in rebased time; t_cut and the plane word are carried to the output unchanged.
+ *   change_map f32[S][out_h][out_w] (in/out): the per-output-pixel accumulators of the down-sampler, carried from step to
+ *         step (scripts/downsample_events.py:146-153); zero a stream's map to restart it (the script starts every recording
+ *         with change_map = None).  Untouched when fx = fy = 1.
+ *   stage i32[4*S + 4*S*max_chunk] (out): header {n_kept, t_cut, s * max_chunk, plane}, then stream s's kept events at
+ *         event s * max_chunk as (x / fx, y / fy, t, polarity +-1) rows: the input of the push.
+ * Per stream, in arrival order: output cell (min(x / fx, out_w - 1), min(y / fy, out_h - 1)); the reference's per-cell
+ * accumulator walk (the arithmetic of dagr_downsample_events, the same device function); the kept events in arrival
+ * order; crop to y / fy < crop_h (dsec_data.py:142-143).  A cell with many events in one chunk is walked serially.
+ * Limits (DAGR_E_ARG before anything is launched): no null pointer; 1 <= S <= 127; fx, fy >= 1; out_w * fx <= 2^16 and
+ * out_h * fy <= 2^15 (the raw record); out_w * out_h <= DAGR_INGEST_MAX_CELLS unless fx = fy = 1 (32-bit sort key
+ * cell << 14 | arrival index); 1 <= crop_h <= out_h; 1 <= max_raw <= DAGR_INGEST_MAX_RAW (the sort runs in shared
+ * memory); max_raw <= max_chunk.  n_raw is clamped to [0, max_raw] on the device.
+ * ------------------------------------------------------------------------------------------- */
+#define DAGR_INGEST_MAX_RAW   16384       /* raw events per stream per step                           */
+#define DAGR_INGEST_MAX_CELLS (1 << 18)   /* output cells of a down-sampling grid (fx * fy > 1)       */
+int dagr_stream_ingest(const int32_t *raw_stage, int streams, int max_raw, int fx, int fy, int out_w, int out_h, int crop_h,
+                       float *change_map, int32_t *stage, int max_chunk, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
