@@ -80,6 +80,7 @@ _SIGS = {
     "dagr_compact_events": (C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, p, p, p, p, p, p, p, p, p]),
     "dagr_ingest_events": (C.c_int, [p, p, p, p, i64, C.c_int, C.c_int, C.c_int, C.c_int, i64, C.c_int, p, p, p, p, p, p, p, p, p]),
     "dagr_stream_ingest": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int, p]),
+    "dagr_frame_preprocess": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, p]),
     "dagr_denormalize_pos": (C.c_int, [p, i64, C.c_int, C.c_int, C.c_int, p, p]),
     "dagr_prepare_events": (C.c_int, [p, p, p, C.c_int, i64, C.c_int, C.c_int, C.c_int, p, p, p, p]),
     "dagr_graph_sort": (C.c_int, [C.POINTER(Geom), p, p, p, i64, p, p, p, p, p, p, p, p, p, p, p]),

@@ -294,3 +294,88 @@ extern "C" int dagr_stream_ingest(const int32_t *raw_stage, int streams, int max
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }
+
+// ------------------------------------------------------------------------------------------------
+// camera frames (dsec_data.py:149-154): crop to scale * H rows, cv2.resize(INTER_CUBIC) by the integer factor `scale`,
+// HWC -> CHW, in one pass.  At an integer factor the cubic is integer arithmetic (oracle/ref_frame.py): the source
+// coordinate of output pixel d is (d + 0.5) * s - 0.5.  Odd s: fraction 0, the output is source pixel s * d + (s - 1) / 2.
+// Even s: sx = s * d + s / 2 - 1, fraction 0.5, taps sx - 1 .. sx + 2 clamped to the cropped frame with weights
+// [-3, 19, 19, -3] / 32 per axis; the 16-tap sum (units of 1/1024) is rounded half to even and saturated.  No floating
+// point, so no contraction or summation order can change a bit.  The f32 form maps the byte through `lut` (the caller's
+// torch u8 -> f32 / 255.0 table, so the bits are those of `.float() / 255.0` on the device).
+// One thread per output pixel, all three channels.  The taps are read straight from global memory: at s = 2 neighbouring
+// threads share half their taps and the L1 serves the repeats; at s >= 4 no tap is shared.  A 640x480 frame is 0.9 MB.
+// ------------------------------------------------------------------------------------------------
+#define FP_THREADS 128
+
+__device__ __forceinline__ int fp_round(int v)                          // round(v / 1024) half to even, saturated to [0, 255]
+{
+    int q = v >> 10;                                                     // floor
+    const int r = v & 1023;
+    q += (r > 512) | ((r == 512) & (q & 1));
+    return min(max(q, 0), 255);
+}
+
+template <bool F32>
+__global__ void __launch_bounds__(FP_THREADS) k_frame_preprocess(const uint8_t *__restrict__ src, int sh, int sw, int s, int H, int W,
+                                                                 uint8_t *__restrict__ out_u8, float *__restrict__ out_f32,
+                                                                 const float *__restrict__ lut)
+{
+    const int x = blockIdx.x * FP_THREADS + threadIdx.x, y = blockIdx.y, f = blockIdx.z;
+    if (x >= W) return;
+    const uint8_t *img = src + (int64_t)f * sh * sw * 3;
+    int v[3];
+    if (s & 1) {
+        const uint8_t *px = img + ((int64_t)(s * y + (s - 1) / 2) * sw + s * x + (s - 1) / 2) * 3;
+        v[0] = __ldg(px); v[1] = __ldg(px + 1); v[2] = __ldg(px + 2);
+    } else {
+        const int wt[4] = {-3, 19, 19, -3};
+        const int ch = s * H;                                            // the cropped frame's rows: the border cv2 replicates
+        const int sy = s * y + s / 2 - 1, sx = s * x + s / 2 - 1;
+        int cx[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) cx[k] = 3 * min(max(sx - 1 + k, 0), sw - 1);
+        int acc[3] = {0, 0, 0};
+#pragma unroll
+        for (int ky = 0; ky < 4; ky++) {
+            const uint8_t *row = img + (int64_t)min(max(sy - 1 + ky, 0), ch - 1) * sw * 3;
+            int hs[3] = {0, 0, 0};
+#pragma unroll
+            for (int kx = 0; kx < 4; kx++)
+#pragma unroll
+                for (int c = 0; c < 3; c++) hs[c] += wt[kx] * (int)__ldg(row + cx[kx] + c);
+#pragma unroll
+            for (int c = 0; c < 3; c++) acc[c] += wt[ky] * hs[c];
+        }
+#pragma unroll
+        for (int c = 0; c < 3; c++) v[c] = fp_round(acc[c]);
+    }
+    const int64_t plane = (int64_t)H * W, o = (int64_t)f * 3 * plane + (int64_t)y * W + x;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        if (F32) out_f32[o + c * plane] = __ldg(lut + v[c]);
+        else out_u8[o + c * plane] = (uint8_t)v[c];
+    }
+}
+
+extern "C" int dagr_frame_preprocess(const uint8_t *frames, int nframes, int src_h, int src_w, int scale, int out_h, int out_w,
+                                     uint8_t *out_u8, float *out_f32, const float *lut, void *stream)
+{
+    DAGR_CHECK_ARG(frames, "null frames");
+    DAGR_CHECK_ARG((out_u8 != nullptr) != (out_f32 != nullptr), "exactly one of out_u8 / out_f32 must be given");
+    DAGR_CHECK_ARG(!out_f32 || lut, "null lut: the f32 output needs the 256-entry u8 -> f32 table");
+    DAGR_CHECK_ARG(nframes >= 1 && nframes <= 65535, "nframes must be in [1, 65535]");
+    DAGR_CHECK_ARG(out_w >= 1 && out_h >= 1 && out_h <= 65535, "out_w >= 1 and 1 <= out_h <= 65535");
+    DAGR_CHECK_ARG(scale >= 1, "scale must be >= 1");
+    DAGR_CHECK_ARG((int64_t)src_w == (int64_t)scale * out_w, "src_w must equal scale * out_w (integer factors only)");
+    DAGR_CHECK_ARG((int64_t)src_h >= (int64_t)scale * out_h, "src_h must be >= scale * out_h (the crop keeps scale * out_h rows)");
+    DAGR_CHECK_ARG((int64_t)src_h * src_w * 3 < (1ll << 31), "a frame must hold fewer than 2^31 bytes");
+    const dim3 grid(dagr_div_up(out_w, FP_THREADS), out_h, nframes);
+    if (out_f32)
+        k_frame_preprocess<true><<<grid, FP_THREADS, 0, (cudaStream_t)stream>>>(frames, src_h, src_w, scale, out_h, out_w, nullptr, out_f32, lut);
+    else
+        k_frame_preprocess<false><<<grid, FP_THREADS, 0, (cudaStream_t)stream>>>(frames, src_h, src_w, scale, out_h, out_w, out_u8, nullptr,
+                                                                                 nullptr);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}

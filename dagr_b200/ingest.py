@@ -9,6 +9,8 @@ Host-side mirror of the reference's CPU functions for this step, same names and 
       dsec_data.py:141-147,177-179 + data/utils.py:6-20 + utils/buffers.py:33-44 + ev_tgn.py:11-16 fused
   collate(samples, width, height, time_window)
       the duck-typed Batch `DAGR.forward` accepts (pos_denorm shortcut, ev_tgn.py:12-13)
+  preprocess_image(frames_u8, height, width, scale)
+      dsec_data.py:149-154 -- crop, cv2.resize(INTER_CUBIC) by an integer factor and HWC -> CHW, bit for bit
 
 Everything runs in hand-written kernels (csrc/ingest.cu) on the current stream; there is no CPU fallback.
 """
@@ -104,6 +106,37 @@ def ingest_window(events: Dict[str, torch.Tensor], width: int, height: int, time
                                       _lib.ptr(n_out), _lib.stream_ptr()), "ingest_events")
     M = int(n_out.item())
     return batch_o[:M], pos_o[:M], feat_o[:M]
+
+
+def frame_lut(device) -> torch.Tensor:
+    """f32[256] u8 -> f32 table of the float frame form: torch's own `.float() / 255.0` on the device, so a table lookup
+    has the bits of the division format_data applies."""
+    return torch.arange(256, dtype=torch.uint8, device=device).float() / 255.0
+
+
+def preprocess_frames(frames: torch.Tensor, height: int, width: int, scale: int, lut: Optional[torch.Tensor] = None):
+    """dagr_frame_preprocess on the current stream: u8 [F, sh, sw, 3] contiguous CUDA -> u8 [F, 3, height, width], or f32
+    through `lut` (frame_lut) when it is given.  Raises RuntimeError on a shape the kernel refuses."""
+    lib = _lib.load()
+    _lib.require_cuda(frames, "frames")
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+        raise ValueError(f"frames {tuple(frames.shape)} {frames.dtype}: expected u8 [F, sh, sw, 3]")
+    F, sh, sw = (int(v) for v in frames.shape[:3])
+    out = torch.empty((F, 3, height, width), dtype=torch.uint8 if lut is None else torch.float32, device=frames.device)
+    _lib.check(lib.dagr_frame_preprocess(_lib.ptr(frames), F, sh, sw, int(scale), int(height), int(width),
+                                         _lib.ptr(out) if lut is None else None, None if lut is None else _lib.ptr(out),
+                                         _lib.ptr(lut), _lib.stream_ptr()), "frame_preprocess")
+    return out
+
+
+def preprocess_image(frames_u8: torch.Tensor, height: int, width: int, scale: int) -> torch.Tensor:
+    """the reference's DSEC.preprocess_image (dsec_data.py:149-154) on the device: camera frames u8 [F, sh, sw, 3] or
+    [sh, sw, 3] (HWC, CUDA, the camera's channel order, passed through) -> u8 [F, 3, height, width], the `data.image` the
+    model was trained on.  Rows from scale * height on are cropped, then the frame is resized by the integer factor
+    `scale` with OpenCV's INTER_CUBIC arithmetic (sw == scale * width, sh >= scale * height; other ratios raise).  No host
+    sync."""
+    f = frames_u8.unsqueeze(0) if frames_u8.dim() == 3 else frames_u8
+    return preprocess_frames(f.contiguous(), height, width, scale)
 
 
 def collate(samples, width: int, height: int, time_window: int = 1_000_000) -> EventBatch:

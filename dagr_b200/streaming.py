@@ -25,7 +25,9 @@ FusionMultiStreamDetector does the same for S hybrid cameras in one step: the fr
 array, and each camera's plane travels in its stage header, so one graph serves every combination of slots.
 
 With sensor=(width, height) any of the four takes the camera's raw events: dagr_stream_ingest runs the reference's 2x
-down-sampler, the crop, 2p - 1 and the time rebase in front of the push, inside the same replay (_RingDetector).
+down-sampler, the crop, 2p - 1 and the time rebase in front of the push, inside the same replay (_RingDetector).  The two fusion
+detectors also take the camera's own frames with raw_frames=True: dagr_frame_preprocess runs the reference's frame crop and
+cubic down-sizing in front of the image trunk (_CameraFrames).
 
 Why the event level is recomputed over the window instead of patched: evicting an event changes the neighbour lists of
 every node it fed (the K cap admits the next candidate of the spiral), i.e. of the window's oldest 10 ms -- and their
@@ -41,7 +43,7 @@ import time
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, ingest
 
 
 RING_CTL = 8                          # ints per stream in a control block (DAGR_RING_CTL)
@@ -383,6 +385,18 @@ def _check_fusion_model(model, name: str, events_only_class: str):
         raise NotImplementedError("--no_events: the model has no event path to stream")
 
 
+def _check_raw_frames(raw_frames, sensor):
+    if raw_frames and sensor is None:
+        raise ValueError("raw_frames takes the camera's own frames: it needs sensor=(width, height)")
+
+
+def _frame_setup(det, raw_frames):
+    """frame handling of the fusion detectors after _setup: the frame stream, and with raw_frames the u8 -> f32 table."""
+    det.frame_stream = torch.cuda.Stream(device=det.dev)
+    det.raw_frames = bool(raw_frames)
+    det._frame_lut = ingest.frame_lut(det.dev) if det.raw_frames else None
+
+
 class _CameraFrames:
     """The frames of one hybrid camera, for the fusion detectors: two frame slots, the frame pending in the trunk, the frame
     in use, and the done-event of the last step that read each slot.
@@ -391,7 +405,10 @@ class _CameraFrames:
     replays) on the detector's frame stream and copies its five feature maps and CNN head maps into the slot the steps do
     not use; `slot_dst(slot, feats, outs)` names the destination tensors of a slot (allocating them on first use).  Two
     hazards are ordered on the device: the copy into a slot waits for the last step that read that slot, and the branch's
-    static output buffers are overwritten (by the next frame or a model(data) call) only after the copy out of them."""
+    static output buffers are overwritten (by the next frame or a model(data) call) only after the copy out of them.
+
+    With the detector's raw_frames a frame is the camera's u8 [sensor_h, sensor_w, 3]; the pinned stage is sized for it,
+    and dagr_frame_preprocess turns it into the trunk's f32 [1, 3, H, W] where `.float() / 255.0` runs otherwise."""
 
     def __init__(self, det, slot_dst):
         self.det, self.slot_dst = det, slot_dst
@@ -409,11 +426,25 @@ class _CameraFrames:
             image = torch.from_numpy(np.ascontiguousarray(image))
         if image.dtype != torch.uint8:
             raise ValueError(f"frame dtype {image.dtype}: expected uint8 (raw camera pixels)")
+        if d.raw_frames:
+            sw, sh = d.sensor
+            if tuple(image.shape) != (sh, sw, 3):
+                raise ValueError(f"frame of shape {tuple(image.shape)}: raw_frames takes the camera's frame, [{sh}, {sw}, 3] "
+                                 f"(rows, columns, channels)")
+            return image.unsqueeze(0)
         if image.dim() == 4 and image.shape[0] == 1:
             image = image[0]
         if image.dim() != 3 or tuple(image.shape) != (3, d.H, d.W):
             raise ValueError(f"frame of shape {tuple(image.shape)}: expected [3, {d.H}, {d.W}] or [1, 3, {d.H}, {d.W}]")
         return image.unsqueeze(0)
+
+    def to_float(self, img):
+        """the checked frame, on the device, -> the f32 [1, 3, H, W] the trunk reads, on the current stream: `.float() / 255.0`
+        as format_data, or with raw_frames the reference's crop and resize fused with it (dagr_frame_preprocess)."""
+        d = self.det
+        if d.raw_frames:
+            return ingest.preprocess_frames(img.contiguous(), d.H, d.W, d.scale, d._frame_lut)
+        return img.float() / 255.0
 
     def promote(self):
         pend, self.pending = self.pending, None
@@ -437,7 +468,7 @@ class _CameraFrames:
         br = m._image_branch
         cur = torch.cuda.current_stream(det.dev)
         if img.is_cuda:
-            x = img.to(det.dev).float() / 255.0                        # on the caller's stream, ordered with its writes
+            x = self.to_float(img.to(det.dev))                         # on the caller's stream, ordered with its writes
         elif self.img_h is None:
             self.img_h = torch.empty(img.shape, dtype=torch.uint8).pin_memory()
         with torch.cuda.stream(fs):
@@ -446,7 +477,7 @@ class _CameraFrames:
                 if self.h2d is not None:
                     self.h2d.synchronize()                             # the previous frame's upload has left the pinned stage
                 self.img_h.copy_(img)
-                x = self.img_h.to(det.dev, non_blocking=True).float() / 255.0    # as format_data
+                x = self.to_float(self.img_h.to(det.dev, non_blocking=True))
                 self.h2d = torch.cuda.Event()
                 self.h2d.record(fs)
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -503,14 +534,20 @@ class FusionStreamingDetector(StreamingDetector):
     Which frame a step uses: the newest frame whose trunk has finished when the chunk is submitted (a non-blocking event
     query).  Chunks keep flowing on the previous frame while the next frame's trunk runs; sync_frame() blocks until the
     pending frame is usable, so the next step uses it.  The first step waits for the first frame.  After every step the
-    detections equal model(data) over the live window with the image of the frame that frame_state reports."""
+    detections equal model(data) over the live window with the image of the frame that frame_state reports.
+
+    raw_frames=True (with sensor=(width, height)): set_frame takes the camera's own frame, u8 [height, width, 3] (HWC, the
+    camera's channel order), and the reference's crop + cv2.resize(INTER_CUBIC) by the integer factor width / W
+    (dsec_data.py:149-154) runs on the device, bit for bit (dagr_frame_preprocess); the detections then equal those of
+    the same detector fed the frame prepared by the reference's loader."""
 
     def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None, sensor=None,
-                 p_is_01: bool = True):
+                 p_is_01: bool = True, raw_frames: bool = False):
         _check_fusion_model(model, "FusionStreamingDetector", "StreamingDetector")
+        _check_raw_frames(raw_frames, sensor)
         self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
         self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
-        self.frame_stream = torch.cuda.Stream(device=self.dev)
+        _frame_setup(self, raw_frames)
         self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
         self._cam = _CameraFrames(self, self._slot_dst)
         self._overlapped = False              # the last submitted step ran while a newer frame's trunk was in flight
@@ -529,7 +566,8 @@ class FusionStreamingDetector(StreamingDetector):
     @torch.no_grad()
     def set_frame(self, image, t_us=None):
         """start a new frame: the trunk runs on the device, this returns without waiting for it.  `image` u8 [3,H,W] or
-        [1,3,H,W] (host or device); `t_us` is the caller's timestamp of the frame, reported back by frame_state.
+        [1,3,H,W], with raw_frames the camera's u8 [sensor_h, sensor_w, 3] (host or device; another shape or dtype raises
+        ValueError before any device work); `t_us` is the caller's timestamp of the frame, reported back by frame_state.
         Returns the frame id (0, 1, 2, ...).  A frame still pending is waited for and becomes current first."""
         return self._cam.set(image, t_us)
 
@@ -744,13 +782,15 @@ class FusionMultiStreamDetector(MultiStreamDetector):
     Frame policy, per camera: a step uses the camera's newest frame whose copy has finished (a non-blocking event query);
     a camera's first step waits on the device for its first frame; submit raises RuntimeError before any device work while
     some camera has never had a frame.  reset() keeps the frames.  With sensor=(width, height) the event chunks are the
-    cameras' raw events (see MultiStreamDetector); frames stay at the model's resolution."""
+    cameras' raw events (see MultiStreamDetector); frames stay at the model's resolution unless raw_frames=True, which
+    takes every camera's own u8 [height, width, 3] frames (see FusionStreamingDetector)."""
 
     def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None,
-                 sensor=None, p_is_01: bool = True):
+                 sensor=None, p_is_01: bool = True, raw_frames: bool = False):
         _check_fusion_model(model, "FusionMultiStreamDetector", "MultiStreamDetector")
+        _check_raw_frames(raw_frames, sensor)
         self._setup_streams(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self.frame_stream = torch.cuda.Stream(device=self.dev)
+        _frame_setup(self, raw_frames)
         self._planes = None                   # (image_feats, image_outs) as plane arrays [2S, ...]
         self._cams = [_CameraFrames(self, lambda j, f, o, s=s: self._plane_dst(2 * s + j, f, o)) for s in range(self.S)]
         self._overlapped = [False] * self.S   # per camera: the last step ran while a newer frame of it was in flight

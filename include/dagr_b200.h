@@ -537,6 +537,23 @@ int dagr_ingest_events(const uint16_t *x, const uint16_t *y, const int64_t *t, c
 int dagr_stream_ingest(const int32_t *raw_stage, int streams, int max_raw, int fx, int fy, int out_w, int out_h, int crop_h,
                        float *change_map, int32_t *stage, int max_chunk, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Camera frames: the reference's DSEC.preprocess_image (dsec_data.py:149-154) on the device, bit for bit: crop to
+ * scale * out_h rows, cv2.resize(INTER_CUBIC) by the integer factor `scale`, HWC -> CHW.
+ *
+ *   frames u8[nframes][src_h][src_w][3] contiguous, the camera's channel order (passed through unchanged).
+ *   out_u8 u8[nframes][3][out_h][out_w] (the reference's data.image), or
+ *   out_f32 f32[nframes][3][out_h][out_w] = lut[byte]; lut f32[256] on the device, built by the caller as
+ *         torch.arange(256, dtype=uint8).float() / 255.0 (the bits of format_data's `.float() / 255.0`).
+ * Exactly one of out_u8 / out_f32 is given.  Integer arithmetic: odd scale picks source pixel scale * d + (scale - 1) / 2;
+ * even scale sums taps sx - 1 .. sx + 2 (sx = scale * d + scale / 2 - 1, clamped to the cropped frame) with weights
+ * [-3, 19, 19, -3] / 32 per axis and rounds the sum half to even, saturated to [0, 255].
+ * Limits (DAGR_E_ARG before anything is launched): no null frames / lut (with out_f32); 1 <= nframes <= 65535;
+ * out_w >= 1, 1 <= out_h <= 65535; scale >= 1; src_w == scale * out_w; src_h >= scale * out_h; src_h * src_w * 3 < 2^31.
+ * ------------------------------------------------------------------------------------------- */
+int dagr_frame_preprocess(const uint8_t *frames, int nframes, int src_h, int src_w, int scale, int out_h, int out_w,
+                          uint8_t *out_u8, float *out_f32, const float *lut, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
