@@ -129,7 +129,20 @@ _SIGS = {
                                        C.c_int, C.c_int, p]),
     "dagr_sample_features_planes": (C.c_int, [p, C.c_int, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p,
                                               C.c_int, C.c_int, p]),
-    "dagr_masked_lin": (C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p]),
+    # bf16 NHWC forms of the image-sampling calls (map as const void *, with its C)
+    "dagr_l1_x0_image_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, p]),
+    "dagr_l1_x0_image_live_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p, p]),
+    "dagr_l1_x0_image_planes_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p, p]),
+    "dagr_voxel_sample_max_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, C.c_int, C.c_int, p]),
+    "dagr_voxel_sample_max_inc_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int,
+                                                 C.c_int, C.c_int, p]),
+    "dagr_voxel_sample_max_planes_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p,
+                                                    C.c_int, C.c_int, C.c_int, p]),
+    "dagr_sample_features_bf16": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p, C.c_int, C.c_int,
+                                            p]),
+    "dagr_sample_features_planes_bf16": (C.c_int, [p, C.c_int, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int,
+                                                   p, C.c_int, C.c_int, p]),
+    "dagr_masked_lin":(C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p]),
     "dagr_masked_inplace_bn": (C.c_int, [p, i64, p, p, p, p, p, p, C.c_int, f32, p]),
     "dagr_masked_isdiff": (C.c_int, [p, i64, p, p, C.c_int, f32, f32, p]),
 }

@@ -89,6 +89,7 @@ class AsyncDAGR:
             raise NotImplementedError("--no_events: the model has no event path to update incrementally")
         self.model = model
         self.use_image = bool(model.backbone.use_image)
+        self.image_precision = model.image_precision          # read once: a later change on the model does not reach this wrapper
         self.state = StreamState()
         self._batch = self._pos = self._feat = None
         self._hb = self._hp = self._hf = None
@@ -115,7 +116,7 @@ class AsyncDAGR:
             m._image_branch = ImageBranch(m)
         br = m._image_branch
         cur = torch.cuda.current_stream(image.device)
-        feats, outs, (_, ev2) = br.run(image, use_graph=m.image_graph)
+        feats, outs, (_, ev2) = br.run(image, use_graph=m.image_graph, precision=self.image_precision)
         cur.wait_event(ev2)                                          # the copy waits for the whole branch
         if (self._feats is None or [tuple(f.shape) for f in feats] != [tuple(f.shape) for f in self._feats]
                 or {k: [tuple(t.shape) for t in v] for k, v in outs.items()} != {k: [tuple(t.shape) for t in v] for k, v in self._outs.items()}):

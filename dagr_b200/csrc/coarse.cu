@@ -849,9 +849,10 @@ extern "C" int dagr_postprocess_nms(const float *pred, int B, int A, int nc, flo
 // ------------------------------------------------------------------------------------------------
 // a8 sample_features: 3-D bilinear grid_sample, align_corners=True, zero padding (net.py:193-221)
 // PLANES: img_in is a plane array [pl.n][C][h][w]; node i samples plane img_plane(pl, bidx[i]) as a batch of one.
+// MT: the map format (common.cuh: float = NCHW, __nv_bfloat16 = NHWC, where the lanes' channels of a tap are one coalesced run).
 // ------------------------------------------------------------------------------------------------
-template <bool PLANES>
-__global__ void k_sample_features(const float *__restrict__ img_in, int Bi_in, int C, int h, int w,
+template <bool PLANES, typename MT = float>
+__global__ void k_sample_features(const MT *__restrict__ img_in, int Bi_in, int C, int h, int w,
                                   const float *__restrict__ posx, const float *__restrict__ posy,
                                   const int32_t *__restrict__ bidx, int64_t n, float width, float height,
                                   float *__restrict__ out, int ldo, int c0, const ImgPlanes pl)
@@ -860,7 +861,7 @@ __global__ void k_sample_features(const float *__restrict__ img_in, int Bi_in, i
     const int lane = threadIdx.x & 31;
     if (i >= n) return;
     const int Bi = PLANES ? 1 : Bi_in;
-    const float *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, bidx[i]) * C * h * w : img_in;
+    const MT *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, bidx[i]) * C * h * w : img_in;
     // normalise exactly as _sample_features does, then unnormalise as grid_sample(align_corners=True)
     float gx = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posx[i], width)), width - 1.f), 1.f);
     float gy = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posy[i], height)), height - 1.f), 1.f);
@@ -889,7 +890,7 @@ __global__ void k_sample_features(const float *__restrict__ img_in, int Bi_in, i
                     const int x = x0 + dx;
                     const float wx = dx ? tx : 1.f - tx;
                     if (x < 0 || x >= w) continue;
-                    acc += img[(((int64_t)z * C + c) * h + y) * w + x] * (wx * wy * wz);
+                    acc += map_ld(img, C, h, w, z, c, y, x) * (wx * wy * wz);
                 }
             }
         }
@@ -920,6 +921,38 @@ extern "C" int dagr_sample_features_planes(const float *img, int nplanes, const 
     k_sample_features<true><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, 1, C, h, w, posx, posy, bidx, n, (float)width,
                                                                                (float)height, out, ldo, c0,
                                                                                ImgPlanes{plane, plane_stride, nplanes});
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+// bf16 NHWC forms (include/dagr_b200.h): the same kernel with MT = __nv_bfloat16
+extern "C" int dagr_sample_features_bf16(const void *img, int Bi, int C, int h, int w, const float *posx, const float *posy,
+                                         const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
+                                         void *stream)
+{
+    DAGR_CHECK_ARG(img && posx && posy && bidx && out, "null argument");
+    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(Bi >= 1 && C >= 1 && h >= 1 && w >= 1, "the map must have Bi, C, h, w >= 1");
+    if (n == 0) return DAGR_OK;
+    k_sample_features<false, __nv_bfloat16><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
+        static_cast<const __nv_bfloat16 *>(img), Bi, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0, ImgPlanes{});
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_sample_features_planes_bf16(const void *img, int nplanes, const int32_t *plane, int plane_stride, int C, int h, int w,
+                                                const float *posx, const float *posy, const int32_t *bidx, int64_t n, int width,
+                                                int height, float *out, int ldo, int c0, void *stream)
+{
+    DAGR_CHECK_ARG(img && posx && posy && bidx && out && plane, "null argument");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C >= 1 && h >= 1 && w >= 1, "the map must have C, h, w >= 1");
+    if (n == 0) return DAGR_OK;
+    k_sample_features<true, __nv_bfloat16><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
+        static_cast<const __nv_bfloat16 *>(img), 1, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0,
+        ImgPlanes{plane, plane_stride, nplanes});
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

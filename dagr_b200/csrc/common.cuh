@@ -1,6 +1,7 @@
 // common.cuh -- shared helpers for libdagr_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -49,6 +50,26 @@ struct ImgPlanes {
 __device__ __forceinline__ int img_plane(const ImgPlanes &pl, int b)
 {
     return min(max(__ldg(pl.plane + (int64_t)b * pl.stride), 0), pl.n - 1);
+}
+
+// Map formats of the image-sampling kernels (their map element type MT): fp32 maps are NCHW [B][C][h][w] (the TF32 image
+// branch), bf16 maps are NHWC [B][h][w][C] (the bf16 image branch's channels_last taps).  map_ld / map_ldg (read-only path)
+// return element (z, c, y, x) of either as fp32; bf16 -> fp32 is exact, so a bf16 map samples to the bits of its fp32 upcast.
+__device__ __forceinline__ float map_ld(const float *__restrict__ m, int C, int h, int w, int z, int c, int y, int x)
+{
+    return m[(((int64_t)z * C + c) * h + y) * w + x];
+}
+__device__ __forceinline__ float map_ld(const __nv_bfloat16 *__restrict__ m, int C, int h, int w, int z, int c, int y, int x)
+{
+    return __bfloat162float(m[(((int64_t)z * h + y) * w + x) * C + c]);
+}
+__device__ __forceinline__ float map_ldg(const float *__restrict__ m, int C, int h, int w, int z, int c, int y, int x)
+{
+    return __ldg(m + (((int64_t)z * C + c) * h + y) * w + x);
+}
+__device__ __forceinline__ float map_ldg(const __nv_bfloat16 *__restrict__ m, int C, int h, int w, int z, int c, int y, int x)
+{
+    return __bfloat162float(__ldg(m + (((int64_t)z * h + y) * w + x) * C + c));
 }
 
 // exclusive prefix sum of n ints (graph.cu); blocksums: int[dagr_scan_blocks(n) + 2]; the grand total is left in

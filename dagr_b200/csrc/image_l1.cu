@@ -2,6 +2,7 @@
 // events (net.py:15-17,193-221), conv_block1.conv_block1 on 1+16+2 input channels, and the per-voxel max
 // of the 64-channel samples that are concatenated before pool1 (net.py:128-131).  sm_90a.
 #include "common.cuh"
+#include <type_traits>
 
 // grid_sample(align_corners=True) of one (x, y, batch) position: weights and corner offsets, mirroring
 // _sample_features (net.py:207-221): normalise with the event resolution, unnormalise with the map size.
@@ -24,7 +25,8 @@ __device__ __forceinline__ Bilin bilin_setup(float posx, float posy, int b, floa
     r.tx = ix - x0f; r.ty = iy - y0f; r.tz = iz - z0f;
     return r;
 }
-__device__ __forceinline__ float bilin_sample(const float *__restrict__ img, int Bi, int C, int h, int w, int c, const Bilin &q)
+template <typename MT>
+__device__ __forceinline__ float bilin_sample(const MT *__restrict__ img, int Bi, int C, int h, int w, int c, const Bilin &q)
 {
     float acc = 0.f;
 #pragma unroll
@@ -42,7 +44,7 @@ __device__ __forceinline__ float bilin_sample(const float *__restrict__ img, int
                 const int x = q.x0 + dx;
                 const float wx = dx ? q.tx : 1.f - q.tx;
                 if (x < 0 || x >= w) continue;
-                acc += __ldg(img + (((int64_t)z * C + c) * h + y) * w + x) * (wx * wy * wz);
+                acc += map_ldg(img, C, h, w, z, c, y, x) * (wx * wy * wz);
             }
         }
     }
@@ -57,9 +59,10 @@ __device__ __forceinline__ float bilin_sample(const float *__restrict__ img, int
 // past posx0 / posy0; the rows they would fill are never read (conv_a_image, conv_b and voxel_sample_max walk the voxels'
 // [start[cell], start[cell+1]) ranges, which lie below the total), so they are simply skipped.  live == NULL: the bound is N.
 // PLANES: img0 is a plane array [pl.n][16][h][w] and the event of sample b samples plane img_plane(pl, b) as a batch of one.
-template <bool PLANES>
+// MT: the map format (common.cuh: float = NCHW, __nv_bfloat16 = NHWC).
+template <bool PLANES, typename MT = float>
 __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ live, const uint32_t *__restrict__ xyb,
-                              const float *__restrict__ img0, int h, int w, float *__restrict__ x0, const ImgPlanes pl)
+                              const MT *__restrict__ img0, int h, int w, float *__restrict__ x0, const ImgPlanes pl)
 {
     // 4 threads per node: thread q computes image channels 4q..4q+3 = one 16-byte chunk of a row
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -70,7 +73,7 @@ __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__r
     const int x = wd & 0xfff, y = (wd >> 12) & 0xfff, b = wd >> 24;
     const float px = g.posx0[x], py = g.posy0[y];
     const int Bi = PLANES ? 1 : g.B;
-    const float *img = PLANES ? img0 + (int64_t)img_plane(pl, b) * 16 * h * w : img0;
+    const MT *img = PLANES ? img0 + (int64_t)img_plane(pl, b) * 16 * h * w : img0;
     const Bilin bl = bilin_setup(px, py, PLANES ? 0 : b, (float)g.W, (float)g.H, Bi, h, w);
     float f[4];
 #pragma unroll
@@ -117,6 +120,58 @@ extern "C" int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const in
     return DAGR_OK;
 }
 
+// bf16 NHWC forms (include/dagr_b200.h): the same kernel with the map loader of MT = __nv_bfloat16.  live == NULL selects the
+// unbounded form, nplanes == 0 the non-plane one.
+static int x0_image_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const void *img0, int h, int w,
+                         int nplanes, const int32_t *plane, int plane_stride, float *x0, void *stream)
+{
+    const __nv_bfloat16 *img = static_cast<const __nv_bfloat16 *>(img0);
+    if (nplanes)
+        k_l1_x0_image<true, __nv_bfloat16><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(
+            *g, N, start, xyb, img, h, w, x0, ImgPlanes{plane, plane_stride, nplanes});
+    else
+        k_l1_x0_image<false, __nv_bfloat16><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(
+            *g, N, start, xyb, img, h, w, x0, ImgPlanes{});
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_l1_x0_image_bf16(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s, const void *img0,
+                                     int C, int h, int w, float *x0, void *stream)
+{
+    (void)feat_s;
+    DAGR_CHECK_ARG(g && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C == 16 && h >= 1 && w >= 1, "the conv1 tap is [B, h, w, 16] with h, w >= 1");
+    if (N == 0) return DAGR_OK;
+    return x0_image_bf16(g, N, nullptr, xyb, img0, h, w, 0, nullptr, 0, x0, stream);
+}
+
+extern "C" int dagr_l1_x0_image_live_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                                          const void *img0, int C, int h, int w, float *x0, void *stream)
+{
+    (void)feat_s;
+    DAGR_CHECK_ARG(g && start && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C == 16 && h >= 1 && w >= 1, "the conv1 tap is [B, h, w, 16] with h, w >= 1");
+    if (N == 0) return DAGR_OK;
+    return x0_image_bf16(g, N, start, xyb, img0, h, w, 0, nullptr, 0, x0, stream);
+}
+
+extern "C" int dagr_l1_x0_image_planes_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
+                                            const float *feat_s, const void *img0, int C, int h, int w, int nplanes, const int32_t *plane,
+                                            int plane_stride, float *x0, void *stream)
+{
+    (void)feat_s;
+    DAGR_CHECK_ARG(g && start && xyb && img0 && plane && x0, "null argument (only feat_s may be NULL)");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C == 16 && h >= 1 && w >= 1, "the conv1 tap is [nplanes, h, w, 16] with h, w >= 1");
+    if (N == 0) return DAGR_OK;
+    return x0_image_bf16(g, N, start, xyb, img0, h, w, nplanes, plane, plane_stride, x0, stream);
+}
+
 // ------------------------------------------------------------------------------------------------
 // per-voxel max of image features sampled at the voxel's events (net.py:128-131 before pool1): one CTA per voxel.
 // All events of a voxel sample a small window of the feature map (voxel extent x map/sensor scale, + 1), so the window
@@ -127,8 +182,8 @@ extern "C" int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const in
 #define VS_THREADS 128
 #define VS_SMEM_FLOATS 10240                                            // 40 KB: e.g. 2 planes x 6 x 6 x 128 channels
 
-template <bool STAGED>
-__device__ __forceinline__ float vs_sample(const float *__restrict__ img, const float *s_patch, int Bi, int C, int h, int w,
+template <bool STAGED, typename MT>
+__device__ __forceinline__ float vs_sample(const MT *__restrict__ img, const float *s_patch, int Bi, int C, int h, int w,
                                            int c, const Bilin &q, int zb, int yb, int xb, int ph, int pw)
 {
     float acc = 0.f;
@@ -148,7 +203,7 @@ __device__ __forceinline__ float vs_sample(const float *__restrict__ img, const 
                 const float wx = dx ? q.tx : 1.f - q.tx;
                 if (x < 0 || x >= w) continue;
                 const float v = STAGED ? s_patch[(((z - zb) * ph + (y - yb)) * pw + (x - xb)) * C + c]
-                                       : __ldg(img + (((int64_t)z * C + c) * h + y) * w + x);
+                                       : map_ldg(img, C, h, w, z, c, y, x);
                 acc += v * (wx * wy * wz);
             }
         }
@@ -165,10 +220,12 @@ template <bool MEAN> __device__ __forceinline__ float vs_comb(float a, float b) 
 // persist and stages nothing.  min_idx == 0 samples every event (the bits of the plain instance) and seeds persist.
 // PLANES: img is a plane array [pl.n][C][h][w]; a voxel of sample b samples plane img_plane(pl, b) as a batch of one, so its
 // window is staged from that one plane (pz = 1).
-template <bool MEAN, bool INC, bool PLANES = false>
+// MT: the map format (common.cuh: float = NCHW, __nv_bfloat16 = NHWC).  The window is staged as fp32 in either, so the sampling
+// below reads the same shared memory in both.
+template <bool MEAN, bool INC, bool PLANES = false, typename MT = float>
 __global__ void __launch_bounds__(VS_THREADS)
 k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
-                   const int2 *__restrict__ ti, const float *__restrict__ img_in, int C, int h, int w, const int min_idx,
+                   const int2 *__restrict__ ti, const MT *__restrict__ img_in, int C, int h, int w, const int min_idx,
                    float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0, const ImgPlanes pl = ImgPlanes{})
 {
     __shared__ float s_m[VS_THREADS / 32][128];
@@ -206,7 +263,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
     };
     // the sampled batch: sample b of the g.B planes of img, or (PLANES) the one plane of sample b as a batch of one (its depth
     // coordinate and batch size are spelled out at each use below: a local copy of g.B changes the plain instances' allocation)
-    const float *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, b) * C * h * w : img_in;
+    const MT *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, b) * C * h * w : img_in;
     // window of the map this voxel's pixels can touch: the sample coordinates are monotone in x / y, so the corner
     // pixels bound it (same arithmetic as the per-event set-up)
     const Bilin lo = bilin_setup(g.posx0[g.vx0[cx]], g.posy0[g.vy0[cy]], PLANES ? 0 : b, (float)g.W, (float)g.H, PLANES ? 1 : g.B, h, w);
@@ -217,9 +274,18 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
     const bool staged = pw > 0 && ph > 0 && pz > 0 && (int64_t)pz * ph * pw * C <= VS_SMEM_FLOATS;   // block-uniform
     if (staged) {
         const int tot = pz * ph * pw * C;
-        for (int i = threadIdx.x; i < tot; i += blockDim.x) {
-            const int x = i % pw, r1 = i / pw, y = r1 % ph, r2 = r1 / ph, c = r2 % C, z = r2 / C;          // x fastest: coalesced
-            s_patch[((z * ph + y) * pw + x) * C + c] = __ldg(img + (((int64_t)(zb + z) * C + c) * h + yb + y) * w + xb + x);
+        if constexpr (std::is_same<MT, float>::value) {
+            for (int i = threadIdx.x; i < tot; i += blockDim.x) {
+                const int x = i % pw, r1 = i / pw, y = r1 % ph, r2 = r1 / ph, c = r2 % C, z = r2 / C;      // x fastest: coalesced
+                s_patch[((z * ph + y) * pw + x) * C + c] = __ldg(img + (((int64_t)(zb + z) * C + c) * h + yb + y) * w + xb + x);
+            }
+        } else {
+            // NHWC: the window has the map's own element order, one contiguous run of pw * C per (z, y) row
+            const int run = pw * C;
+            for (int i = threadIdx.x; i < tot; i += blockDim.x) {
+                const int k = i % run, r = i / run, y = r % ph, z = r / ph;
+                s_patch[i] = __bfloat162float(__ldg(img + (((int64_t)(zb + z) * h + yb + y) * w + xb) * C + k));
+            }
         }
         __syncthreads();
     }
@@ -359,4 +425,66 @@ extern "C" int dagr_voxel_sample_max_planes(const dagr_geom_t *g, int64_t N, con
                                                                                                        w, 0, nullptr, xg, ldx, c0, pl);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
+}
+
+// bf16 NHWC forms (include/dagr_b200.h): the same kernel with MT = __nv_bfloat16.  ti == NULL selects the non-incremental
+// instances, nplanes == 0 the non-plane ones.
+static int voxel_sample_bf16(const dagr_geom_t *g, const int32_t *start, const uint32_t *xyb, const int32_t *ti, const void *img_in,
+                             int C, int h, int w, int min_idx, float *persist, int nplanes, const int32_t *plane, int plane_stride,
+                             float *xg, int ldx, int c0, int pool_mean, void *stream)
+{
+    typedef __nv_bfloat16 bf;
+    const bf *img = static_cast<const bf *>(img_in);
+    const int cells = g->B * g->ny1 * g->nx1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const ImgPlanes pl{plane, plane_stride, nplanes};
+    if (ti)             k_voxel_sample_max<false, true, false, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, (const int2 *)ti, img, C, h, w,
+                                                                                               min_idx, persist, xg, ldx, c0);
+    else if (nplanes && pool_mean) k_voxel_sample_max<true, false, true, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h,
+                                                                                                          w, 0, nullptr, xg, ldx, c0, pl);
+    else if (nplanes)   k_voxel_sample_max<false, false, true, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
+                                                                                                nullptr, xg, ldx, c0, pl);
+    else if (pool_mean) k_voxel_sample_max<true, false, false, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
+                                                                                                nullptr, xg, ldx, c0);
+    else                k_voxel_sample_max<false, false, false, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
+                                                                                                 nullptr, xg, ldx, c0);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+extern "C" int dagr_voxel_sample_max_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const void *img,
+                                          int C, int h, int w, float *xg, int ldx, int c0, int pool_mean, void *stream)
+{
+    DAGR_CHECK_ARG(g && start && xyb && img && xg, "null argument");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
+    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
+    return voxel_sample_bf16(g, start, xyb, nullptr, img, C, h, w, 0, nullptr, 0, nullptr, 0, xg, ldx, c0, pool_mean, stream);
+}
+
+extern "C" int dagr_voxel_sample_max_inc_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                                              const void *img, int C, int h, int w, int min_idx, float *persist, float *xg, int ldx, int c0,
+                                              int pool_mean, void *stream)
+{
+    DAGR_CHECK_ARG(g && start && xyb && ti && img && persist && xg, "null argument");
+    DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
+    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
+    DAGR_CHECK_ARG(!pool_mean, "pool_mean: the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
+    return voxel_sample_bf16(g, start, xyb, ti, img, C, h, w, min_idx, persist, 0, nullptr, 0, xg, ldx, c0, 0, stream);
+}
+
+extern "C" int dagr_voxel_sample_max_planes_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const void *img,
+                                                 int C, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *xg,
+                                                 int ldx, int c0, int pool_mean, void *stream)
+{
+    DAGR_CHECK_ARG(g && start && xyb && img && plane && xg, "null argument");
+    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
+    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
+    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
+    return voxel_sample_bf16(g, start, xyb, nullptr, img, C, h, w, 0, nullptr, nplanes, plane, plane_stride, xg, ldx, c0, pool_mean,
+                             stream);
 }

@@ -46,6 +46,17 @@ def _fill(arr, t: torch.Tensor):
     C.memmove(arr, flat.data_ptr(), flat.numel() * 4)
 
 
+def _image_format(image_feats) -> torch.dtype:
+    """the format of the image taps, which selects the sampling entry points: fp32 NCHW (the TF32 image branch) or bf16 in
+    channels_last memory format (NHWC, the bf16 branch, DAGR.image_precision); the taps of one call share it."""
+    dt = image_feats[0].dtype
+    if dt not in (torch.float32, torch.bfloat16) or any(f.dtype != dt for f in image_feats):
+        raise ValueError(f"image_feats of dtypes {[f.dtype for f in image_feats]}: expected all float32 or all bfloat16")
+    if dt == torch.bfloat16 and not all(f.dim() == 4 and f.is_contiguous(memory_format=torch.channels_last) for f in image_feats):
+        raise ValueError("bfloat16 image_feats must be [B, C, h, w] tensors in channels_last memory format (NHWC)")
+    return dt
+
+
 class _ConvPack:
     def __init__(self, conv, norm=None, relu=False, dev=None):
         self.cin, self.cout = conv.in_channels, conv.out_channels
@@ -158,7 +169,10 @@ class Engine:
                      dagr_l1_x0_image_planes=1, dagr_voxel_sample_max_planes=1, dagr_sample_features_planes=1, dagr_head_finish_planes=1,
                      dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
                      dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
-                     dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1)
+                     dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1,
+                     dagr_l1_x0_image_bf16=1, dagr_l1_x0_image_live_bf16=1, dagr_l1_x0_image_planes_bf16=1, dagr_voxel_sample_max_bf16=1,
+                     dagr_voxel_sample_max_inc_bf16=1, dagr_voxel_sample_max_planes_bf16=1, dagr_sample_features_bf16=1,
+                     dagr_sample_features_planes_bf16=1)
 
     def _run(self, label, fn, *args):
         if self.prof is not None:
@@ -511,12 +525,13 @@ class Engine:
         if key not in ws:
             per = geom.levels[lv].nx * geom.levels[lv].ny
             ws[key] = (torch.arange(cells, device=dev) // per).int()
+        sfx = "_bf16" if feat.dtype == torch.bfloat16 else ""           # the map's format (_image_format)
         if planes is not None:
-            self._run("sample_features", self.lib.dagr_sample_features_planes, _lib.ptr(feat), int(feat.shape[0]), _lib.ptr(planes[0]),
+            self._run("sample_features", getattr(self.lib, "dagr_sample_features_planes" + sfx), _lib.ptr(feat), int(feat.shape[0]), _lib.ptr(planes[0]),
                       int(planes[1]), Cf, int(feat.shape[2]), int(feat.shape[3]), _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells,
                       geom.W, geom.H, _lib.ptr(xcat), Cc + Cf, Cc, st)
             return xcat
-        self._run("sample_features", self.lib.dagr_sample_features, _lib.ptr(feat), int(feat.shape[0]), Cf, int(feat.shape[2]),
+        self._run("sample_features", getattr(self.lib, "dagr_sample_features" + sfx), _lib.ptr(feat), int(feat.shape[0]), Cf, int(feat.shape[2]),
                   int(feat.shape[3]), _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells, geom.W, geom.H, _lib.ptr(xcat),
                   Cc + Cf, Cc, st)
         return xcat
@@ -550,6 +565,8 @@ class Engine:
             if self.keep_node_features:
                 raise ValueError("keep_node_features: the dense head maps (dagr_grid_to_dense) have no plane mode")
             plane_tab, plane_stride = image_planes
+        # the taps' format picks the fp32 or the bf16 sampling entry points (checked before any device work)
+        sfx = "_bf16" if image_feats is not None and _image_format(image_feats) == torch.bfloat16 else ""
         geom = self.geometry(W, H, B, dev)
         pk = self.pack(geom, dev)
         ws = self.workspace(geom, N, dev)
@@ -613,21 +630,22 @@ class Engine:
             if image_event is not None:                       # stage 1 of the image branch ran on a side stream next to sort + probe
                 torch.cuda.current_stream().wait_event(image_event[0])
             f0 = image_feats[0]
+            c0w = (int(f0.shape[1]),) if sfx else ()                  # the bf16 forms take the tap's channel count
             x0 = self._buf(ws, "x0img", (2 * max(N, 1) * 8,), torch.float32, dev)
             skipv = self._buf(ws, "skipv", (max(N, 1), 16), torch.float32, dev)
             if image_planes is not None:
-                self._run("l1_x0_image", lib.dagr_l1_x0_image_planes, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
-                          _lib.ptr(f0), int(f0.shape[2]), int(f0.shape[3]), int(f0.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
+                self._run("l1_x0_image", getattr(lib, "dagr_l1_x0_image_planes" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                          _lib.ptr(ws["feat_s"]), _lib.ptr(f0), *c0w, int(f0.shape[2]), int(f0.shape[3]), int(f0.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
                           _lib.ptr(x0), st)
             elif ring is not None:
                 # N = ring capacity: positions behind the live total hold stale xyb words, so the launch is bounded by the
                 # total the sort wrote (start[NK]); the synchronous path keeps the unbounded form (N is the live count there)
-                self._run("l1_x0_image", lib.dagr_l1_x0_image_live, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
-                          _lib.ptr(f0), int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
+                self._run("l1_x0_image", getattr(lib, "dagr_l1_x0_image_live" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                          _lib.ptr(ws["feat_s"]), _lib.ptr(f0), *c0w, int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
             else:
                 # incremental steps resample every node too: a new node's conv reads the x0 rows of its older neighbours
-                self._run("l1_x0_image", lib.dagr_l1_x0_image, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(f0),
-                          int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
+                self._run("l1_x0_image", getattr(lib, "dagr_l1_x0_image" + sfx), g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
+                          _lib.ptr(f0), *c0w, int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
             if stream_state is not None:
                 # only the new nodes are convolved; the xa rows of the older ones are final and stay as gathered
                 self._run("l1_conv_a_image_inc", lib.dagr_l1_conv_a_image_inc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
@@ -674,17 +692,17 @@ class Engine:
             self._dense_report(ws, wl_hdr)
             if use_image and stream_state is not None:        # running per-voxel max of the samples, new events only
                 f1 = image_feats[1]
-                self._run("voxel_sample_max_inc", lib.dagr_voxel_sample_max_inc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                self._run("voxel_sample_max_inc", getattr(lib, "dagr_voxel_sample_max_inc" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
                           _lib.ptr(ws["ti"]), _lib.ptr(f1), int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), min_idx,
                           _lib.ptr(stream_state.imgmax), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
             elif image_planes is not None:
                 f1 = image_feats[1]
-                self._run("voxel_sample_max", lib.dagr_voxel_sample_max_planes, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
+                self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max_planes" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
                           int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), int(f1.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
                           _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
             elif use_image:                                   # sampling_skip before pool1 (net.py:128-131)
                 f1 = image_feats[1]
-                self._run("voxel_sample_max", lib.dagr_voxel_sample_max, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
+                self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
                           int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
         else:
             self._run("l1_conv_b_pool", lib.dagr_l1_conv_b_pool, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(ws["xa"]),

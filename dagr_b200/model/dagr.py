@@ -95,6 +95,7 @@ class DAGR(YOLOX):
         self._image_branch = None
         self.image_graph = True         # dense image branch as a replayed CUDA graph on a side stream (model/image_branch.py)
         self.keep_stream = False        # True: forward(reset=True) starts a stream that forward(reset=False) extends
+        self.image_precision = "tf32"   # image branch precision, see the property
         if "img_net_checkpoint" in args:
             sd = torch.load(args.img_net_checkpoint, map_location="cpu")["ema"]
             for name in ("backbone.net.", "head.cnn_head."):
@@ -136,6 +137,22 @@ class DAGR(YOLOX):
         if getattr(self, "_image_branch", None) is not None:
             self._image_branch.invalidate()
         return out
+
+    @property
+    def image_precision(self) -> str:
+        """precision of the dense image branch (--use_image): "tf32" (default) runs the model's own fp32 trunk and CNN head
+        with TF32 convolutions and fp32 NCHW feature maps; "bf16" runs a bf16, channels_last copy of them under autocast,
+        whose feature taps stay bf16 NHWC and are sampled by the bf16 forms of the event-level image kernels (everything
+        downstream of the samples stays fp32).  Any other value raises ValueError.  model(data) reads it per call; AsyncDAGR
+        and the fusion streaming detectors read it once, when they are constructed."""
+        return self.__dict__.get("_image_precision", "tf32")
+
+    @image_precision.setter
+    def image_precision(self, value):
+        from .image_branch import PRECISIONS
+        if value not in PRECISIONS:
+            raise ValueError(f"image_precision {value!r}: expected one of {PRECISIONS}")
+        self.__dict__["_image_precision"] = value
 
     @property
     def engine(self):
@@ -228,7 +245,8 @@ class DAGR(YOLOX):
             if self._image_branch is None:
                 from .image_branch import ImageBranch
                 self._image_branch = ImageBranch(self)
-            image_feats, image_outs, image_event = self._image_branch.run(x.image, use_graph=self.image_graph)
+            image_feats, image_outs, image_event = self._image_branch.run(x.image, use_graph=self.image_graph,
+                                                                          precision=self.image_precision)
             self.last_image_outs, self.last_image_feats = image_outs, image_feats
             if self.head.no_events:
                 # --no_events (dagr.py:284): detections from the image branch alone -- collect_outputs + decode_outputs on

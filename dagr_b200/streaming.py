@@ -391,8 +391,10 @@ def _check_raw_frames(raw_frames, sensor):
 
 
 def _frame_setup(det, raw_frames):
-    """frame handling of the fusion detectors after _setup: the frame stream, and with raw_frames the u8 -> f32 table."""
+    """frame handling of the fusion detectors after _setup: the frame stream, the image branch precision (read once from the
+    model: a later change of model.image_precision does not reach the detector), and with raw_frames the u8 -> f32 table."""
     det.frame_stream = torch.cuda.Stream(device=det.dev)
+    det.image_precision = det.model.image_precision
     det.raw_frames = bool(raw_frames)
     det._frame_lut = ingest.frame_lut(det.dev) if det.raw_frames else None
 
@@ -482,7 +484,7 @@ class _CameraFrames:
                 self.h2d.record(fs)
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record(fs)
-            feats, outs, (_, ev2) = br.run(x, use_graph=m.image_graph)
+            feats, outs, (_, ev2) = br.run(x, use_graph=m.image_graph, precision=det.image_precision)
             x.record_stream(fs)
             x.record_stream(br.stream)
             fs.wait_event(ev2)
@@ -798,7 +800,9 @@ class FusionMultiStreamDetector(MultiStreamDetector):
     def _plane_dst(self, k, feats, outs):
         if self._planes is None:
             n = 2 * self.S
-            self._planes = ([torch.empty((n,) + tuple(f.shape[1:]), dtype=f.dtype, device=self.dev) for f in feats],
+            # bf16 feature maps are NHWC (channels_last), and so are their plane arrays: [2S, h, w, C] in memory
+            fmt = torch.channels_last if feats[0].dtype == torch.bfloat16 else torch.contiguous_format
+            self._planes = ([torch.empty((n,) + tuple(f.shape[1:]), dtype=f.dtype, device=self.dev, memory_format=fmt) for f in feats],
                             {key: [torch.empty((n,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev) for t in v]
                              for key, v in outs.items()})
         pf, po = self._planes

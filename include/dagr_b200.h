@@ -470,6 +470,36 @@ int dagr_head_finish_planes(const dagr_grid_t *gr, const int32_t *cnt, const flo
                             const float *add_cls, const float *add_reg, const float *add_obj, int nc, int stride, int a0, int A,
                             int nplanes, const int32_t *plane, int plane_stride, float *out, void *stream);
 
+/* bf16 NHWC maps (the taps of the bf16 image branch, DAGR.image_precision = "bf16"): each sampling entry point above has a
+ * _bf16 form that takes the map as `const void *` to bf16 in NHWC order -- [B][h][w][C], or [nplanes][h][w][C] for the
+ * _planes forms; a torch tensor [B, C, h, w] in channels_last memory format -- with its (C, h, w), and otherwise the same
+ * arguments.  Each returns exactly the floats its fp32 form returns on the NCHW fp32 upcast of the same map (bf16 -> fp32
+ * is exact; the taps, their order and the fp32 arithmetic are those of the fp32 form).  Every _bf16 entry point returns
+ * DAGR_E_ARG with a message before launching anything on a null pointer (feat_s may be NULL), N outside [0, 2^31), h or
+ * w < 1, and as its _planes / _inc sibling on nplanes < 1, plane_stride < 1, min_idx < 0, c0 + C > ldx or pool_mean with
+ * _inc.  The x0 forms take C and require C == 16. */
+int dagr_l1_x0_image_bf16(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
+                          const void *img0 /*bf16 [B,h,w,16]*/, int C, int h, int w, float *x0, void *stream);
+int dagr_l1_x0_image_live_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                               const void *img0 /*bf16 [B,h,w,16]*/, int C, int h, int w, float *x0, void *stream);
+int dagr_l1_x0_image_planes_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+                                 const void *img0 /*bf16 [nplanes,h,w,16]*/, int C, int h, int w, int nplanes, const int32_t *plane,
+                                 int plane_stride, float *x0, void *stream);
+int dagr_voxel_sample_max_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
+                               const void *img /*bf16 [B,h,w,C]*/, int C, int h, int w, float *xg, int ldx, int c0, int pool_mean,
+                               void *stream);
+int dagr_voxel_sample_max_inc_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                                   const void *img /*bf16 [B,h,w,C]*/, int C, int h, int w, int min_idx, float *persist, float *xg,
+                                   int ldx, int c0, int pool_mean, void *stream);
+int dagr_voxel_sample_max_planes_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
+                                      const void *img /*bf16 [nplanes,h,w,C]*/, int C, int h, int w, int nplanes, const int32_t *plane,
+                                      int plane_stride, float *xg, int ldx, int c0, int pool_mean, void *stream);
+int dagr_sample_features_bf16(const void *img /*bf16 [Bi,h,w,C]*/, int Bi, int C, int h, int w, const float *posx, const float *posy,
+                              const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0, void *stream);
+int dagr_sample_features_planes_bf16(const void *img /*bf16 [nplanes,h,w,C]*/, int nplanes, const int32_t *plane, int plane_stride,
+                                     int C, int h, int w, const float *posx, const float *posy, const int32_t *bidx, int64_t n,
+                                     int width, int height, float *out, int ldo, int c0, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * a14  asy_tools (src/dagr/asynchronous/asy_tools/main.cu:239-244), same argument meaning.
  * masked_isdiff writes kept[i] = idx[i] or -1 (the reference clobbers `indices` in place, :30-37);
