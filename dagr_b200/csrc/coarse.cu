@@ -762,17 +762,18 @@ k_postprocess_nms(const float *__restrict__ pred, int A, int nc, float conf_thre
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     if (threadIdx.x == 0) ncand = 0;
     __syncthreads();
-    // per anchor: xyxy, class max, score, confidence mask (model/utils.py:62-87)
+    // per anchor: xyxy, class max, score, confidence mask (model/utils.py:62-87).  Every rounding step that decides the
+    // output is an explicit _rn intrinsic, so nvcc / ptxas cannot contract it into an FMA (w * 0.5 == w / 2 exactly).
     for (int a = threadIdx.x; a < A; a += blockDim.x) {
         const float *p = P + (int64_t)a * (5 + nc);
-        const float x1 = p[0] - p[2] / 2.f, y1 = p[1] - p[3] / 2.f;
-        const float x2 = p[2] + x1, y2 = p[3] + y1;
+        const float x1 = __fsub_rn(p[0], __fmul_rn(p[2], 0.5f)), y1 = __fsub_rn(p[1], __fmul_rn(p[3], 0.5f));
+        const float x2 = __fadd_rn(p[2], x1), y2 = __fadd_rn(p[3], y1);
         float cc = p[5]; int cl = 0;
         for (int c = 1; c < nc; c++) if (p[5 + c] > cc) { cc = p[5 + c]; cl = c; }
-        const float score = p[4] * cc;
-        const bool keep = !filtering || (score * cc >= conf_thre);
+        const float score = __fmul_rn(p[4], cc);
+        const bool keep = !filtering || (__fmul_rn(score, cc) >= conf_thre);
         raw[a][0] = x1; raw[a][1] = y1; raw[a][2] = x2; raw[a][3] = y2; raw[a][4] = score; raw[a][5] = (float)cl;
-        const float offs = (float)cl * max_dim1;
+        const float offs = (float)cl * max_dim1;                          // exact integer product: an FMA here is harmless
         bx[a][0] = x1 + offs; bx[a][1] = y1 + offs; bx[a][2] = x2 + offs; bx[a][3] = y2 + offs;
         sc[a] = score;
         alive[a] = keep ? 1 : 0;
@@ -799,18 +800,20 @@ k_postprocess_nms(const float *__restrict__ pred, int A, int nc, float conf_thre
     for (int i = warp; i < n; i += nwarps) {
         const int ai = order[i];
         const float ax1 = bx[ai][0], ay1 = bx[ai][1], ax2 = bx[ai][2], ay2 = bx[ai][3];
-        const float sa = (ax2 - ax1) * (ay2 - ay1);
+        const float sa = __fmul_rn(__fsub_rn(ax2, ax1), __fsub_rn(ay2, ay1));
         for (int wd = i >> 5; wd < nwords; wd++) {
             const int k = wd * 32 + lane;
             bool hit = false;
             if (k > i && k < n) {
+                // torchvision's CPU IoU, every step rounded on its own: with plain operators nvcc turned sa + sb into
+                // fma(dx_b, dy_b, sa), which flips the decision for pairs within an ulp of nms_thre
                 const int aj = order[k];
                 const float l = fmaxf(ax1, bx[aj][0]), t = fmaxf(ay1, bx[aj][1]);
                 const float r = fminf(ax2, bx[aj][2]), bt = fminf(ay2, bx[aj][3]);
-                const float iw = fmaxf(r - l, 0.f), ih = fmaxf(bt - t, 0.f);
-                const float inter = iw * ih;
-                const float sb = (bx[aj][2] - bx[aj][0]) * (bx[aj][3] - bx[aj][1]);
-                hit = inter / (sa + sb - inter) > nms_thre;
+                const float iw = fmaxf(__fsub_rn(r, l), 0.f), ih = fmaxf(__fsub_rn(bt, t), 0.f);
+                const float inter = __fmul_rn(iw, ih);
+                const float sb = __fmul_rn(__fsub_rn(bx[aj][2], bx[aj][0]), __fsub_rn(bx[aj][3], bx[aj][1]));
+                hit = __fdiv_rn(inter, __fsub_rn(__fadd_rn(sa, sb), inter)) > nms_thre;
             }
             const uint32_t bits = __ballot_sync(0xffffffffu, hit);
             if (lane == 0) supp[i][wd] = bits;
@@ -839,7 +842,11 @@ k_postprocess_nms(const float *__restrict__ pred, int A, int nc, float conf_thre
 extern "C" int dagr_postprocess_nms(const float *pred, int B, int A, int nc, float conf_thre, float nms_thre, int width,
                                     int height, int filtering, float *det, int32_t *ndet, void *stream)
 {
+    DAGR_CHECK_ARG(pred && det && ndet, "null pred / det / ndet");
+    DAGR_CHECK_ARG(nc >= 1, "nc must be >= 1 (a row is cx, cy, w, h, obj and at least one class score)");
     DAGR_CHECK_ARG(A > 0 && A <= NMS_MAX, "A must be in [1,256] (two-scale DAGR heads have 175 anchors)");
+    DAGR_CHECK_ARG(B >= 0, "B must be >= 0");
+    if (B == 0) return DAGR_OK;
     const float max_dim1 = (float)((width > height ? width : height) + 1);
     k_postprocess_nms<<<B, NMS_THREADS, 0, (cudaStream_t)stream>>>(pred, A, nc, conf_thre, nms_thre, max_dim1, filtering, det, ndet);
     DAGR_CHECK_LAUNCH();

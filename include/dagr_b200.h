@@ -435,7 +435,14 @@ int dagr_head_finish(const dagr_grid_t *gr, const int32_t *cnt, const float *cls
 
 /* a11 postprocess_network_output + batched_nms_coordinate_trick (model/utils.py:25-33,61-110).
  * pred f32[B,A,5+nc] (decoded, cxcywh) -> det f32[B,A,6] = (x1,y1,x2,y2,score,label) compacted in
- * descending-score order, ndet i32[B].  One CTA per image, A <= 256. */
+ * descending-score order, ndet i32[B].  One CTA per image, A <= 256.  torchvision.ops.nms semantics bit for bit: the
+ * IoU, areas, xyxy corners and obj * cls^2 round every step on its own (no FMA), as torchvision's CPU kernel and the
+ * reference's torch code do,
+ * compared against the fp32 nms_thre / conf_thre as the reference's torch code does (torchvision compares the IoU with
+ * the double threshold: the same decisions wherever fl32(nms_thre) <= nms_thre, as at 0.65); ties in score go to the
+ * lower anchor, ties in class to the first class.
+ * Returns DAGR_E_ARG with a message before launching anything on a null pred / det / ndet, nc < 1, A outside [1, 256]
+ * or B < 0; B == 0 returns DAGR_OK without a launch. */
 int dagr_postprocess_nms(const float *pred, int B, int A, int nc, float conf_thre, float nms_thre,
                          int width, int height, int filtering, float *det, int32_t *ndet, void *stream);
 
