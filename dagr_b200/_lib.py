@@ -114,6 +114,7 @@ _SIGS = {
     "dagr_pool1_finalize": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, p, p, p, p, p, p]),
     "dagr_grid_cat_pos": (C.c_int, [C.POINTER(Grid), p, p, p, C.c_int, p, p]),
     "dagr_grid_conv": (C.c_int, [C.POINTER(Grid), p, p, p, p, C.c_int, C.c_int, C.c_int, p, p, p, p, p, p, C.c_int, f32, f32, p, p]),
+    "dagr_grid_conv_last_instance": (C.c_int, []),
     "dagr_grid_linear_bn": (C.c_int, [i64, p, p, C.c_int, C.c_int, p, p, p, p, p]),
     "dagr_grid_pool": (C.c_int, [C.POINTER(Grid), C.POINTER(Grid), p, p, p, p, p, p, p, p, C.c_int, C.c_int,
                                  p, p, p, p, p, p, p, p]),

@@ -383,6 +383,11 @@ static int launch_grid_conv_sk(const dagr_grid_t *gr, const int32_t *cnt, const 
     return 0;
 }
 
+// kernel of the last successful dagr_grid_conv call on this thread (see dagr_grid_conv_last_instance)
+static thread_local int grid_conv_last = -1;
+
+extern "C" int dagr_grid_conv_last_instance(void) { return grid_conv_last; }
+
 extern "C" int dagr_grid_conv(const dagr_grid_t *gr, const int32_t *cnt, const int32_t *pxy, const uint32_t *mask,
                               const float *xin, int ldin, int Cin, int Cout, const float *weight, const float *rootT,
                               const float *bias, const float *scale, const float *shift, const float *skip, int relu,
@@ -399,14 +404,17 @@ extern "C" int dagr_grid_conv(const dagr_grid_t *gr, const int32_t *cnt, const i
         DAGR_CUDA(cudaGetDevice(&dev));
         DAGR_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     }
-    int rc = -1;
+    int rc = -1, cpb = 0;
     const size_t per_cell = ((size_t)SK_SLOTS * Cin + (Cout <= 64 ? 0 : (size_t)SK_WARPS * Cout)) * sizeof(float);
     if (cells >= n_sm * 16 * 2 && per_cell * 16 <= 110 * 1024)
         rc = launch_grid_conv_sk<16>(gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out, st);
+    if (rc == 0 && cpb == 0) cpb = 16;
     if (rc != 0 && cells >= n_sm * 4 && per_cell * 4 <= 160 * 1024)
         rc = launch_grid_conv_sk<4>(gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out, st);
+    if (rc == 0 && cpb == 0) cpb = 4;
     if (rc != 0)
         rc = launch_grid_conv_sk<1>(gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out, st);
+    if (rc == 0 && cpb == 0) cpb = 1;
     if (rc != 0) {
         // very wide layers: v1 kernel (one warp per voxel)
         const size_t smem = (size_t)GC_WARPS * GC_SLOTS * Cin * sizeof(float);
@@ -416,6 +424,7 @@ extern "C" int dagr_grid_conv(const dagr_grid_t *gr, const int32_t *cnt, const i
             *gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out);
     }
     DAGR_CHECK_LAUNCH();
+    grid_conv_last = cpb;
     return DAGR_OK;
 }
 
@@ -472,7 +481,10 @@ extern "C" int dagr_grid_linear_bn(int64_t cells, const int32_t *cnt, const floa
 {
     DAGR_CHECK_ARG(Cin > 0 && Cout > 0 && (size_t)LB_CELLS * Cin * 4 <= 48 * 1024, "bad channels");
     if (cells <= 0) return DAGR_OK;
-    k_grid_linear_bn<<<dagr_div_up(cells, LB_CELLS), 256, (size_t)LB_CELLS * Cin * sizeof(float), (cudaStream_t)stream>>>(
+    const size_t smem = (size_t)LB_CELLS * Cin * sizeof(float);
+    // rows plus the static s_valid exceed the 48 KB a CTA gets without an opt-in once the rows come close to 48 KB
+    if (smem > 40 * 1024) DAGR_CUDA(dagr_allow_smem(k_grid_linear_bn, smem));
+    k_grid_linear_bn<<<dagr_div_up(cells, LB_CELLS), 256, smem, (cudaStream_t)stream>>>(
         cells, cnt, xin, Cin, Cout, wT, scale, shift, out);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;

@@ -591,7 +591,8 @@ def test_batch_independence_and_full_size_properties():
     single = EventBatch(x=data.x[m], pos=data.pos[m], batch=torch.zeros(int(m.sum()), dtype=torch.long),
                         width=data.width[:1], height=data.height[:1], time_window=data.time_window[:1], num_graphs=1)
     dec1, _, _ = _run_graph(model, single, 1)
-    assert_close(dec1[0].cpu(), dec[b].cpu(), tol=1e-5, what="sample alone vs inside batch")
+    diff = (dec1[0] - dec[b]).abs().max().item()
+    assert torch.equal(dec1[0], dec[b]), f"sample alone vs inside batch: max |diff| {diff:.3g}"
 
 
 # ---------------------------------------------------------------------------------------------
