@@ -88,22 +88,17 @@ _SIGS = {
     "dagr_stream_push": (C.c_int, [p, p, p, p, p, i64, C.c_int, C.c_int, p]),
     "dagr_stream_push_multi": (C.c_int, [p, p, p, p, p, i64, C.c_int, C.c_int, p]),
     "dagr_graph_sort_rings": (C.c_int, [C.POINTER(Geom), p, p, p, i64, C.c_int, p, p, p, p, p, p, p, p, p, p, p, p]),
-    "dagr_graph_search": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p]),
-    "dagr_l1_build": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, C.POINTER(L1AParams), p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
+    "dagr_l1_build": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.POINTER(L1AParams), p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
     "dagr_l1a_tc_weights": (C.c_int, [C.POINTER(L1AParams), p]),
     "dagr_l1_build_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.POINTER(L1AParams), p, p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
     "dagr_xa_permute": (C.c_int, [i64, p, C.c_int, p, p, C.c_int, p]),
     "dagr_l1_x0_image": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, p, p]),
     "dagr_l1_x0_image_live": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, p, p]),
     "dagr_l1_x0_image_planes": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, p, p]),
-    "dagr_l1_conv_a_image": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1ImgParams), p, p, p, p, C.c_int, p]),
     "dagr_voxel_sample_max": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, C.c_int, C.c_int, p]),
     "dagr_voxel_sample_max_planes": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p, C.c_int,
                                                C.c_int, C.c_int, p]),
     "dagr_graph_export": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, p, i64, p]),
-    "dagr_l1_conv_a": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, C.POINTER(L1AParams), p, p]),
-    "dagr_l1_conv_b_pool": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1BParams), p, p, p]),
-    "dagr_l1_conv_b_pool_voxel": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, p, C.POINTER(L1BParams), p, C.c_int, p, p, p, p, p, p, p, C.c_int, p, p, C.c_int, p]),
     "dagr_l1_tc_weights": (C.c_int, [p, p, C.c_int, p]),
     "dagr_l1_conv_b_pool_voxel_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, C.POINTER(L1BParams), p, p, C.c_int, p, p, p, p, p, p, p, C.c_int, p, p, C.c_int, p]),
     "dagr_l1_conv_a_image_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1ImgParams), p, p, p, p, p, C.c_int, p]),
@@ -111,7 +106,6 @@ _SIGS = {
                                            C.c_int, p]),
     "dagr_voxel_sample_max_inc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int, C.c_int,
                                             C.c_int, p]),
-    "dagr_pool1_finalize": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, p, p, p, p, p, p]),
     "dagr_grid_cat_pos": (C.c_int, [C.POINTER(Grid), p, p, p, C.c_int, p, p]),
     "dagr_grid_conv": (C.c_int, [C.POINTER(Grid), p, p, p, p, C.c_int, C.c_int, C.c_int, p, p, p, p, p, p, C.c_int, f32, f32, p, p]),
     "dagr_grid_conv_last_instance": (C.c_int, []),
@@ -121,7 +115,6 @@ _SIGS = {
     "dagr_grid_pool_finalize": (C.c_int, [C.POINTER(Grid), C.c_int, C.c_int, p, p, p, p, p, p, p, p, p, p]),
     "dagr_grid_temporal_filter": (C.c_int, [C.POINTER(Grid), p, p, p, p]),
     "dagr_grid_to_dense": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, C.c_int, p, p, p]),
-    "dagr_head_decode": (C.c_int, [p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p]),
     "dagr_head_finish": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, p, C.c_int, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p]),
     "dagr_head_finish_planes": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, p, C.c_int, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_int, p, C.c_int, p, p]),
@@ -178,7 +171,7 @@ def load():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
-    if lib.dagr_abi_version() != 2:
+    if lib.dagr_abi_version() != 3:
         raise RuntimeError("dagr_b200: ABI version mismatch between python host and libdagr_b200.so")
     _lib = lib
     return lib

@@ -831,11 +831,10 @@ static int l1_build_launch(const dagr_geom_t *g, int64_t N, const int32_t *start
 }
 
 extern "C" int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
-                             const uint32_t *xyb, const float *feat_s, const float *tab,
+                             const uint32_t *xyb, const float *feat_s,
                              const dagr_l1a_params_t *p_host, const int32_t *flags, int min_idx, int32_t *nbr, uint16_t *off,
                              uint32_t *cellmask, float *xa, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
 {
-    (void)tab;                                                          // the slot weights come from g->tabx / g->taby
     return l1_build_launch<false>(g, N, start, ti, xyb, feat_s, p_host, nullptr, flags, min_idx, nbr, off, cellmask, xa, wl_hdr,
                                   wl_ids, defer, (cudaStream_t)stream);
 }

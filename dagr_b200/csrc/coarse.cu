@@ -10,91 +10,6 @@
 #include "common.cuh"
 
 // ------------------------------------------------------------------------------------------------
-// pool1 finalize: one warp per voxel
-// ------------------------------------------------------------------------------------------------
-// torch.div(a, b, rounding_mode='floor') for fp32 (c10::div_floor_floating), needed because
-// floorf(a/b) differs when the rounded quotient lands on an integer from below.
-__device__ __forceinline__ float div_floor_f32(float a, float b)
-{
-    const float mod = fmodf(a, b);
-    float div = __fdiv_rn(__fsub_rn(a, mod), b);
-    if ((mod != 0.f) && ((b < 0.f) != (mod < 0.f))) div -= 1.f;
-    float fl;
-    if (div != 0.f) {
-        fl = floorf(div);
-        if (div - fl > 0.5f) fl += 1.f;
-    } else {
-        fl = copysignf(0.f, __fdiv_rn(a, b));
-    }
-    return fl;
-}
-
-__device__ __forceinline__ int round_to_pixel(float mean, int size)
-{
-    // floor((pos + 1e-5) / (1/size))   (pooling.py:47-49), wh_inv = fl(1/size)
-    const float inv = __frcp_rn((float)size);
-    const float q = div_floor_f32(__fadd_rn(mean, 1e-5f), inv);
-    const int k = (int)q;
-    return min(max(k, 0), size - 1);
-}
-
-__global__ void __launch_bounds__(128)
-k_pool1_finalize(const dagr_geom_t g, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
-                 const int2 *__restrict__ ti, const uint32_t *__restrict__ poolmax, int C,
-                 int32_t *__restrict__ cnt, int32_t *__restrict__ pxy, float *__restrict__ tmean,
-                 float *__restrict__ tmax, float *__restrict__ x)
-{
-    const int cells = g.B * g.ny1 * g.nx1;
-    const int cell = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (cell >= cells) return;
-    const int s = start[(int64_t)cell * g.CP], e = start[(int64_t)(cell + 1) * g.CP];
-    long long sx = 0, sy = 0, st = 0;
-    int tm = -2147483647;
-    for (int p = s + lane; p < e; p += 32) {
-        const uint32_t w = xyb[p];
-        sx += w & 0xfff; sy += (w >> 12) & 0xfff;
-        const int t = ti[p].x;
-        st += t; tm = max(tm, t);
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        sx += __shfl_xor_sync(0xffffffffu, sx, d);
-        sy += __shfl_xor_sync(0xffffffffu, sy, d);
-        st += __shfl_xor_sync(0xffffffffu, st, d);
-        tm = max(tm, __shfl_xor_sync(0xffffffffu, tm, d));
-    }
-    const int n = e - s;
-    if (lane == 0) {
-        cnt[cell] = n;
-        if (n > 0) {
-            const float mx = (float)((double)sx / ((double)n * (double)g.W));
-            const float my = (float)((double)sy / ((double)n * (double)g.H));
-            pxy[2 * cell] = round_to_pixel(mx, g.W);
-            pxy[2 * cell + 1] = round_to_pixel(my, g.H);
-            tmean[cell] = (float)((double)st / ((double)n * (double)g.T));
-            tmax[cell] = __fdiv_rn((float)tm, (float)g.T);
-        } else {
-            pxy[2 * cell] = 0; pxy[2 * cell + 1] = 0; tmean[cell] = 0.f; tmax[cell] = 0.f;
-        }
-    }
-    for (int c = lane; c < C; c += 32)
-        x[(int64_t)cell * C + c] = n > 0 ? dec_ordered(poolmax[(int64_t)cell * C + c]) : 0.f;
-}
-
-extern "C" int dagr_pool1_finalize(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
-                                   const int32_t *ti, const uint32_t *poolmax, int C, int32_t *cnt, int32_t *pxy,
-                                   float *tmean, float *tmax, float *x, void *stream)
-{
-    (void)N;
-    const int cells = g->B * g->ny1 * g->nx1;
-    k_pool1_finalize<<<dagr_div_up(cells, 4), 128, 0, (cudaStream_t)stream>>>(*g, start, xyb, (const int2 *)ti, poolmax, C,
-                                                                            cnt, pxy, tmean, tmax, x);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
 // cat(x, pos[:, :2])
 // ------------------------------------------------------------------------------------------------
 __global__ void k_cat_pos(const dagr_grid_t gr, const int32_t *__restrict__ cnt, const int32_t *__restrict__ pxy,
@@ -657,37 +572,11 @@ extern "C" int dagr_grid_to_dense(const dagr_grid_t *gr, const int32_t *cnt, con
     return DAGR_OK;
 }
 
-__global__ void k_head_decode(const float *__restrict__ reg, const float *__restrict__ obj, const float *__restrict__ cls,
-                              int B, int nc, int h, int w, float stride, int a0, int A, float *__restrict__ out)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int hw = h * w;
-    if (i >= B * hw) return;
-    const int b = i / hw, a = i % hw, gy = a / w, gx = a % w;
-    float *o = out + ((int64_t)b * A + a0 + a) * (5 + nc);
-    const float *r = reg + (int64_t)b * 4 * hw + a;
-    o[0] = (r[0] + (float)gx) * stride;
-    o[1] = (r[hw] + (float)gy) * stride;
-    o[2] = expf(r[2 * hw]) * stride;
-    o[3] = expf(r[3 * hw]) * stride;
-    o[4] = 1.f / (1.f + expf(-obj[(int64_t)b * hw + a]));
-    for (int c = 0; c < nc; c++) o[5 + c] = 1.f / (1.f + expf(-cls[((int64_t)b * nc + c) * hw + a]));
-}
-
-extern "C" int dagr_head_decode(const float *reg, const float *obj, const float *cls, int B, int nc, int h, int w,
-                                int stride, int a0, int A, float *out, void *stream)
-{
-    k_head_decode<<<dagr_div_up((int64_t)B * h * w, 128), 128, 0, (cudaStream_t)stream>>>(reg, obj, cls, B, nc, h, w,
-                                                                                       (float)stride, a0, A, out);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
 // to_dense (spline_conv.py:80-107) of the three prediction convs + CNN maps (dagr.py:219-222) + collect_outputs /
 // decode_outputs (dagr.py:292-312) of one scale in ONE pass: per voxel of the dense head grid
 //   reg/obj/cls = (valid ? conv output : 0) + CNN map;  xy = (reg_xy + grid) * stride, wh = exp(reg_wh) * stride,
 //   sigmoid(obj), sigmoid(cls)  -> out[b, a0 + cell, 5 + nc]
-// (the separate to_dense + head_decode launches, 8 per forward, remain for callers that want the dense maps)
+// (dagr_grid_to_dense remains for callers that want the dense maps)
 // PLANES: the CNN maps add_* are plane arrays [pl.n][C][ny][nx] and sample b reads plane img_plane(pl, b).
 template <bool PLANES>
 __global__ void k_head_finish(const dagr_grid_t gr, const int32_t *__restrict__ cnt, const float *__restrict__ cls, int ldc,

@@ -123,6 +123,33 @@ __device__ __forceinline__ float dec_ordered(uint32_t e)
     return __uint_as_float(u);
 }
 
+// torch.div(a, b, rounding_mode='floor') for fp32 (c10::div_floor_floating), needed because
+// floorf(a/b) differs when the rounded quotient lands on an integer from below.
+__device__ __forceinline__ float div_floor_f32(float a, float b)
+{
+    const float mod = fmodf(a, b);
+    float div = __fdiv_rn(__fsub_rn(a, mod), b);
+    if ((mod != 0.f) && ((b < 0.f) != (mod < 0.f))) div -= 1.f;
+    float fl;
+    if (div != 0.f) {
+        fl = floorf(div);
+        if (div - fl > 0.5f) fl += 1.f;
+    } else {
+        fl = copysignf(0.f, __fdiv_rn(a, b));
+    }
+    return fl;
+}
+
+// pixel position of a pooled voxel (pool1 in conv_l1.cu, pool2..4 in coarse.cu)
+__device__ __forceinline__ int round_to_pixel(float mean, int size)
+{
+    // floor((pos + 1e-5) / (1/size))   (pooling.py:47-49), wh_inv = fl(1/size)
+    const float inv = __frcp_rn((float)size);
+    const float q = div_floor_f32(__fadd_rn(mean, 1e-5f), inv);
+    const int k = (int)q;
+    return min(max(k, 0), size - 1);
+}
+
 // fp32 FMA on both halves of a float2: d = a*b + c, round-to-nearest on each.  Hopper has no packed fp32 FMA, so this is
 // two FFMA; the kernels keep their paired accumulator layout.
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }

@@ -1,306 +1,22 @@
-// conv_l1.cu -- event-level Layer (conv_block1) of DAGR's backbone, sm_90a.
+// conv_l1.cu -- event-level Layer (conv_block1) of DAGR's backbone, sm_90a: the per-voxel SplineConv kernel.
 //
-//   conv_a : SplineConv(3->16) + BN + act                      (conv.py:10-28)
-//   conv_b : SplineConv(16->16) + BN, Linear(3->16)+BN skip, add, act   (conv.py:31-56)
-//            fused with pool1's per-voxel channel max          (pooling.py:74-75)
+//   conv_b      : SplineConv(16->16) + BN, Linear(3->16)+BN skip, add, act   (conv.py:31-56)
+//                 fused with pool1's per-voxel max / mean, mean position and pixel rounding   (pooling.py:66-86)
+//   image fusion: the 16 image channels of conv_a = SplineConv(19->16) + BN + act (conv.py:10-28), on top of the
+//                 (polarity, x, y) sums the build kernel left in xa (build_l1.cu), and the layer's skip branch
+// conv_a of the events-only model (SplineConv(3->16) + BN + act) runs inside the build kernel (build_l1.cu).
 //
 // Formulation ("slot form" of MySplineConv.message_lut, spline_conv.py:39-47).  At the event level
 // every edge offset is an integer pixel offset d in [-r,r]^2 and v = 4*attr lies in (1,3), so only
 // 15 (3 in x, 5 in y) of the 5x5 spline kernels are reachable.  With tab[c][u] = LUT basis weight of
 // slot u for spiral cell c:
-//       A_u[i]  = sum_{e in N(i) + self}  tab[c_e][u] * x[src_e]          (phase 1, per edge)
-//       out[i]  = sum_u  W_u^T A_u[i]  +  W_root^T x[i]                    (phase 2, per node)
-// Phase-2 weights are uniform across lanes and are passed by value as a __grid_constant__ kernel
-// parameter, so every FFMA takes its weight straight from the constant bank (no load instructions).
-// One thread per destination node; nodes are in cell-major sorted order, so own rows, ELL columns
-// and outputs are fully coalesced and the pool1 max is a warp-segmented reduction.
+//       A_u[i]  = sum_{e in N(i) + self}  tab[c_e][u] * x[src_e]          (phase 1, per edge, fp32 FMA)
+//       out[i]  = sum_u  W_u^T A_u[i]  +  W_root^T x[i]                    (phase 2, per node, 3xTF32 on tensor cores)
 #include <string.h>
 #include "common.cuh"
 
-#define L1_THREADS 128
-
-struct L1Smem {
-    float *tab;     // [ncell][DAGR_TABW]
-    float *posx;    // [W]
-    float *posy;    // [H]
-    short *sp;      // [ncell]
-};
-
-__device__ __forceinline__ L1Smem l1_smem_init(const dagr_geom_t &g, const float *__restrict__ tab, unsigned char *raw)
-{
-    L1Smem s;
-    s.tab = (float *)raw;
-    s.posx = s.tab + g.ncell * DAGR_TABW;
-    s.posy = s.posx + g.W;
-    s.sp = (short *)(s.posy + g.H);
-    for (int i = threadIdx.x; i < g.ncell * DAGR_TABW; i += blockDim.x) s.tab[i] = tab[i];
-    for (int i = threadIdx.x; i < g.W; i += blockDim.x) s.posx[i] = g.posx0[i];
-    for (int i = threadIdx.x; i < g.H; i += blockDim.x) s.posy[i] = g.posy0[i];
-    for (int i = threadIdx.x; i < g.ncell; i += blockDim.x)
-        s.sp[i] = (short)(((int)g.spiral[2 * i] & 0xff) | ((int)g.spiral[2 * i + 1] << 8));
-    __syncthreads();
-    return s;
-}
-
-static size_t l1_smem_bytes(const dagr_geom_t *g)
-{
-    return (size_t)g->ncell * DAGR_TABW * 4 + (size_t)(g->W + g->H) * 4 + (size_t)g->ncell * 2 + 16;
-}
-
-__device__ __forceinline__ void load_tab(const float *row, float w[DAGR_KU])
-{
-    static_assert(DAGR_KU == 15 && DAGR_TABW == 16, "table row layout");
-    const float4 a = *reinterpret_cast<const float4 *>(row);
-    const float4 b = *reinterpret_cast<const float4 *>(row + 4);
-    const float4 c = *reinterpret_cast<const float4 *>(row + 8);
-    const float4 d = *reinterpret_cast<const float4 *>(row + 12);
-    w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
-    w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-    w[8] = c.x; w[9] = c.y; w[10] = c.z; w[11] = c.w;
-    w[12] = d.x; w[13] = d.y; w[14] = d.z;
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv_a
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(L1_THREADS)
-k_l1_conv_a(const dagr_geom_t g, int64_t N, const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
-            const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off, const float *__restrict__ tab,
-            const __grid_constant__ dagr_l1a_params_t P, float *__restrict__ xa)
-{
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const L1Smem s = l1_smem_init(g, tab, smem_raw);
-    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= N) return;
-
-    const uint32_t w = xyb[p];
-    const int x = w & 0xfff, y = (w >> 12) & 0xfff;
-    const float f0 = feat_s[p], f1 = s.posx[x], f2 = s.posy[y];
-    const int n = nbr[(int64_t)(DAGR_ELL - 1) * N + p];
-
-    float A[DAGR_KU][3];
-    {
-        float t[DAGR_KU];
-        load_tab(s.tab, t);                                   // self loop: spiral cell 0, attr (0.5,0.5)
-#pragma unroll
-        for (int u = 0; u < DAGR_KU; u++) { A[u][0] = t[u] * f0; A[u][1] = t[u] * f1; A[u][2] = t[u] * f2; }
-    }
-    for (int q = 0; q < n; q++) {
-        const int j = nbr[(int64_t)q * N + p];
-        const int c = off[(int64_t)q * N + p];
-        const int sp = s.sp[c];
-        const float e0 = __ldg(feat_s + j);
-        const float e1 = s.posx[x + (int)(signed char)(sp & 0xff)];
-        const float e2 = s.posy[y + (sp >> 8)];
-        float t[DAGR_KU];
-        load_tab(s.tab + c * DAGR_TABW, t);
-#pragma unroll
-        for (int u = 0; u < DAGR_KU; u++) {
-            A[u][0] = fmaf(t[u], e0, A[u][0]);
-            A[u][1] = fmaf(t[u], e1, A[u][1]);
-            A[u][2] = fmaf(t[u], e2, A[u][2]);
-        }
-    }
-    float o[16];
-#pragma unroll
-    for (int k = 0; k < 16; k++) o[k] = 0.f;
-#pragma unroll
-    for (int u = 0; u < DAGR_KU; u++)
-#pragma unroll
-        for (int ci = 0; ci < 3; ci++)
-#pragma unroll
-            for (int k = 0; k < 16; k++) o[k] = fmaf(A[u][ci], P.w[u][ci][k], o[k]);
-#pragma unroll
-    for (int k = 0; k < 16; k++) {
-        float r = o[k];
-        r = fmaf(f0, P.root[0][k], r);
-        r = fmaf(f1, P.root[1][k], r);
-        r = fmaf(f2, P.root[2][k], r);
-        r = fmaf(r, P.scale[k], P.shift[k]);
-        o[k] = P.relu ? fmaxf(r, 0.f) : r;
-    }
-    // xa is stored half-major: [2][N][8] (channels 0-7, then 8-15), see conv_b v2
-    const int sw = XA_SWZ(p);
-    float4 *dst = reinterpret_cast<float4 *>(xa + p * 8);
-    dst[sw] = make_float4(o[0], o[1], o[2], o[3]);
-    dst[sw ^ 1] = make_float4(o[4], o[5], o[6], o[7]);
-    dst = reinterpret_cast<float4 *>(xa + (N + p) * 8);
-    dst[sw] = make_float4(o[8], o[9], o[10], o[11]);
-    dst[sw ^ 1] = make_float4(o[12], o[13], o[14], o[15]);
-}
-
-extern "C" int dagr_l1_conv_a(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
-                              const int32_t *nbr, const uint16_t *off, const float *tab,
-                              const dagr_l1a_params_t *p_host, float *xa, void *stream)
-{
-    DAGR_CHECK_ARG(g && p_host, "null argument");
-    if (N <= 0) return DAGR_OK;
-    size_t smem = l1_smem_bytes(g);
-    DAGR_CUDA(dagr_allow_smem(k_l1_conv_a, smem));
-    k_l1_conv_a<<<dagr_div_up(N, L1_THREADS), L1_THREADS, smem, (cudaStream_t)stream>>>(
-        *g, N, xyb, feat_s, nbr, off, tab, *p_host, xa);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv_b + skip + act + pool1 max
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(L1_THREADS)
-k_l1_conv_b(const dagr_geom_t g, int64_t N, const uint32_t *__restrict__ xyb, const float *__restrict__ feat_s,
-            const float *__restrict__ xa, const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
-            const float *__restrict__ tab, const __grid_constant__ dagr_l1b_params_t P,
-            float *__restrict__ x1, uint32_t *__restrict__ poolmax)
-{
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const L1Smem s = l1_smem_init(g, tab, smem_raw);
-    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool active = p < N;
-    float o[16];
-#pragma unroll
-    for (int k = 0; k < 16; k++) o[k] = 0.f;
-    int cell = -1;
-    if (active) {
-        const uint32_t w = xyb[p];
-        const int x = w & 0xfff, y = (w >> 12) & 0xfff, b = w >> 24;
-        cell = b * (g.ny1 * g.nx1) + (__ldg(g.ykey + y) / (g.nx1 * g.CP)) * g.nx1 + __ldg(g.xkey + x) / g.CP;
-        const int n = nbr[(int64_t)(DAGR_ELL - 1) * N + p];
-
-        // Two passes over the input-channel halves keep the slot accumulators A[15][8] in registers
-        // (15 of the 25 spline kernels are reachable: 3 in x, 5 in y because attr_y is normalised by H).
-#pragma unroll 1
-        for (int half = 0; half < 2; half++) {
-            float2 A[DAGR_KU][4];
-            {
-                // self loop (spiral cell 0) and root weight: own row
-                const float4 *src = reinterpret_cast<const float4 *>(xa + ((int64_t)half * N + p) * 8);
-                const float4 t0 = src[XA_SWZ(p)], t1 = src[XA_SWZ(p) ^ 1];
-                const float2 v[4] = {make_float2(t0.x, t0.y), make_float2(t0.z, t0.w), make_float2(t1.x, t1.y), make_float2(t1.z, t1.w)};
-                float t[DAGR_KU];
-                load_tab(s.tab, t);
-#pragma unroll
-                for (int u = 0; u < DAGR_KU; u++)
-#pragma unroll
-                    for (int k = 0; k < 4; k++) A[u][k] = make_float2(t[u] * v[k].x, t[u] * v[k].y);
-                if (half == 0) {
-#pragma unroll
-                    for (int k = 0; k < 4; k++)
-#pragma unroll
-                        for (int c = 0; c < 16; c++) {
-                            o[c] = fmaf(v[k].x, P.root[2 * k][c], o[c]);
-                            o[c] = fmaf(v[k].y, P.root[2 * k + 1][c], o[c]);
-                        }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 4; k++)
-#pragma unroll
-                        for (int c = 0; c < 16; c++) {
-                            o[c] = fmaf(v[k].x, P.root[8 + 2 * k][c], o[c]);
-                            o[c] = fmaf(v[k].y, P.root[8 + 2 * k + 1][c], o[c]);
-                        }
-                }
-            }
-            // phase 1: gather neighbours
-            for (int q = 0; q < n; q++) {
-                const int j = nbr[(int64_t)q * N + p];
-                const int c = off[(int64_t)q * N + p];
-                const float4 *src = reinterpret_cast<const float4 *>(xa + ((int64_t)half * N + j) * 8);
-                const float4 t0 = __ldg(src + XA_SWZ(j)), t1 = __ldg(src + (XA_SWZ(j) ^ 1));
-                const float2 e[4] = {make_float2(t0.x, t0.y), make_float2(t0.z, t0.w), make_float2(t1.x, t1.y), make_float2(t1.z, t1.w)};
-                float t[DAGR_KU];
-                load_tab(s.tab + c * DAGR_TABW, t);
-#pragma unroll
-                for (int u = 0; u < DAGR_KU; u++) {
-                    const float2 tt = make_float2(t[u], t[u]);
-#pragma unroll
-                    for (int k = 0; k < 4; k++) A[u][k] = ffma2(tt, e[k], A[u][k]);
-                }
-            }
-            // phase 2: o += sum_u W_u^T A_u   (weights from the constant bank, uniform across the warp)
-            if (half == 0) {
-#pragma unroll
-                for (int u = 0; u < DAGR_KU; u++)
-#pragma unroll
-                    for (int k = 0; k < 4; k++)
-#pragma unroll
-                        for (int c = 0; c < 16; c++) {
-                            o[c] = fmaf(A[u][k].x, P.w[u][2 * k][c], o[c]);
-                            o[c] = fmaf(A[u][k].y, P.w[u][2 * k + 1][c], o[c]);
-                        }
-            } else {
-#pragma unroll
-                for (int u = 0; u < DAGR_KU; u++)
-#pragma unroll
-                    for (int k = 0; k < 4; k++)
-#pragma unroll
-                        for (int c = 0; c < 16; c++) {
-                            o[c] = fmaf(A[u][k].x, P.w[u][8 + 2 * k][c], o[c]);
-                            o[c] = fmaf(A[u][k].y, P.w[u][8 + 2 * k + 1][c], o[c]);
-                        }
-            }
-        }
-        // BN, skip branch BN(Linear(x0)), add, act  (conv.py:47-56)
-        const float f0 = feat_s[p], f1 = s.posx[x], f2 = s.posy[y];
-#pragma unroll
-        for (int c = 0; c < 16; c++) {
-            float sk = f0 * P.skip[0][c];
-            sk = fmaf(f1, P.skip[1][c], sk);
-            sk = fmaf(f2, P.skip[2][c], sk);
-            sk = fmaf(sk, P.sscale[c], P.sshift[c]);
-            float r = fmaf(o[c], P.scale[c], P.shift[c]) + sk;
-            o[c] = P.relu ? fmaxf(r, 0.f) : r;
-        }
-        if (x1 != nullptr) {
-            float4 *dst = reinterpret_cast<float4 *>(x1 + p * 16);
-            dst[0] = make_float4(o[0], o[1], o[2], o[3]);
-            dst[1] = make_float4(o[4], o[5], o[6], o[7]);
-            dst[2] = make_float4(o[8], o[9], o[10], o[11]);
-            dst[3] = make_float4(o[12], o[13], o[14], o[15]);
-        }
-    }
-    // pool1 max: nodes of one voxel are contiguous -> warp-segmented max, heads publish with atomicMax
-    if (poolmax != nullptr) {
-        const int lane = threadIdx.x & 31;
-        uint32_t eo[16];
-#pragma unroll
-        for (int c = 0; c < 16; c++) eo[c] = active ? enc_ordered(o[c]) : 0u;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const int oc = __shfl_down_sync(0xffffffffu, cell, d);
-            const bool take = (lane + d < 32) && (oc == cell);
-#pragma unroll
-            for (int c = 0; c < 16; c++) {
-                const uint32_t ov = __shfl_down_sync(0xffffffffu, eo[c], d);
-                if (take) eo[c] = max(eo[c], ov);
-            }
-        }
-        const int pc = __shfl_up_sync(0xffffffffu, cell, 1);
-        const bool head = active && (lane == 0 || pc != cell);
-        if (head) {
-            uint32_t *dst = poolmax + (int64_t)cell * 16;
-#pragma unroll
-            for (int c = 0; c < 16; c++) atomicMax(dst + c, eo[c]);
-        }
-    }
-}
-
-extern "C" int dagr_l1_conv_b_pool(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
-                                   const float *xa, const int32_t *nbr, const uint16_t *off, const float *tab,
-                                   const dagr_l1b_params_t *p_host, float *x1, uint32_t *poolmax, void *stream)
-{
-    DAGR_CHECK_ARG(g && p_host, "null argument");
-    DAGR_CHECK_ARG(p_host->pool_mean == 0, "mean pooling needs the per-voxel kernel (dagr_l1_conv_b_pool_voxel)");
-    if (N <= 0) return DAGR_OK;
-    size_t smem = l1_smem_bytes(g);
-    DAGR_CUDA(dagr_allow_smem(k_l1_conv_b, smem));
-    k_l1_conv_b<<<dagr_div_up(N, L1_THREADS), L1_THREADS, smem, (cudaStream_t)stream>>>(
-        *g, N, xyb, feat_s, xa, nbr, off, tab, *p_host, x1, poolmax);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
 // ================================================================================================
-// conv_b v2: one CTA per pool1 voxel, neighbour rows staged in shared memory by TMA bulk copies
+// conv_b: one CTA per pool1 voxel, neighbour rows staged in shared memory by TMA bulk copies
 // ================================================================================================
 // Because nodes are stored in cell-major order, the xa rows any node of the voxel can gather are the
 // rows of its 3x3 voxel neighbourhood = THREE contiguous runs.  One elected thread issues three
@@ -354,10 +70,10 @@ struct CB2Tile {
     int run_start[3], run_len[3], run_off[3];
 };
 
-// ---- phase 2 on tensor cores (CB2_TC = 1) ------------------------------------------------------------------------------
+// ---- phase 2 on tensor cores ------------------------------------------------------------------------------------------
 // Phase 2 of a pass is a dense product with node-independent weights, [32 nodes of a warp x 40] x [40 x 16]: on CUDA cores it
-// costs as many issue slots as the edge loop (every FFMA needs its weight through a uniform constant load on sm_90).  With
-// CB2_TC it runs as mma.sync.m16n8k8 TF32 in 3xTF32 form (a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, hi = cvt.rna.tf32(x),
+// costs as many issue slots as the edge loop (every FFMA needs its weight through a uniform constant load on sm_90).  It
+// runs as mma.sync.m16n8k8 TF32 in 3xTF32 form (a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, hi = cvt.rna.tf32(x),
 // lo = x - hi; relative error ~1e-6): the warp's 32 nodes are two m16 tiles, the 16 outputs two n8 tiles, one k8 step per
 // spline slot (8 channels of the current half) plus one per half for the root weight.  o2[8] then holds the FP32 C fragments
 // across all passes: o2[4 mt + 2 nt] = (c0, c1), o2[4 mt + 2 nt + 1] = (c2, c3) of m-tile mt, n-tile nt.  An output element
@@ -366,10 +82,7 @@ struct CB2Tile {
 // float4 [half][k-step: slot 0..14, root = 15][lane][n-tile] = (hi k=t, hi k=t+4, lo k=t, lo k=t+4), t = lane & 3.
 // Phase 1 leaves one node per lane; the A fragment needs other lanes' values, which go through a 256-byte per-warp tile
 // (16 rows x 4 floats: one m-tile and half a k-step at a time, so that four CTAs still fit an SM).
-#ifndef CB2_TC
-#define CB2_TC 1
-#endif
-#define CB2_TC_KSTEPS 16                   // per channel half: 15 spline slots + root
+#define CB2_KSTEPS 16                   // per channel half: 15 spline slots + root
 
 // o2 (C fragments) += [this warp's nodes x 8] x [8 x 16]; this lane's node contributes a[0..7], wf = this k-step's fragments
 // of this lane.  Warp-uniform call; lanes without a node pass zeros.  (tf32_split / mma_3xtf32 / ldsm_*: common.cuh)
@@ -432,19 +145,18 @@ __device__ __forceinline__ void cb2_tc_unfrag(float *xt, float2 o2[8])
 //     o  += sum_j W_{k+3j}[half]^T A_j
 // The slot weights are rebuilt from the two per-axis factor tables (2r+1 rows each, geometry.py) instead of a
 // [ncell][16] table: 1.5 KB instead of 21 KB of shared memory per CTA, which is what lets four CTAs share an SM.
-// `half` and `k` are template parameters so the phase-2 weights come through the uniform datapath (LDCU.128);
-// a run-time pass index makes ptxas fetch them with register-indexed LDC, which saturates the ADU pipe.
+// `half` and `grp` are template parameters, so the offsets of the weight fragments and factor tables are compile-time constants.
 // s_ell[q][tid]: see the staged loop below (byte offsets of the row chunks and of the two factor-table rows).
 // Variants measured and rejected (ELL entries ordered by the x-slots they feed so that the outer x-slot passes skip their
 // exact-zero edges: slower, the per-lane loop bounds cost more than the skipped iterations save): 15 slots x 8 channels per pass (120
 // accumulators, 2 CTAs/SM), 15 slots x 4 channels, phase-2 weights from shared memory or half/half.
-// With TC, phase 2 runs on tensor cores (see cb2_tc_kstep) and o2 holds C fragments; the call is then warp-uniform and a lane
-// without a node passes n = -1 (no edge, A = 0).
-template <bool STAGED, int half, int grp, int THREADS, bool TC, class PT>
+// Phase 2 runs on tensor cores (see cb2_tc_kstep) and o2 holds C fragments; the call is warp-uniform and a lane without a node
+// passes n = -1 (no edge, A = 0).
+template <bool STAGED, int half, int grp, int THREADS>
 __device__ __forceinline__ void cb2_pass(int64_t N, int p, int n, const float *__restrict__ xa, const float *s_rows,
                                          const float *s_wx, const float4 *s_wy, const float *s_wy4, const uint32_t *s_ell, const uint16_t *s_sp,
                                          const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
-                                         const PT &P, const float4 *__restrict__ wfrag, float *xt, int own_row, int r, int tix, float2 o2[8])
+                                         const float4 *__restrict__ wfrag, float *xt, int own_row, int r, int tix, float2 o2[8])
 {
     float2 A[CB2_G][4];
 #pragma unroll
@@ -508,11 +220,12 @@ __device__ __forceinline__ void cb2_pass(int64_t N, int p, int n, const float *_
         }
     }
 #undef CB2_EDGE_FMA
-    if constexpr (TC) {
+    {
         // phase 2 on tensor cores: k-step j = spline slot grp + 3 j, k = channel of this half
         // The pass sums into fresh fragments which are then added to o2 with IEEE fp32 adds: the tensor cores' fp32
         // accumulation truncates, and chaining all 6 passes x 15 mma through it doubled the largest errors against the oracle.
-        const float4 *wf = wfrag + ((size_t)half * CB2_TC_KSTEPS * 32 + (threadIdx.x & 31)) * 2;
+        // (The block scope ends the fragments' lifetime here; without it ptxas assigns registers differently.)
+        const float4 *wf = wfrag + ((size_t)half * CB2_KSTEPS * 32 + (threadIdx.x & 31)) * 2;
         float2 c2[8];
 #pragma unroll
         for (int i = 0; i < 8; i++) c2[i] = make_float2(0.f, 0.f);
@@ -523,39 +236,7 @@ __device__ __forceinline__ void cb2_pass(int64_t N, int p, int n, const float *_
         }
 #pragma unroll
         for (int i = 0; i < 8; i++) o2[i] = make_float2(__fadd_rn(o2[i].x, c2[i].x), __fadd_rn(o2[i].y, c2[i].y));
-        return;
     }
-    // phase 2: weights from the constant bank through uniform 128-bit loads, two FFMA2 per load
-#pragma unroll
-    for (int j = 0; j < CB2_G; j++)
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-#pragma unroll
-            for (int c4 = 0; c4 < 4; c4++) {
-                const float4 wa = *reinterpret_cast<const float4 *>(&P.w[grp + 3 * j][8 * half + 2 * k][4 * c4]);
-                const float4 wb = *reinterpret_cast<const float4 *>(&P.w[grp + 3 * j][8 * half + 2 * k + 1][4 * c4]);
-                o2[2 * c4] = ffma2(make_float2(A[j][k].x, A[j][k].x), make_float2(wa.x, wa.y), o2[2 * c4]);
-                o2[2 * c4 + 1] = ffma2(make_float2(A[j][k].x, A[j][k].x), make_float2(wa.z, wa.w), o2[2 * c4 + 1]);
-                o2[2 * c4] = ffma2(make_float2(A[j][k].y, A[j][k].y), make_float2(wb.x, wb.y), o2[2 * c4]);
-                o2[2 * c4 + 1] = ffma2(make_float2(A[j][k].y, A[j][k].y), make_float2(wb.z, wb.w), o2[2 * c4 + 1]);
-            }
-}
-
-__device__ __forceinline__ float cb2_div_floor(float a, float b)
-{
-    const float mod = fmodf(a, b);
-    float div = __fdiv_rn(__fsub_rn(a, mod), b);
-    if ((mod != 0.f) && ((b < 0.f) != (mod < 0.f))) div -= 1.f;
-    float fl;
-    if (div != 0.f) { fl = floorf(div); if (div - fl > 0.5f) fl += 1.f; }
-    else fl = copysignf(0.f, __fdiv_rn(a, b));
-    return fl;
-}
-__device__ __forceinline__ int cb2_round_to_pixel(float mean, int size)
-{
-    const float inv = __frcp_rn((float)size);
-    const int k = (int)cb2_div_floor(__fadd_rn(mean, 1e-5f), inv);
-    return min(max(k, 0), size - 1);
 }
 
 // The kernel is a template over the input rows: <dagr_l1b_params_t, 2, false> is conv_block2 (16 channels = 2 staged
@@ -580,7 +261,7 @@ struct CB2Shared {
 // chunk-major for conv_block2, plus the layer's skip branch BN(Linear(x0)) -> skip_out; no pooling).
 // work list: wl_hdr[0] = number of voxels beyond this instance's staging capacity (queued in wl_ids when `defer`, otherwise
 // only counted and gathered from global memory / L2), wl_hdr[1] = pop cursor of the dense kernel
-template <class PT, int NCH, bool MODE_A, int CAP, int THREADS, bool POOL_MEAN, bool PLAIN, bool TC>
+template <class PT, int NCH, bool MODE_A, int CAP, int THREADS, bool POOL_MEAN, bool PLAIN>
 __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
              const int2 *__restrict__ ti, const float *__restrict__ feat_s, const float *__restrict__ xa,
              const int32_t *__restrict__ nbr, const uint16_t *__restrict__ off,
@@ -724,11 +405,12 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
                 mbar_wait(&s_bar, parity);                              // (one waiting thread + a CTA barrier instead: slower)
                 parity ^= 1;
             }
-            // with TC the warp's lanes run the passes together (mma.sync): a lane without a node joins with no edges
-            if (TC ? __any_sync(0xffffffffu, active) : active) {
+            // the warp's lanes run the passes together (mma.sync): a lane without a node joins with no edges
+            if (__any_sync(0xffffffffu, active)) {
                 const int nn = active ? n : -1;
-                // root weight on this half of x_i.  `half` must be a compile-time constant here as well: with a run-time index
-                // the 64 weight fetches per half become register-indexed LDC through the address-divergence unit
+                // root weight (and with MODE_A the skip weights) on this half of x_i.  `half` must be a compile-time constant here as
+                // well: with a run-time index the 64 skip-weight fetches per half become register-indexed LDC through the
+                // address-divergence unit
 #define CB2_ROOT(H)                                                                                                  \
     do {                                                                                                            \
         const float4 *src = staged ? reinterpret_cast<const float4 *>(s_rows + (int64_t)(p + d1) * 8)               \
@@ -736,20 +418,13 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
         const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);                                                         \
         const float4 t0 = active ? src[XA_SWZ(p)] : z4, t1 = active ? src[XA_SWZ(p) ^ 1] : z4;                      \
         const float v[8] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w};                                        \
-        if constexpr (TC) {                                                                                         \
-            float2 c2[8];                                                                                           \
-            _Pragma("unroll") for (int i = 0; i < 8; i++) c2[i] = make_float2(0.f, 0.f);                            \
-            cb2_tc_kstep(xt, v, wfrag + (((H) * CB2_TC_KSTEPS + 15) * 32 + lane_) * 2, c2);                         \
-            _Pragma("unroll") for (int i = 0; i < 8; i++)                                                           \
-                o2[i] = make_float2(__fadd_rn(o2[i].x, c2[i].x), __fadd_rn(o2[i].y, c2[i].y));                      \
-        }                                                                                                           \
+        float2 c2[8];                                                                                               \
+        _Pragma("unroll") for (int i = 0; i < 8; i++) c2[i] = make_float2(0.f, 0.f);                                \
+        cb2_tc_kstep(xt, v, wfrag + (((H) * CB2_KSTEPS + 15) * 32 + lane_) * 2, c2);                             \
+        _Pragma("unroll") for (int i = 0; i < 8; i++)                                                               \
+            o2[i] = make_float2(__fadd_rn(o2[i].x, c2[i].x), __fadd_rn(o2[i].y, c2[i].y));                          \
         _Pragma("unroll") for (int k = 0; k < 8; k++)                                                               \
             _Pragma("unroll") for (int c4 = 0; c4 < 4; c4++) {                                                      \
-                if constexpr (!TC) {                                                                                \
-                    const float4 w4 = *reinterpret_cast<const float4 *>(&P.root[8 * (H) + k][4 * c4]);              \
-                    o2[2 * c4] = ffma2(make_float2(v[k], v[k]), make_float2(w4.x, w4.y), o2[2 * c4]);               \
-                    o2[2 * c4 + 1] = ffma2(make_float2(v[k], v[k]), make_float2(w4.z, w4.w), o2[2 * c4 + 1]);       \
-                }                                                                                                   \
                 if constexpr (MODE_A) {                 /* the layer's skip branch Linear(x0) (conv.py:41-52) */    \
                     const float4 k4 = *reinterpret_cast<const float4 *>(&P.skip[8 * (H) + k][4 * c4]);              \
                     sk2[2 * c4] = ffma2(make_float2(v[k], v[k]), make_float2(k4.x, k4.y), sk2[2 * c4]);             \
@@ -765,8 +440,8 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
 #undef CB2_ROOT
 #define CB2_PASS(H, G)                                                                                               \
     do {                                                                                                            \
-        if (staged) cb2_pass<true, H, G, THREADS, TC>(N, p, nn, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, P, wfrag, xt, p + d1, g.r, tix, o2); \
-        else        cb2_pass<false, H, G, THREADS, TC>(N, p, nn, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, P, wfrag, xt, 0, g.r, tix, o2);     \
+        if (staged) cb2_pass<true, H, G, THREADS>(N, p, nn, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, wfrag, xt, p + d1, g.r, tix, o2); \
+        else        cb2_pass<false, H, G, THREADS>(N, p, nn, xa, s_rows, s_wx, s_wy, s_wy4, s_ell, s_sp, nbr, off, wfrag, xt, 0, g.r, tix, o2);     \
     } while (0)
 #define CB2_HALF(H)                                                                                                  \
     do {                                                                                                            \
@@ -782,9 +457,7 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
 #undef CB2_PASS
             }
         }
-        if constexpr (TC) {
-            if (__any_sync(0xffffffffu, active)) cb2_tc_unfrag(xt, o2);
-        }
+        if (__any_sync(0xffffffffu, active)) cb2_tc_unfrag(xt, o2);
         if (sparse) {
             // add the partial sums of warps 1 and 2 (x-slots 1 and 2) to warp 0's: the staged rows are dead by now
             __syncthreads();
@@ -930,15 +603,15 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
         const float mx = (float)((double)ax / ((double)nown * (double)g.W));
         const float my = (float)((double)ay / ((double)nown * (double)g.H));
         cnt[cell] = nown;
-        pxy[2 * cell] = cb2_round_to_pixel(mx, g.W);
-        pxy[2 * cell + 1] = cb2_round_to_pixel(my, g.H);
+        pxy[2 * cell] = round_to_pixel(mx, g.W);
+        pxy[2 * cell + 1] = round_to_pixel(my, g.H);
         tmean[cell] = (float)((double)at / ((double)nown * (double)g.T));
         tmax[cell] = __fdiv_rn((float)tmx, (float)g.T);
     }
 }
 
 
-template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN, bool TC>
+template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN>
 __global__ void __launch_bounds__(CB2_THREADS, MODE_A ? 3 : 4)       // (3 CTAs / 128 registers, no spills: slower)
 k_l1_conv_b2(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
              const int2 *__restrict__ ti, const float *__restrict__ feat_s, const float *__restrict__ xa,
@@ -949,17 +622,17 @@ k_l1_conv_b2(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, 
              float *__restrict__ xa_out, float *__restrict__ skip_out, int32_t *__restrict__ wl_hdr, int32_t *__restrict__ wl_ids,
              const int defer)
 {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
+    extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ __align__(16) CB2Shared<CB2_THREADS> S;
     if (threadIdx.x == 0) mbar_init(&S.bar, 1);                         // made visible by the routine's first __syncthreads
     uint32_t parity = 0;
-    cb2_voxel<PT, NCH, MODE_A, CB2_CAP, CB2_THREADS, POOL_MEAN, PLAIN, TC>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, wfrag, skip_pre, min_idx,
+    cb2_voxel<PT, NCH, MODE_A, CB2_CAP, CB2_THREADS, POOL_MEAN, PLAIN>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, wfrag, skip_pre, min_idx,
                                                       persist, x1, cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out, (int)blockIdx.x,
                                                       smem_raw, S, parity, wl_hdr, wl_ids, defer);
 }
 
 // dense voxels: persistent CTAs (one per SM) pop voxel ids from the work list the regular kernel filled
-template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN, bool TC>
+template <class PT, int NCH, bool MODE_A, bool POOL_MEAN, bool PLAIN>
 __global__ void __launch_bounds__(CB2_THREADS_BIG, 1)
 k_l1_conv_b2_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
                    const int2 *__restrict__ ti, const float *__restrict__ feat_s, const float *__restrict__ xa,
@@ -969,7 +642,7 @@ k_l1_conv_b2_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ s
                    float *__restrict__ tmean, float *__restrict__ tmax, float *__restrict__ xg, int ldx,
                    float *__restrict__ xa_out, float *__restrict__ skip_out, int32_t *__restrict__ wl_hdr, const int32_t *__restrict__ wl_ids)
 {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
+    extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ __align__(16) CB2Shared<CB2_THREADS_BIG> S;
     __shared__ int s_next;
     if (threadIdx.x == 0) mbar_init(&S.bar, 1);
@@ -981,7 +654,7 @@ k_l1_conv_b2_dense(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ s
         __syncthreads();
         const int i = s_next;
         if (i >= count) break;
-        cb2_voxel<PT, NCH, MODE_A, CB2_CAP_BIG, CB2_THREADS_BIG, POOL_MEAN, PLAIN, TC>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, wfrag, skip_pre,
+        cb2_voxel<PT, NCH, MODE_A, CB2_CAP_BIG, CB2_THREADS_BIG, POOL_MEAN, PLAIN>(g, N, start, xyb, ti, feat_s, xa, nbr, off, P, wfrag, skip_pre,
                                                                   min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out,
                                                                   wl_ids[i], smem_raw, S, parity, nullptr, nullptr, 0);
     }
@@ -992,7 +665,7 @@ static size_t cb2_smem_bytes(const dagr_geom_t *g, int cap, int threads)
     return (size_t)cap * 32 + 96 * 16 + (size_t)DAGR_ELL * threads * 4 + (size_t)g->ncell * 2 + 32;
 }
 
-template <class PT, int NCH, bool MODE_A, bool TC, bool POOL_MEAN = false, bool PLAIN = false>
+template <class PT, int NCH, bool MODE_A, bool POOL_MEAN = false, bool PLAIN = false>
 static int cb2_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int2 *ti, const float *feat_s,
                       const float *xa, const int32_t *nbr, const uint16_t *off, const PT *p_host, const float4 *wfrag, const float *skip_pre,
                       int min_idx, float *persist, float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx,
@@ -1000,7 +673,7 @@ static int cb2_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, con
 {
     const int cells = g->B * g->ny1 * g->nx1;
     const size_t smem = cb2_smem_bytes(g, CB2_CAP, CB2_THREADS);
-    auto kern = k_l1_conv_b2<PT, NCH, MODE_A, POOL_MEAN, PLAIN, TC>;
+    auto kern = k_l1_conv_b2<PT, NCH, MODE_A, POOL_MEAN, PLAIN>;
     DAGR_CUDA(dagr_allow_smem(kern, smem, true));
     kern<<<cells, CB2_THREADS, smem, st>>>(*g, N, start, xyb, ti, feat_s, xa, nbr, off, *p_host, wfrag, skip_pre, min_idx, persist, x1, cnt,
                                            pxy, tmean, tmax, xg, ldx, xa_out, skip_out, wl_hdr, wl_ids,
@@ -1014,7 +687,7 @@ static int cb2_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, con
             DAGR_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
         }
         const size_t smem_big = cb2_smem_bytes(g, CB2_CAP_BIG, CB2_THREADS_BIG);
-        auto kd = k_l1_conv_b2_dense<PT, NCH, MODE_A, POOL_MEAN, PLAIN, TC>;
+        auto kd = k_l1_conv_b2_dense<PT, NCH, MODE_A, POOL_MEAN, PLAIN>;
         DAGR_CUDA(dagr_allow_smem(kd, smem_big));
         kd<<<n_sm, CB2_THREADS_BIG, smem_big, st>>>(*g, N, start, xyb, ti, feat_s, xa, nbr, off, *p_host, wfrag, skip_pre, min_idx, persist,
                                                     x1, cnt, pxy, tmean, tmax, xg, ldx, xa_out, skip_out, wl_hdr, wl_ids);
@@ -1023,83 +696,45 @@ static int cb2_launch(const dagr_geom_t *g, int64_t N, const int32_t *start, con
     return DAGR_OK;
 }
 
-template <bool TC>
-static int conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
-                             const float *feat_s, const float *xa, const int32_t *nbr, const uint16_t *off, const dagr_l1b_params_t *p_host,
-                             const float4 *wfrag, const float *skip_pre, int min_idx, float *persist, float *x1, int32_t *cnt,
-                             int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx, int32_t *wl_hdr, int32_t *wl_ids, int defer,
-                             cudaStream_t st)
-{
-    DAGR_CHECK_ARG(g && p_host, "null argument");
-    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
-    DAGR_CHECK_ARG(!(p_host->pool_mean && persist), "the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
-    if (p_host->pool_mean)
-        return cb2_launch<dagr_l1b_params_t, 2, false, TC, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag,
-                                                                 skip_pre, min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr,
-                                                                 nullptr, wl_hdr, wl_ids, defer, st);
-    if (min_idx <= 0 && persist == nullptr && x1 == nullptr && skip_pre == nullptr && p_host->relu)
-        return cb2_launch<dagr_l1b_params_t, 2, false, TC, false, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag,
-                                                                        nullptr, 0, nullptr, nullptr, cnt, pxy, tmean, tmax, xg, ldx, nullptr,
-                                                                        nullptr, wl_hdr, wl_ids, defer, st);
-    return cb2_launch<dagr_l1b_params_t, 2, false, TC>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag, skip_pre,
-                                                       min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr, nullptr, wl_hdr, wl_ids,
-                                                       defer, st);
-}
-
-extern "C" int dagr_l1_conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
-                                         const int32_t *ti, const float *feat_s, const float *xa, const int32_t *nbr,
-                                         const uint16_t *off, const float *tab, const dagr_l1b_params_t *p_host,
-                                         const float *skip_pre, int min_idx, float *persist, float *x1, int32_t *cnt,
-                                         int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx, int32_t *wl_hdr, int32_t *wl_ids,
-                                         int defer, void *stream)
-{
-    (void)tab;
-    return conv_b_pool_voxel<false>(g, N, start, xyb, ti, feat_s, xa, nbr, off, p_host, nullptr, skip_pre, min_idx, persist, x1, cnt, pxy,
-                                    tmean, tmax, xg, ldx, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
-}
-
 extern "C" int dagr_l1_conv_b_pool_voxel_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
                                             const int32_t *ti, const float *feat_s, const float *xa, const int32_t *nbr,
-                                            const uint16_t *off, const dagr_l1b_params_t *p_host, const float *wfrag,
+                                            const uint16_t *off, const dagr_l1b_params_t *p_host, const float *wfrag_f,
                                             const float *skip_pre, int min_idx, float *persist, float *x1, int32_t *cnt,
                                             int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx, int32_t *wl_hdr, int32_t *wl_ids,
                                             int defer, void *stream)
 {
-    DAGR_CHECK_ARG(wfrag, "null weight fragments (dagr_l1_tc_weights)");
-    return conv_b_pool_voxel<CB2_TC != 0>(g, N, start, xyb, ti, feat_s, xa, nbr, off, p_host, (const float4 *)wfrag, skip_pre, min_idx,
-                                          persist, x1, cnt, pxy, tmean, tmax, xg, ldx, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
+    DAGR_CHECK_ARG(wfrag_f, "null weight fragments (dagr_l1_tc_weights)");
+    DAGR_CHECK_ARG(g && p_host, "null argument");
+    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
+    DAGR_CHECK_ARG(!(p_host->pool_mean && persist), "the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
+    const float4 *wfrag = (const float4 *)wfrag_f;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p_host->pool_mean)
+        return cb2_launch<dagr_l1b_params_t, 2, false, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag,
+                                                             skip_pre, min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr,
+                                                             nullptr, wl_hdr, wl_ids, defer, st);
+    if (min_idx <= 0 && persist == nullptr && x1 == nullptr && skip_pre == nullptr && p_host->relu)
+        return cb2_launch<dagr_l1b_params_t, 2, false, false, true>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag,
+                                                                    nullptr, 0, nullptr, nullptr, cnt, pxy, tmean, tmax, xg, ldx, nullptr,
+                                                                    nullptr, wl_hdr, wl_ids, defer, st);
+    return cb2_launch<dagr_l1b_params_t, 2, false>(g, N, start, xyb, (const int2 *)ti, feat_s, xa, nbr, off, p_host, wfrag, skip_pre,
+                                                   min_idx, persist, x1, cnt, pxy, tmean, tmax, xg, ldx, nullptr, nullptr, wl_hdr, wl_ids,
+                                                   defer, st);
 }
 
 // image fusion: the 16 image channels of conv_block1.conv_block1 (x0 chunk-major [2][N][8], chunks swizzled like xa) on top
 // of the event-channel sums the probe kernel left in xa
-template <bool TC>
-static int conv_a_image(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s, const float *x0,
-                        const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host, const float4 *wfrag, float *xa,
-                        float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, cudaStream_t st)
-{
-    DAGR_CHECK_ARG(g && p_host && xyb && feat_s, "null argument");
-    if (N <= 0) return DAGR_OK;
-    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
-    return cb2_launch<dagr_l1img_params_t, 2, true, TC>(g, N, start, xyb, nullptr, feat_s, x0, nbr, off, p_host, wfrag, nullptr, 0, nullptr,
-                                                        nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr, wl_ids,
-                                                        defer, st);
-}
-
-extern "C" int dagr_l1_conv_a_image(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
-                                    const float *x0, const int32_t *nbr,
-                                    const uint16_t *off, const dagr_l1img_params_t *p_host, float *xa, float *skipv,
-                                    int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
-{
-    return conv_a_image<false>(g, N, start, xyb, feat_s, x0, nbr, off, p_host, nullptr, xa, skipv, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
-}
-
 extern "C" int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
                                        const float *x0, const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host,
                                        const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
 {
     DAGR_CHECK_ARG(wfrag, "null weight fragments (dagr_l1_tc_weights)");
-    return conv_a_image<CB2_TC != 0>(g, N, start, xyb, feat_s, x0, nbr, off, p_host, (const float4 *)wfrag, xa, skipv, wl_hdr, wl_ids, defer,
-                                     (cudaStream_t)stream);
+    DAGR_CHECK_ARG(g && p_host && xyb && feat_s, "null argument");
+    if (N <= 0) return DAGR_OK;
+    DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
+    return cb2_launch<dagr_l1img_params_t, 2, true>(g, N, start, xyb, nullptr, feat_s, x0, nbr, off, p_host, (const float4 *)wfrag, nullptr,
+                                                    0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr,
+                                                    wl_ids, defer, (cudaStream_t)stream);
 }
 
 // incremental stream step of the same instances: only nodes with arrival index ti[p].y >= min_idx are convolved, their xa rows
@@ -1116,10 +751,9 @@ extern "C" int dagr_l1_conv_a_image_inc(const dagr_geom_t *g, int64_t N, const i
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
     if (N == 0) return DAGR_OK;
     DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
-    return cb2_launch<dagr_l1img_params_t, 2, true, CB2_TC != 0>(g, N, start, xyb, (const int2 *)ti, feat_s, x0, nbr, off, p_host,
-                                                                  (const float4 *)wfrag, nullptr, min_idx, nullptr, nullptr, nullptr,
-                                                                  nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr, wl_ids, defer,
-                                                                  (cudaStream_t)stream);
+    return cb2_launch<dagr_l1img_params_t, 2, true>(g, N, start, xyb, (const int2 *)ti, feat_s, x0, nbr, off, p_host, (const float4 *)wfrag,
+                                                    nullptr, min_idx, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, xa,
+                                                    skipv, wl_hdr, wl_ids, defer, (cudaStream_t)stream);
 }
 
 // host-side packing of the weight fragments the tensor-core instances read (layout: see cb2_tc_kstep)
@@ -1128,14 +762,14 @@ extern "C" int dagr_l1_tc_weights(const float *w_host, const float *root_host, i
     DAGR_CHECK_ARG(w_host && root_host && wfrag_host, "null argument");
     DAGR_CHECK_ARG(cin >= 16, "the tensor-core instances take input channels 0..15");
     for (int half = 0; half < 2; half++)
-        for (int s = 0; s < CB2_TC_KSTEPS; s++)
+        for (int s = 0; s < CB2_KSTEPS; s++)
             for (int lane = 0; lane < 32; lane++)
                 for (int nt = 0; nt < 2; nt++) {
                     const int g = lane >> 2, t = lane & 3, n = 8 * nt + g;
                     const float *W = s < DAGR_KU ? w_host + (size_t)s * cin * 16 : root_host;
                     const float x0 = W[(8 * half + t) * 16 + n], x1 = W[(8 * half + t + 4) * 16 + n];
                     const float h0 = tf32_rna_host(x0), h1 = tf32_rna_host(x1);
-                    float *o = wfrag_host + ((((size_t)half * CB2_TC_KSTEPS + s) * 32 + lane) * 2 + nt) * 4;
+                    float *o = wfrag_host + ((((size_t)half * CB2_KSTEPS + s) * 32 + lane) * 2 + nt) * 4;
                     o[0] = h0; o[1] = h1; o[2] = x0 - h0; o[3] = x1 - h1;
                 }
     return DAGR_OK;

@@ -6,9 +6,9 @@
 //      voxel, then arrival order).  A pixel's FIFO column == the tail of its bin read backwards;
 //      a pool1 voxel's members == one contiguous range, which is what lets the event-level convs
 //      and pool1 run as streaming, coalesced passes with warp-segmented reductions.
-//   2. a probe kernel that walks the same spiral over bins (hashed grid = key tables in shared
-//      memory, bins in L1/L2) and writes a column-major ELL adjacency (slot q of node p at
-//      [q*N + p]) in probe order, so that every later pass reads it fully coalesced.
+//   2. a probe that walks the same spiral over bins and writes a column-major ELL adjacency (slot q
+//      of node p at [q*N + p]) in probe order, so that every later pass reads it fully coalesced.
+//      It runs per pool1 voxel on staged records, fused with conv_a (build_l1.cu).
 #include "common.cuh"
 
 #define SCAN_THREADS 256
@@ -379,87 +379,6 @@ extern "C" int dagr_stream_push_multi(int32_t *ctl, const int32_t *stage, int32_
     if (rc != DAGR_OK) return rc;
     stream_push_launch(ctl, stage, batch, pos, feat, capacity, streams, max_chunk, 0, ctl + DAGR_RING_CTL * streams,
                        (cudaStream_t)stream);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// probe: one thread per destination event (sorted position p)
-// ------------------------------------------------------------------------------------------------
-#define SEARCH_THREADS 256
-
-__global__ void __launch_bounds__(SEARCH_THREADS) k_search(dagr_geom_t g, int64_t N, const int32_t *__restrict__ start,
-                                                           const int2 *__restrict__ ti, const uint32_t *__restrict__ xyb,
-                                                           int32_t *__restrict__ nbr, uint16_t *__restrict__ off,
-                                                           uint32_t *__restrict__ cellmask)
-{
-    extern __shared__ int smem_i[];
-    int *s_xkey = smem_i;                 // [W]
-    int *s_ykey = smem_i + g.W;           // [H]
-    short *s_sp = (short *)(s_ykey + g.H);// [ncell] packed (dx & 0xff) | dy << 8
-    for (int i = threadIdx.x; i < g.W; i += blockDim.x) s_xkey[i] = g.xkey[i];
-    for (int i = threadIdx.x; i < g.H; i += blockDim.x) s_ykey[i] = g.ykey[i];
-    for (int i = threadIdx.x; i < g.ncell; i += blockDim.x)
-        s_sp[i] = (short)(((int)g.spiral[2 * i] & 0xff) | ((int)g.spiral[2 * i + 1] << 8));
-    __syncthreads();
-
-    int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool active = p < N;
-    int n = 0;
-    uint32_t m = 0;
-    int cell = -1;
-    if (active) {
-        const uint32_t w = xyb[p];
-        const int x = w & 0xfff, y = (w >> 12) & 0xfff, b = w >> 24;
-        const int2 me = ti[p];
-        const int bbase = b * (g.ny1 * g.nx1 * g.CP);
-        const int kmax = g.K - 1;
-        const int mykey = bbase + s_ykey[y] + s_xkey[x];
-        cell = mykey / g.CP;
-        const int mycx = s_xkey[x] / g.CP, mycy = s_ykey[y] / (g.nx1 * g.CP);
-        for (int c = 0; c < g.ncell && n < kmax; c++) {
-            const int sp = s_sp[c];
-            const int xn = x + (int)(signed char)(sp & 0xff), yn = y + (sp >> 8);
-            if (xn < 0 || yn < 0 || xn >= g.W || yn >= g.H) continue;           // ev_graph.cu:56
-            const int kx = s_xkey[xn], ky = s_ykey[yn];
-            const int k = bbase + ky + kx;
-            const int s = __ldg(start + k), e = __ldg(start + k + 1);
-            if (e == s) continue;                                               // empty FIFO column (:62)
-            const int lo = max(s, e - g.Q);                                     // newest Q entries (:201-211)
-            bool hit = false;
-            for (int j = e - 1; j >= lo; j--) {
-                const int2 o = __ldg(ti + j);
-                if (o.y < me.y) {                                               // strictly earlier arrival (:64)
-                    if (me.x - o.x > g.dt_us) continue;                         // too old (:66-69)
-                    nbr[(int64_t)n * N + p] = j; off[(int64_t)n * N + p] = (uint16_t)c; n++; hit = true;
-                    if (n >= kmax) break;                                       // (:74)
-                }
-            }
-            if (hit) {
-                const int dcx = kx / g.CP - mycx, dcy = ky / (g.nx1 * g.CP) - mycy;
-                if (dcx | dcy) m |= 1u << ((dcy + 1) * 3 + (dcx + 1));
-            }
-        }
-        nbr[(int64_t)(DAGR_ELL - 1) * N + p] = n;
-    }
-    // one atomicOr per distinct voxel per warp
-    const unsigned act = __ballot_sync(0xffffffffu, active && m != 0);
-    if (active && m != 0) {
-        const unsigned peers = __match_any_sync(act, cell);
-        uint32_t mm = __reduce_or_sync(peers, m);
-        if ((threadIdx.x & 31) == __ffs(peers) - 1) atomicOr(cellmask + cell, mm);
-    }
-}
-
-extern "C" int dagr_graph_search(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
-                                 const uint32_t *xyb, int32_t *nbr, uint16_t *off, uint32_t *cellmask, void *stream)
-{
-    DAGR_CHECK_ARG(g && g->K >= 1 && g->K <= DAGR_ELL, "max_neighbors must be in [1,16]");
-    DAGR_CHECK_ARG(g->r >= 0 && g->r <= 15, "radius must be <= 15 px");
-    if (N <= 0) return DAGR_OK;
-    size_t smem = (size_t)(g->W + g->H) * sizeof(int) + (size_t)g->ncell * sizeof(short);
-    k_search<<<dagr_div_up(N, SEARCH_THREADS), SEARCH_THREADS, smem, (cudaStream_t)stream>>>(
-        *g, N, start, (const int2 *)ti, xyb, nbr, off, cellmask);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }

@@ -141,9 +141,7 @@ class Engine:
         self._sentinels = None
         self._ws: Dict[tuple, dict] = {}
         self.keep_node_features = False      # debug / parity: materialise per-event activations
-        self.voxel_conv_b = True             # conv_b + pool1 as one CTA per voxel with TMA-staged rows (False: v1)
         self.use_graphs = True               # replay the fixed-shape coarse stack as a CUDA graph
-        self.fused_build = True              # probe + conv_a in one shared-memory-tiled kernel (False: v1 split kernels)
         # voxels beyond the per-voxel kernels' staging capacity (moving edges): "auto" = the kernels always COUNT them; once a
         # forward has seen some, the following forwards queue them for the persistent dense kernels (two more launches,
         # even when empty, which is why uniform streams do not pay for them); True / False force the behaviour (tests, A/B)
@@ -164,11 +162,11 @@ class Engine:
         self._out_slot = {}
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
-    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_stream_ingest=1, dagr_graph_search=1, dagr_l1_build=2, dagr_l1_build_tc=2, dagr_graph_export=5, dagr_l1_conv_a=1, dagr_l1_conv_b_pool=1, dagr_l1_conv_b_pool_voxel=2, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image=2, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
+    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_stream_ingest=1, dagr_l1_build=2, dagr_l1_build_tc=2, dagr_graph_export=5, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_l1_conv_a_image_inc=2, dagr_voxel_sample_max_inc=1,
                      dagr_l1_x0_image_planes=1, dagr_voxel_sample_max_planes=1, dagr_sample_features_planes=1, dagr_head_finish_planes=1,
-                     dagr_pool1_finalize=1, dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
-                     dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_decode=1, dagr_head_finish=1,
+                     dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
+                     dagr_grid_pool_finalize=1, dagr_grid_temporal_filter=1, dagr_grid_to_dense=1, dagr_head_finish=1,
                      dagr_postprocess_nms=1, dagr_sample_features=1, dagr_denormalize_pos=1,
                      dagr_l1_x0_image_bf16=1, dagr_l1_x0_image_live_bf16=1, dagr_l1_x0_image_planes_bf16=1, dagr_voxel_sample_max_bf16=1,
                      dagr_voxel_sample_max_inc_bf16=1, dagr_voxel_sample_max_planes_bf16=1, dagr_sample_features_bf16=1,
@@ -343,7 +341,6 @@ class Engine:
                 off += nbytes
 
             take("cellmask", int(sz.cellmask))
-            take("poolmax", geom.cells1 * 16 * 4)
             bb = self.model.backbone
             fc = list(getattr(getattr(bb, "net", None), "feature_channels", [])) if bb.use_image else []
             for lv in (1, 2, 3):
@@ -598,7 +595,6 @@ class Engine:
             # the frame is the same for every step between two re-seeds (dagr_b200.asynchronous)
             stream_state.ensure(geom, N, dev, img_channels=int(image_feats[1].shape[1]) if image_feats is not None else 0)
             cellmask, persist, min_idx = stream_state.cellmask, stream_state.voxmax, int(n_old)
-        poolmax = self._zs(ws, "poolmax", torch.int32)
         flags = self._zs(ws, "flags", torch.int32)
         wl_hdr = self._zs(ws, "wl_hdr", torch.int32)
         defer = self._dense_policy(ws, wl_hdr, ring is not None or stream_state is not None)
@@ -623,7 +619,7 @@ class Engine:
                 self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
                           _lib.ptr(stream_state.xa_arr), 0, st)
             # adjacency + the (polarity, x, y) part of conv_block1.conv_block1, which runs on [polarity, 16 image samples, x, y]
-            # (net.py:117-126); the image channels follow in dagr_l1_conv_a_image
+            # (net.py:117-126); the image channels follow in dagr_l1_conv_a_image_tc
             self._run("l1_build", lib.dagr_l1_build_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
                       _lib.ptr(ws["feat_s"]), C.byref(pk["l1a_img"]), _lib.ptr(pk["l1a_img_wfrag"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr), _lib.ptr(off),
                       _lib.ptr(cellmask), _lib.ptr(ws["xa"]), _lib.ptr(wl_hdr), _lib.ptr(self._zs(ws, "wl_build", torch.int32)), defer[0], st)
@@ -659,7 +655,7 @@ class Engine:
                           _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off),
                           C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
                           _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
-        elif self.fused_build or stream_state is not None:
+        else:
             if min_idx > 0:
                 self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
                           _lib.ptr(stream_state.xa_arr), 0, st)
@@ -670,11 +666,6 @@ class Engine:
             if stream_state is not None:
                 self._run("xa_scatter", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
                           _lib.ptr(stream_state.xa_arr), 1, st)
-        else:
-            self._run("graph_search", lib.dagr_graph_search, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(nbr), _lib.ptr(off), _lib.ptr(cellmask), st)
-            self._run("l1_conv_a", lib.dagr_l1_conv_a, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(nbr), _lib.ptr(off),
-                      _lib.ptr(geom.d_tab1), C.byref(pk["l1a"]), _lib.ptr(ws["xa"]), st)
         x1 = None
         if self.keep_node_features:
             if ws["x1"] is None or ws["x1"].shape[0] < ws["cap"]:
@@ -683,33 +674,26 @@ class Engine:
         g1: GridState = ws["grids"][0]
         c1 = 16 + (int(image_feats[1].shape[1]) if use_image else 0)
         g1.x = self._buf(ws, "gx0", (g1.cells, c1), torch.float32, dev)
-        if self.voxel_conv_b or use_image or stream_state is not None:
-            self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["ti"]), _lib.ptr(ws["feat_s"]), _lib.ptr(ws["xa"]), _lib.ptr(nbr), _lib.ptr(off),
-                      C.byref(pk["l1b"]), _lib.ptr(pk["l1b_wfrag"]), _lib.ptr(skipv) if use_image else None, min_idx, _lib.ptr(persist),
-                      _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy), _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1,
-                      _lib.ptr(wl_hdr[4:]), _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
-            self._dense_report(ws, wl_hdr)
-            if use_image and stream_state is not None:        # running per-voxel max of the samples, new events only
-                f1 = image_feats[1]
-                self._run("voxel_sample_max_inc", getattr(lib, "dagr_voxel_sample_max_inc" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                          _lib.ptr(ws["ti"]), _lib.ptr(f1), int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), min_idx,
-                          _lib.ptr(stream_state.imgmax), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
-            elif image_planes is not None:
-                f1 = image_feats[1]
-                self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max_planes" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
-                          int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), int(f1.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
-                          _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
-            elif use_image:                                   # sampling_skip before pool1 (net.py:128-131)
-                f1 = image_feats[1]
-                self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
-                          int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
-        else:
-            self._run("l1_conv_b_pool", lib.dagr_l1_conv_b_pool, g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(ws["xa"]),
-                      _lib.ptr(nbr), _lib.ptr(off), _lib.ptr(geom.d_tab1), C.byref(pk["l1b"]), _lib.ptr(x1), _lib.ptr(poolmax), st)
-            self._run("pool1_finalize", lib.dagr_pool1_finalize, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["ti"]),
-                      _lib.ptr(poolmax), 16, _lib.ptr(g1.cnt), _lib.ptr(g1.pxy), _lib.ptr(g1.tmean), _lib.ptr(g1.tmax),
-                      _lib.ptr(g1.x), st)
+        self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                  _lib.ptr(ws["ti"]), _lib.ptr(ws["feat_s"]), _lib.ptr(ws["xa"]), _lib.ptr(nbr), _lib.ptr(off),
+                  C.byref(pk["l1b"]), _lib.ptr(pk["l1b_wfrag"]), _lib.ptr(skipv) if use_image else None, min_idx, _lib.ptr(persist),
+                  _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy), _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1,
+                  _lib.ptr(wl_hdr[4:]), _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
+        self._dense_report(ws, wl_hdr)
+        if use_image and stream_state is not None:        # running per-voxel max of the samples, new events only
+            f1 = image_feats[1]
+            self._run("voxel_sample_max_inc", getattr(lib, "dagr_voxel_sample_max_inc" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
+                      _lib.ptr(ws["ti"]), _lib.ptr(f1), int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), min_idx,
+                      _lib.ptr(stream_state.imgmax), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
+        elif image_planes is not None:
+            f1 = image_feats[1]
+            self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max_planes" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
+                      int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), int(f1.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
+                      _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
+        elif use_image:                                   # sampling_skip before pool1 (net.py:128-131)
+            f1 = image_feats[1]
+            self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
+                      int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
         g1.mask = cellmask[:g1.cells]
         if kto and stream_state is not None:
             # the persistent stream mask only ever gains edges; the temporal filter (pooling.py:69-72) depends on the CURRENT

@@ -228,7 +228,6 @@ class Geometry:
         self.d_posy0 = self.posy0.to(dev)
         self.d_posxr = self.posxr.to(dev)
         self.d_posyr = self.posyr.to(dev)
-        self.d_tab1 = self.tab1.to(dev)
         self.d_tabx = self.tabx.to(dev)
         self.d_taby = self.taby.to(dev)
         self.d_vx0 = self.vx0.to(dev)

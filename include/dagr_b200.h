@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define DAGR_ABI_VERSION 2
+#define DAGR_ABI_VERSION 3
 
 #define DAGR_OK            0
 #define DAGR_E_ARG        -1   /* bad argument / unsupported shape        */
@@ -102,10 +102,10 @@ int dagr_prepare_events(const float *pos /*[N,3]*/, const int64_t *batch /*[N]*/
  *                       xyb u32[N] = x | y<<12 | b<<24, feat_s f32[N]
  *                       work: key i32[N], tmp i32[N], count i32[NK+1] (MUST be zero on entry; is
  *                       zero again on exit), blocksums i32[dagr_scan_blocks(NK+1)+1]
- *   dagr_graph_search : -> nbr i32[16,N] COLUMN-MAJOR ELL: slot q of node p at [q*N+p]; slots 0..14 =
+ *   dagr_l1_build     : (below) -> nbr i32[16,N] COLUMN-MAJOR ELL: slot q of node p at [q*N+p]; slots 0..14 =
  *                       src positions in probe order, slot 15 = degree without the self loop;
  *                       off u16[16,N] (spiral cell index of each neighbour, same layout), cellmask u32[B*ny1*nx1] (bit (dcy+1)*3+(dcx+1) set when some
- *                       fine edge enters the cell from that neighbouring cell; MUST be zero on entry)
+ *                       fine edge enters the cell from that neighbouring cell)
  *   dagr_graph_export : -> edge_index i64[2,E] exactly as the reference returns it
  *                       (dst ascending in arrival order, self loop first, then probe order);
  *                       rowptr i32[N+1] is written too; E is left in rowptr[N].
@@ -158,21 +158,16 @@ int dagr_graph_sort_rings(const dagr_geom_t *g, const int32_t *batch, const int3
                           int32_t *blocksums, int32_t *start, int32_t *perm, int32_t *ti, uint32_t *xyb, float *feat_s,
                           int32_t *flags, void *stream);
 
-int dagr_graph_search(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
-                      const uint32_t *xyb, int32_t *nbr, uint16_t *off, uint32_t *cellmask,
-                      void *stream);
-
-/* Fused event-level build (the production path): one CTA per pool1 voxel stages the (t, arrival idx,
- * polarity) records of the voxel's 3x3 neighbourhood in shared memory (three coalesced runs, thanks to the
- * cell-major order), probes the spiral entirely on chip, writes the ELL adjacency + cellmask exactly like
- * dagr_graph_search and applies conv_block1.conv_block1 (SplineConv 3->16 + BN + act, see dagr_l1_conv_a)
- * to the neighbours as they are found -> xa (half-major [2][N][8]).  cellmask needs no zeroing for this
- * entry point.  With p_host == NULL only the adjacency / cellmask are produced (image path).  The per-edge slot
- * weights come from the per-axis factor tables g->tabx / g->taby; `tab` is not read by this kernel any more (kept in
- * the signature for ABI stability, may be NULL). */
+/* Fused event-level build: one CTA per pool1 voxel stages the (t, arrival idx, polarity) records of the voxel's 3x3
+ * neighbourhood in shared memory (three coalesced runs, thanks to the cell-major order), probes the spiral entirely on chip,
+ * writes the ELL adjacency + cellmask described above and applies conv_block1.conv_block1 (SplineConv 3->16 + BN + act) to
+ * the neighbours as they are found -> xa (half-major [2][N][8]), in fp32 FMA.  cellmask needs no zeroing.  With
+ * p_host == NULL only the adjacency / cellmask are produced: the graph builder for callers that bring their own convs.  The
+ * per-edge slot weights come from the per-axis factor tables g->tabx / g->taby.  The engine runs the tensor-core form,
+ * dagr_l1_build_tc (below). */
 struct dagr_l1a_params_s;
 int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
-                  const uint32_t *xyb, const float *feat_s, const float *tab,
+                  const uint32_t *xyb, const float *feat_s,
                   const struct dagr_l1a_params_s *p_host, const int32_t *flags /* from dagr_graph_sort, or NULL */,
                   int min_idx /* incremental mode: only events with arrival idx >= min_idx are processed and cellmask is
                                  OR-ed into its previous content; 0 = everything */,
@@ -211,19 +206,6 @@ typedef struct {
     int32_t relu;
 } dagr_l1img_params_t;
 
-/* conv_block1.conv_block1 on 19 input channels, image fusion.  The (polarity, x, y) channels need no gather: dagr_l1_build runs
- * first with their weights (rows 0, 17, 18 of the conv, scale 1 / shift 0 / relu 0) and leaves their sums in xa; this call adds
- * the 16 sampled image channels (x0 chunk-major [2][N][8] from dagr_l1_x0_image; rows 0..15 of p_host->w / root / skip), applies
- * BN + act -> xa (half-major [2][N][8]) and writes the layer's skip branch skipv f32[N,16] = BN(Linear(x0)) (rows 16..18 of
- * p_host->skip = polarity, x, y) consumed by dagr_l1_conv_b_pool_voxel(skip_pre).  Same one-CTA-per-voxel, TMA-staged kernel as
- * conv_block2. */
-int dagr_l1_conv_a_image(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
-                         const float *x0, const int32_t *nbr,
-                         const uint16_t *off, const dagr_l1img_params_t *p_host /* passed by value to the kernel (26 KB) */,
-                         float *xa, float *skipv,
-                         int32_t *wl_hdr, int32_t *wl_ids, int defer /* dense-voxel work list, see dagr_l1_conv_b_pool_voxel */,
-                         void *stream);
-
 /* per-voxel channel max (pool_mean = 0, every shipped config) or mean (pool_mean = 1, args.pooling_aggr) of image features
  * sampled at the voxel's events (sampling_skip before pool1, net.py:128-131): xg[cell*ldx + c0 + c], c < C, empty voxels -> 0 */
 int dagr_voxel_sample_max(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
@@ -238,8 +220,8 @@ int dagr_graph_export(const dagr_geom_t *g, int64_t N, const int32_t *perm, cons
 /* ---------------------------------------------------------------------------------------------
  * a5-a7  event-level Layer (conv_block1): Cartesian attrs + MySplineConv (LUT form) + BN + act
  * (src/dagr/model/layers/spline_conv.py:39-78, conv.py:10-72, components.py:9-35, net.py:122-126).
- * `tab` f32[ncell][DAGR_TABW]: for spiral cell c the weights of the DAGR_KU reachable spline
- * kernel slots (built from MySplineConv.init_lut's basis, spline_conv.py:27-35).
+ * For spiral cell c, slot u of the DAGR_KU reachable spline kernel slots has the weight
+ * tab[c][u] = tabx[dx+r][u%3] * taby[dy+r][u/3] (MySplineConv.init_lut's basis, spline_conv.py:27-35; geometry.py).
  * Weights are passed by value (constant bank): slot-major  w[u][cin][cout].
  * ------------------------------------------------------------------------------------------- */
 typedef struct dagr_l1a_params_s {
@@ -263,11 +245,7 @@ typedef struct {
     float den_x, den_y;           /* fl32(2*M*W), fl32(2*M*H)  (spline_conv.py:28-29) */
 } dagr_l1b_params_t;
 
-int dagr_l1_conv_a(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
-                   const int32_t *nbr, const uint16_t *off, const float *tab,
-                   const dagr_l1a_params_t *p_host, float *xa /*[N,16]*/, void *stream);
-
-/* Tensor-core form of dagr_l1_build (the engine's path).  Same arguments without the unused `tab`, plus `wfrag`
+/* Tensor-core form of dagr_l1_build (the engine's path).  Same arguments plus `wfrag`
  * f32[DAGR_L1A_TC_WFRAG_FLOATS] on the DEVICE: p_host->w and p_host->root as one [48][16] matrix (k = 3 u + cin for the slot
  * weights, 45 + cin for the root) in mma fragment order, split for 3xTF32, as written by dagr_l1a_tc_weights.  conv_a's
  * per-node product (45 slot inputs + 3 root inputs -> 16 channels) then runs as mma.sync TF32 (hi*hi + hi*lo + lo*hi, ~1e-6
@@ -282,43 +260,18 @@ int dagr_l1_build_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, cons
                      const int32_t *flags, int min_idx, int32_t *nbr, uint16_t *off, uint32_t *cellmask, float *xa,
                      int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
 
-/* conv_b + skip + activation, fused with pool1's per-voxel max (a9, pooling.py:74-75):
- * poolmax u32[B*ny1*nx1][16] holds order-preserving encodings (0 = empty; MUST be zero on entry).
- * x1 (optional, may be NULL) receives the per-node activations [N,16] in sorted order. */
-int dagr_l1_conv_b_pool(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
-                        const float *xa, const int32_t *nbr, const uint16_t *off, const float *tab,
-                        const dagr_l1b_params_t *p_host, float *x1, uint32_t *poolmax, void *stream);
-
-/* Production form of conv_b: one CTA per pool1 voxel; the xa rows of the voxel's 3x3 neighbourhood (three
- * contiguous runs in cell-major order) are staged in shared memory with TMA bulk copies (cp.async.bulk
- * + mbarrier) and pool1 is finished in the same CTA (replaces dagr_l1_conv_b_pool + dagr_pool1_finalize):
- * -> cnt i32[cells], pxy i32[cells,2], tmean/tmax f32[cells], xg f32[cells*ldx] (16 channels at column 0); x1 optional
- * as above.  The per-edge slot weights come from the per-axis factor tables g->tabx / g->taby; `tab` is not read by this
- * kernel any more (kept in the signature for ABI stability, may be NULL).  skip_pre f32[N,16] (optional): the layer's skip
- * branch if it was produced elsewhere (image fusion), else it is computed from (polarity, x/W, y/H).  min_idx > 0:
- * incremental step, only nodes with arrival index >= min_idx are convolved and `persist` f32[cells,16] carries the
- * running per-voxel max between steps. */
-int dagr_l1_conv_b_pool_voxel(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
-                              const int32_t *ti, const float *feat_s, const float *xa, const int32_t *nbr,
-                              const uint16_t *off, const float *tab, const dagr_l1b_params_t *p_host,
-                              const float *skip_pre /* f32[N,16] or NULL: precomputed skip branch (image path) */,
-                              int min_idx /* incremental mode: only nodes with arrival idx >= min_idx are convolved */,
-                              float *persist /* f32[cells,16] or NULL: running per-voxel max across streaming steps */,
-                              float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg,
-                              int ldx /* row stride of xg (>= 16) */,
-                              int32_t *wl_hdr /* i32[2] ZERO on entry, or NULL: [0] counts the voxels whose 3x3 neighbourhood holds more
-                                                 than 1344 rows, [1] is the dense kernel's cursor */,
-                              int32_t *wl_ids /* i32[cells] or NULL */,
-                              int defer /* 1: those voxels are queued and processed by a second, persistent launch that stages up to
-                                           6144 rows (196 KB of shared memory per SM); 0: counted only, rows gathered from L2 */,
-                              void *stream);
-
-/* Tensor-core forms of the two per-voxel conv calls above (the engine's path).  Same arguments (conv_b drops the unused `tab`)
- * plus `wfrag` f32[DAGR_L1_TC_WFRAG_FLOATS] on the DEVICE: the weights of input channels 0..15 (w and root) in mma fragment order,
- * split for 3xTF32, as written by dagr_l1_tc_weights.  The slot-weight products of phase 2 and the root term then run as
- * mma.sync TF32 (hi*hi + hi*lo + lo*hi, ~1e-6 relative to the fp32 sums) instead of fp32 FMA; every node gets the same bits in
- * every instance (regular / dense, staged / gathered), as with the plain calls.  Re-run dagr_l1_tc_weights whenever the weights
- * change. */
+/* conv_b (conv_block2: SplineConv 16->16 + BN, skip branch, act) fused with pool1 (a9, pooling.py:66-86): one CTA per pool1
+ * voxel; the xa rows of the voxel's 3x3 neighbourhood (three contiguous runs in cell-major order) are staged in shared memory
+ * with TMA bulk copies (cp.async.bulk + mbarrier) and pool1 is finished in the same CTA:
+ * -> cnt i32[cells], pxy i32[cells,2], tmean/tmax f32[cells], xg f32[cells*ldx] (16 channels at column 0); x1 (optional, may
+ * be NULL) receives the per-node activations [N,16] in sorted order.  The per-edge slot weights come from the per-axis factor
+ * tables g->tabx / g->taby.  skip_pre f32[N,16] (optional): the layer's skip branch if it was produced elsewhere (image
+ * fusion), else it is computed from (polarity, x/W, y/H).  min_idx > 0: incremental step, only nodes with arrival index
+ * >= min_idx are convolved and `persist` f32[cells,16] carries the running per-voxel max between steps.
+ * `wfrag` f32[DAGR_L1_TC_WFRAG_FLOATS] on the DEVICE: the weights of input channels 0..15 (w and root) in mma fragment order,
+ * split for 3xTF32, as written by dagr_l1_tc_weights.  The slot-weight products of phase 2 and the root term run as mma.sync
+ * TF32 (hi*hi + hi*lo + lo*hi, ~1e-6 relative to the fp32 sums); every node gets the same bits in every instance (regular /
+ * dense, staged / gathered).  Re-run dagr_l1_tc_weights whenever the weights change. */
 #define DAGR_L1_TC_WFRAG_FLOATS 8192   /* 2 channel halves x 16 k-steps (15 slots + root) x 32 lanes x 2 n-tiles x 4 */
 int dagr_l1_tc_weights(const float *w_host /* [DAGR_KU][cin][16] slot-major, as in the params structs */,
                        const float *root_host /* [cin][16] */, int cin /* 16 (dagr_l1b_params_t) or 24 (dagr_l1img_params_t) */,
@@ -326,9 +279,25 @@ int dagr_l1_tc_weights(const float *w_host /* [DAGR_KU][cin][16] slot-major, as 
 int dagr_l1_conv_b_pool_voxel_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
                                  const int32_t *ti, const float *feat_s, const float *xa, const int32_t *nbr,
                                  const uint16_t *off, const dagr_l1b_params_t *p_host, const float *wfrag,
-                                 const float *skip_pre, int min_idx, float *persist,
-                                 float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg, int ldx,
-                                 int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
+                                 const float *skip_pre /* f32[N,16] or NULL: precomputed skip branch (image path) */,
+                                 int min_idx /* incremental mode: only nodes with arrival idx >= min_idx are convolved */,
+                                 float *persist /* f32[cells,16] or NULL: running per-voxel max across streaming steps */,
+                                 float *x1, int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *xg,
+                                 int ldx /* row stride of xg (>= 16) */,
+                                 int32_t *wl_hdr /* i32[2] ZERO on entry, or NULL: [0] counts the voxels whose 3x3 neighbourhood holds
+                                                    more than 1344 rows, [1] is the dense kernel's cursor */,
+                                 int32_t *wl_ids /* i32[cells] or NULL */,
+                                 int defer /* 1: those voxels are queued and processed by a second, persistent launch that stages up
+                                              to 6144 rows (196 KB of shared memory per SM); 0: counted only, rows gathered from L2 */,
+                                 void *stream);
+
+/* conv_block1.conv_block1 on 19 input channels, image fusion.  The (polarity, x, y) channels need no gather: dagr_l1_build_tc
+ * runs first with their weights (rows 0, 17, 18 of the conv, scale 1 / shift 0 / relu 0) and leaves their sums in xa; this call
+ * adds the 16 sampled image channels (x0 chunk-major [2][N][8] from dagr_l1_x0_image; rows 0..15 of p_host->w / root / skip),
+ * applies BN + act -> xa (half-major [2][N][8]) and writes the layer's skip branch skipv f32[N,16] = BN(Linear(x0)) (rows 16..18
+ * of p_host->skip = polarity, x, y) consumed by dagr_l1_conv_b_pool_voxel_tc(skip_pre).  Same one-CTA-per-voxel, TMA-staged
+ * kernel and tensor-core phase 2 as conv_b; `wfrag` as written by dagr_l1_tc_weights with cin = 24; p_host is passed by value
+ * to the kernel (26 KB); wl_hdr / wl_ids / defer: the dense-voxel work list, see dagr_l1_conv_b_pool_voxel_tc. */
 int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
                             const float *x0, const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host,
                             const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
@@ -364,13 +333,6 @@ typedef struct {
     const float *posxr;            /* [W] fl(k * fl(1/W))  (pooling.py:47-49)         */
     const float *posyr;            /* [H]                                             */
 } dagr_grid_t;
-
-/* a9 finalize of pool1: per voxel count / mean position (pool_pos) / round_to_pixel / decode max.
- * out: cnt i32[cells], pxy i32[cells,2] (pixel coords after rounding), tmean f32[cells],
- *      x f32[cells, C] (C = 16), cells = B*ny1*nx1.  One warp per voxel. */
-int dagr_pool1_finalize(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
-                        const int32_t *ti, const uint32_t *poolmax, int C,
-                        int32_t *cnt, int32_t *pxy, float *tmean, float *tmax, float *x, void *stream);
 
 /* cat(x, pos[:, :2]) (net.py:135-136 etc.): xin[cells, Cx+2] */
 int dagr_grid_cat_pos(const dagr_grid_t *gr, const int32_t *cnt, const int32_t *pxy, const float *x,
@@ -423,11 +385,6 @@ int dagr_grid_temporal_filter(const dagr_grid_t *gr, const int32_t *cnt, const f
 /* a10 to_dense (spline_conv.py:80-107): grid-major [cells, C] -> dense [B, C, ny, nx] (+= add, optional) */
 int dagr_grid_to_dense(const dagr_grid_t *gr, const int32_t *cnt, const float *x, int C, int ldx /* row stride of x, 0 = C */,
                        const float *add /*[B,C,ny,nx] or NULL*/, float *dense, void *stream);
-
-/* a11 collect_outputs + decode_outputs (dagr.py:292-312): per scale reg[B,4,h,w], obj[B,1,h,w],
- * cls[B,nc,h,w] -> out[B, A, 5+nc] rows [a0, a0+h*w)  */
-int dagr_head_decode(const float *reg, const float *obj, const float *cls, int B, int nc, int h, int w,
-                     int stride, int a0, int A, float *out, void *stream);
 
 /* to_dense of the three prediction convs + the CNN head maps (dagr.py:219-222) + collect_outputs + decode_outputs of one
  * scale in one launch: cls f32[cells, ldc] (nc used), regobj f32[cells, ldr] = (reg[4], obj[1]) as written by ONE conv over the

@@ -185,7 +185,7 @@ def test_forward_with_another_image_between_steps_does_not_disturb_the_stream():
     assert a.frames == 1
 
 
-def test_incremental_entry_points_at_min_idx_zero_equal_the_synchronous_kernels():
+def test_incremental_entry_points_at_min_idx_zero_equal_the_synchronous_tc_kernels():
     """both C entry points on the inputs of a synchronous forward: conv_a_image_inc(min_idx=0) == conv_a_image_tc and
     voxel_sample_max_inc(min_idx=0) == voxel_sample_max, bit for bit; persist is seeded with the result (-inf when empty)."""
     from dagr_b200 import _lib
@@ -208,7 +208,7 @@ def test_incremental_entry_points_at_min_idx_zero_equal_the_synchronous_kernels(
     for inc in (False, True):
         xa = torch.zeros_like(ws["xa"])
         cellmask = torch.zeros(geom.cells1, dtype=torch.int32, device="cuda")
-        _lib.check(lib.dagr_l1_build(g, N, P(ws["start"]), P(ws["ti"]), P(ws["xyb"]), P(ws["feat_s"]), P(geom.d_tab1), C.byref(pk["l1a_img"]),
+        _lib.check(lib.dagr_l1_build(g, N, P(ws["start"]), P(ws["ti"]), P(ws["xyb"]), P(ws["feat_s"]), C.byref(pk["l1a_img"]),
                                      P(flags), 0, P(ws["nbr"]), P(ws["off"]), P(cellmask), P(xa), None, None, 0, st), "l1_build")
         skipv = torch.full((N, 16), float("nan"), device="cuda")
         if inc:

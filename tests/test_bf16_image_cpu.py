@@ -18,7 +18,7 @@ NAMES = ["dagr_l1_x0_image_bf16", "dagr_l1_x0_image_live_bf16", "dagr_l1_x0_imag
          "dagr_sample_features_planes_bf16"]
 
 
-def test_bf16_entry_points_are_exported_declared_and_counted():
+def test_bf16_entry_points_are_exported_declared_and_counted_at_abi_3():
     from dagr_b200 import _lib
     from dagr_b200.engine import Engine
     lib = _lib.load()
@@ -32,7 +32,7 @@ def test_bf16_entry_points_are_exported_declared_and_counted():
         fp32 = n[: -len("_bf16")]
         extra = 1 if "x0_image" in n else 0
         assert len(_lib._SIGS[n][1]) == len(_lib._SIGS[fp32][1]) + extra
-    assert lib.dagr_abi_version() == 2
+    assert lib.dagr_abi_version() == 3
 
 
 def _geom(B=2):

@@ -1,7 +1,8 @@
 """dagr_l1_build_tc (conv_block1.conv_block1's per-node product on tensor cores, 3xTF32) against dagr_l1_build on the same
 inputs: the adjacency (nbr, off, the degree slot) and cellmask are the same bits, xa agrees within 1e-5, and every node's xa
 row has the same bits in every instance -- the lean launch with its global-memory fallback (defer = 0) and the regular launch
-with the dense kernel behind it (defer = 1).  The stream has a dense cluster so that both fallbacks run."""
+with the dense kernel behind it (defer = 1).  The adjacency-only form of dagr_l1_build (p_host = NULL) gives the same adjacency
+bits.  The stream has a dense cluster so that both fallbacks run."""
 import ctypes as C
 
 import pytest
@@ -27,13 +28,12 @@ def _dense_stream(W, H):
                       height=torch.tensor([H]), time_window=torch.tensor([1000000]), pos_denorm=pos_denorm, num_graphs=1)
 
 
-def test_tc_build_keeps_the_adjacency_and_gives_each_node_the_same_bits_in_every_instance():
+def test_tc_build_keeps_the_adjacency_of_both_fp32_forms_and_gives_each_node_the_same_bits_in_every_instance():
     from dagr_b200 import _lib
     W, H = 640, 480
     model, _ = make_model("n", H, W)
     model.cuda()
     eng = model.engine
-    eng.fused_build = True
     batch_i, pos_i, feat, W_, H_ = model._prepare_events(_dense_stream(W, H).cuda())
     eng.forward_events(batch_i, pos_i, feat, 1, W_, H_)
     torch.cuda.synchronize()
@@ -42,7 +42,7 @@ def test_tc_build_keeps_the_adjacency_and_gives_each_node_the_same_bits_in_every
     lib, pk, g, st, P = eng.lib, eng._pack, C.byref(geom.c_geom), _lib.stream_ptr(), _lib.ptr
     flags = eng._zs(ws, "flags", torch.int32)
 
-    def run(tc, defer):
+    def run(tc, defer, adjacency_only=False):
         nbr, off = torch.zeros_like(ws["nbr"]), torch.zeros_like(ws["off"])
         xa = torch.zeros_like(ws["xa"])
         cellmask = torch.zeros(geom.cells1, dtype=torch.int32, device="cuda")
@@ -53,7 +53,7 @@ def test_tc_build_keeps_the_adjacency_and_gives_each_node_the_same_bits_in_every
         if tc:
             _lib.check(lib.dagr_l1_build_tc(*head, C.byref(pk["l1a"]), P(pk["l1a_wfrag"]), *tail), "l1_build_tc")
         else:
-            _lib.check(lib.dagr_l1_build(*head, P(geom.d_tab1), C.byref(pk["l1a"]), *tail), "l1_build")
+            _lib.check(lib.dagr_l1_build(*head, None if adjacency_only else C.byref(pk["l1a"]), *tail), "l1_build")
         torch.cuda.synchronize()
         return dict(nbr=nbr[:16 * N], off=off[:16 * N], cellmask=cellmask, xa=xa[:2 * N * 8], beyond=int(wl_hdr[0]))
 
@@ -66,5 +66,9 @@ def test_tc_build_keeps_the_adjacency_and_gives_each_node_the_same_bits_in_every
         rows = lambda xa: torch.cat([xa[:N * 8].view(N, 8), xa[N * 8:].view(N, 8)], 1).cpu()
         assert_close(rows(tc["xa"]), rows(plain["xa"]), tol=1e-5, what=f"l1_build_tc vs l1_build xa (defer={defer})")
     assert torch.equal(out[(True, 0)]["xa"], out[(True, 1)]["xa"])
+    for defer in (0, 1):
+        adj = run(False, defer, adjacency_only=True)
+        for k in ("nbr", "off", "cellmask"):
+            assert torch.equal(adj[k], out[(False, defer)][k]), ("adjacency only", k, defer)
     # the engine's own forward ran the tensor-core kernel as well
     assert torch.equal(ws["xa"][:2 * N * 8], out[(True, 0)]["xa"]) or torch.equal(ws["xa"][:2 * N * 8], out[(True, 1)]["xa"])

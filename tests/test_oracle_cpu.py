@@ -205,7 +205,7 @@ def test_oracle_masked_ops():
 # ---------------------------------------------------------------------------------------------
 # host logic + C-ABI surface
 # ---------------------------------------------------------------------------------------------
-def test_capi_exports_every_declared_symbol():
+def test_capi_exports_every_declared_symbol_of_abi_3():
     from dagr_b200 import _lib, build
     so = build.build()
     lib = ctypes.CDLL(str(so))
@@ -215,7 +215,7 @@ def test_capi_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/dagr_b200.h but not exported"
     assert set(_lib.EXPORTS) == declared
-    assert lib.dagr_abi_version() == 2
+    assert lib.dagr_abi_version() == 3
 
 
 def test_product_has_no_cpu_fallback_and_never_imports_oracle():

@@ -12,7 +12,7 @@ ROOT = Path(__file__).resolve().parents[1]
 so = ROOT / "dagr_b200" / "libdagr_b200.so"
 txt = subprocess.run(["cuobjdump", "-sass", str(so)], capture_output=True, text=True).stdout
 funcs = re.split(r"(?=\t\tFunction : )", txt)
-want = {"l1_build": "_Z10k_l1_buildILi1536ELi5E", "conv_b2": "_Z12k_l1_conv_b2I17dagr_l1b_params_tLi2ELb0ELb0ELb1ELb1E"}
+want = {"l1_build": "_Z10k_l1_buildILi1536ELi5E", "conv_b2": "_Z12k_l1_conv_b2I17dagr_l1b_params_tLi2ELb0ELb0ELb1EEv"}
 for tag, prefix in want.items():
     body = next(f for f in funcs if f.lstrip().startswith("Function : " + prefix))
     hist = collections.Counter()
