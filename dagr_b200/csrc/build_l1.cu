@@ -21,11 +21,15 @@
 //             of the events of the clustered benchmark stream) are pushed on a device work list by the regular kernel and
 //             processed by a persistent second kernel (one 512-thread CTA per SM, 12288 staged records, dynamic pop) --
 //             the global-memory probe remains only as the fallback behind that.
+// The capacities are public (include/dagr_b200.h), so that callers and tests can tell which instance a voxel reaches.
 #define BL_THREADS 160
-#define BL_CAP 2048
-#define BL_CAP_LEAN 1536           // the count-only launch (defer = 0): 44 KB per CTA -> five CTAs per SM instead of four
+#define BL_CAP DAGR_L1_BUILD
+#define BL_CAP_LEAN DAGR_L1_BUILD_LEAN   // the count-only launch (defer = 0): 44 KB per CTA -> five CTAs per SM instead of four
 #define BL_THREADS_BIG 512
-#define BL_CAP_BIG 12288
+#define BL_CAP_BIG DAGR_L1_BUILD_DENSE
+static_assert(BL_CAP_LEAN <= BL_CAP && BL_CAP < BL_CAP_BIG, "lean <= regular < dense staging capacity");
+static_assert(BL_CAP % 4 == 0 && BL_CAP_LEAN % 4 == 0 && BL_CAP_BIG % 4 == 0, "s_rng must stay 16-byte aligned");
+static_assert(BL_CAP_BIG < (1 << 22), "phase B packs the staged record index in 22 bits (record << 10 | cell)");
 #define BL_NB 8                  // time buckets of width delta_t kept per tile pixel
 
 struct BLTile {
@@ -798,7 +802,24 @@ static int l1_build_launch(const dagr_geom_t *g, int64_t N, const int32_t *start
     DAGR_CHECK_ARG(g->r >= 0 && g->r <= 15 && g->Q <= 255, "radius must be <= 15 px and max_queue_size <= 255");
     DAGR_CHECK_ARG(N < (1ll << 24), "the staged probe packs positions in 24 bits (N < 16.7M per call)");
     const int cells = g->B * g->ny1 * g->nx1;
-    const bool deferring = wl_hdr != nullptr && wl_ids != nullptr && defer;
+    bool deferring = wl_hdr != nullptr && wl_ids != nullptr && defer;
+    if (deferring) {
+        // The dense instance stages 12288 records next to the tile tables of the geometry.  Where the two do not fit the
+        // device's shared memory (large pool1 voxels at r >= 13, e.g. 1280 x 960 at radius 0.01), the call takes the
+        // count-only launch instead: every instance gives a node the same bits, and the over-capacity voxels probe global
+        // memory.  Deciding before anything is launched keeps a voxel from being queued for a kernel that cannot run.
+        static int optin = 0;
+        static size_t dense_static = 0;
+        if (optin == 0) {
+            int dev = 0;
+            cudaFuncAttributes fa;
+            DAGR_CUDA(cudaGetDevice(&dev));
+            DAGR_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+            DAGR_CUDA(cudaFuncGetAttributes(&fa, k_l1_build_dense<TC>));
+            dense_static = fa.sharedSizeBytes;
+        }
+        if (bl_smem_bytes(g, BL_CAP_BIG, BL_THREADS_BIG) + dense_static > (size_t)optin) deferring = false;
+    }
     if (deferring) {
         const size_t smem = bl_smem_bytes(g, BL_CAP, BL_THREADS);
         auto kern = k_l1_build<BL_CAP, 4, TC>;

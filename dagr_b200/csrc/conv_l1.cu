@@ -29,11 +29,15 @@
 //   dense   : voxels whose 3x3 neighbourhood holds more rows (75 % of the events of the clustered benchmark stream) are
 //             queued by the regular kernel and processed by persistent 384-thread CTAs (one per SM) that stage up to
 //             6144 rows (196 KB); only beyond that rows are gathered from global memory / L2.
+// (The capacities are public, include/dagr_b200.h.)
 #define CB2_THREADS 160
-#define CB2_CAP 1344
+#define CB2_CAP DAGR_L1_CONV
 #define CB2_THREADS_BIG 384
-#define CB2_CAP_BIG 6144
+#define CB2_CAP_BIG DAGR_L1_CONV_DENSE
+static_assert(CB2_CAP < CB2_CAP_BIG, "regular < dense staging capacity");
 static_assert(2 * CB2_CAP_BIG <= 16384, "the ELL word keeps 2*row+swizzle in 14 bits");
+static_assert(DAGR_L1_SPARSE_NODES == 32 && 2 * 32 * 16 <= CB2_CAP * 8,
+              "the sparse split runs one warp of nodes and parks two warps' partial sums in the staging buffer");
 #define CB2_G 5                  // spline slots per pass: one x-slot k, all five y-slots (u = k + 3 j)
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -353,8 +357,11 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
     // the serial work per thread.  Block-uniform; the dense path below is unchanged.
     // (compiled into the image-fusion instance only: in the 2-chunk conv_block2 instance the extra live state costs the
     // dense path 1.3 % and the sparse gain is small, measured).  Incremental steps take the same path, so that a new node gets
-    // the bits the synchronous forward gives it (the passes skip the nodes that are not active).
-    const bool sparse = MODE_A && staged && nown <= 32;
+    // the bits the synchronous forward gives it (the passes skip the nodes that are not active).  The split does not depend
+    // on `staged`: its partial sums associate differently from the single chain of the dense path, so a voxel must take it in
+    // every instance (a gathered neighbourhood reads its rows from global memory and leaves s_rows free for the partials) --
+    // otherwise its nodes would get other bits with defer = 0 than with defer = 1.
+    const bool sparse = MODE_A && nown <= DAGR_L1_SPARSE_NODES;
     const int lane_ = threadIdx.x & 31, wid_ = threadIdx.x >> 5;
     for (int pb0 = p0; pb0 < p1; pb0 += blockDim.x) {
         const int p = sparse ? p0 + lane_ : pb0 + threadIdx.x;
@@ -704,9 +711,16 @@ extern "C" int dagr_l1_conv_b_pool_voxel_tc(const dagr_geom_t *g, int64_t N, con
                                             int defer, void *stream)
 {
     DAGR_CHECK_ARG(wfrag_f, "null weight fragments (dagr_l1_tc_weights)");
-    DAGR_CHECK_ARG(g && p_host, "null argument");
+    DAGR_CHECK_ARG(g && start && xyb && ti && feat_s && xa && nbr && off && p_host && cnt && pxy && tmean && tmax && xg,
+                   "null argument (only skip_pre / persist / x1 / wl_hdr / wl_ids may be NULL)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
+    DAGR_CHECK_ARG(ldx >= 16, "ldx (row stride of xg) must be >= 16");
     DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
     DAGR_CHECK_ARG(!(p_host->pool_mean && persist), "the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
+    // without the running aggregate an incremental step would pool its new nodes alone (max) or divide their sum by every
+    // node of the voxel (mean)
+    DAGR_CHECK_ARG(min_idx == 0 || persist, "an incremental step (min_idx > 0) needs persist, the running per-voxel max");
     const float4 *wfrag = (const float4 *)wfrag_f;
     const cudaStream_t st = (cudaStream_t)stream;
     if (p_host->pool_mean)
@@ -729,8 +743,10 @@ extern "C" int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const in
                                        const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream)
 {
     DAGR_CHECK_ARG(wfrag, "null weight fragments (dagr_l1_tc_weights)");
-    DAGR_CHECK_ARG(g && p_host && xyb && feat_s, "null argument");
-    if (N <= 0) return DAGR_OK;
+    DAGR_CHECK_ARG(g && start && xyb && feat_s && x0 && nbr && off && p_host && xa && skipv,
+                   "null argument (only wl_hdr / wl_ids may be NULL)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    if (N == 0) return DAGR_OK;
     DAGR_CHECK_ARG(g->r <= 15, "radius must be <= 15 px (offsets are packed in 5 bits)");
     return cb2_launch<dagr_l1img_params_t, 2, true>(g, N, start, xyb, nullptr, feat_s, x0, nbr, off, p_host, (const float4 *)wfrag, nullptr,
                                                     0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, xa, skipv, wl_hdr,

@@ -34,6 +34,25 @@ extern "C" {
 #define DAGR_TABW 16           /* row stride (floats) of the offset->slot-weight table       */
 #define DAGR_RING_CTL 8        /* ints per stream in a streaming control block (ctl)          */
 
+/* Staging capacities of the per-voxel event-level kernels.  Each kernel picks its instance per pool1 voxel, on the device,
+ * from `total` = the number of nodes in the voxel's 3x3 neighbourhood:
+ *   dagr_l1_build[_tc]     defer = 0: staged when total <= BUILD_LEAN, else the global-memory probe;
+ *                          defer = 1: staged when total <= BUILD, else the dense kernel, staged when total <= BUILD_DENSE,
+ *                          else the global-memory probe inside it;
+ *   dagr_l1_conv_b_pool_voxel_tc / dagr_l1_conv_a_image_tc / _inc
+ *                          staged when total <= CONV; above that the dense kernel when defer = 1 (staged when
+ *                          total <= CONV_DENSE, else rows gathered from global memory), rows gathered in the regular kernel
+ *                          when defer = 0.
+ * The image conv splits a voxel with at most SPARSE_NODES own nodes over three warps (one x-slot each), in every instance.
+ * wl_hdr[0] counts the voxels above BUILD_LEAN / BUILD (build, by defer) or above CONV (convs).  The build kernel's defer = 1
+ * falls back to the defer = 0 launch where the dense instance does not fit the device's shared memory (dagr_l1_build). */
+#define DAGR_L1_BUILD_LEAN        1536
+#define DAGR_L1_BUILD             2048
+#define DAGR_L1_BUILD_DENSE      12288
+#define DAGR_L1_CONV              1344
+#define DAGR_L1_CONV_DENSE        6144
+#define DAGR_L1_SPARSE_NODES        32
+
 int         dagr_abi_version(void);
 const char *dagr_last_error(void);
 
@@ -178,7 +197,10 @@ int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const i
                   int32_t *wl_ids /* i32[cells] or NULL: ids of those voxels when `defer` */,
                   int defer /* 1: such voxels are queued and processed by a second, persistent launch with a 12288-record staging
                                buffer; 0: they are only counted and probe global memory (slow, exact) -- a caller can watch
-                               wl_hdr[0] and switch `defer` on for streams that have dense voxels */,
+                               wl_hdr[0] and switch `defer` on for streams that have dense voxels.  Where the dense launch's
+                               shared memory (12288 records plus the geometry's tile tables) exceeds the device's opt-in limit
+                               -- large pool1 voxels at r >= 13, e.g. 1280 x 960 at radius 0.01 on an H100 -- defer = 1 runs
+                               the defer = 0 launch: the same bits, wl_hdr[0] counting the voxels over 1536 records */,
                   void *stream);
 
 /* streaming (a13): node rows live in arrival order between steps; gather (scatter=0: rows of nodes < n_old into the
@@ -271,7 +293,13 @@ int dagr_l1_build_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, cons
  * `wfrag` f32[DAGR_L1_TC_WFRAG_FLOATS] on the DEVICE: the weights of input channels 0..15 (w and root) in mma fragment order,
  * split for 3xTF32, as written by dagr_l1_tc_weights.  The slot-weight products of phase 2 and the root term run as mma.sync
  * TF32 (hi*hi + hi*lo + lo*hi, ~1e-6 relative to the fp32 sums); every node gets the same bits in every instance (regular /
- * dense, staged / gathered).  Re-run dagr_l1_tc_weights whenever the weights change. */
+ * dense, staged / gathered), and so do the per-voxel max (xg, persist), cnt, pxy, tmean and tmax.  The per-voxel MEAN
+ * (pool_mean = 1) is an fp32 sum over the CTA's warps, 5 in the regular and 12 in the dense instance: a voxel over the
+ * regular capacity may get other last bits with defer = 0 than with defer = 1.  Re-run dagr_l1_tc_weights whenever the
+ * weights change.
+ * Returns DAGR_E_ARG with a message before launching anything on a null pointer (skip_pre / persist / x1 / wl_hdr / wl_ids
+ * may be NULL), N outside [0, 2^31), min_idx < 0, ldx < 16, persist with pool_mean, or min_idx > 0 without persist (the new
+ * nodes alone would be pooled). */
 #define DAGR_L1_TC_WFRAG_FLOATS 8192   /* 2 channel halves x 16 k-steps (15 slots + root) x 32 lanes x 2 n-tiles x 4 */
 int dagr_l1_tc_weights(const float *w_host /* [DAGR_KU][cin][16] slot-major, as in the params structs */,
                        const float *root_host /* [cin][16] */, int cin /* 16 (dagr_l1b_params_t) or 24 (dagr_l1img_params_t) */,
@@ -297,7 +325,9 @@ int dagr_l1_conv_b_pool_voxel_tc(const dagr_geom_t *g, int64_t N, const int32_t 
  * applies BN + act -> xa (half-major [2][N][8]) and writes the layer's skip branch skipv f32[N,16] = BN(Linear(x0)) (rows 16..18
  * of p_host->skip = polarity, x, y) consumed by dagr_l1_conv_b_pool_voxel_tc(skip_pre).  Same one-CTA-per-voxel, TMA-staged
  * kernel and tensor-core phase 2 as conv_b; `wfrag` as written by dagr_l1_tc_weights with cin = 24; p_host is passed by value
- * to the kernel (26 KB); wl_hdr / wl_ids / defer: the dense-voxel work list, see dagr_l1_conv_b_pool_voxel_tc. */
+ * to the kernel (26 KB); wl_hdr / wl_ids / defer: the dense-voxel work list, see dagr_l1_conv_b_pool_voxel_tc.  Every node's xa
+ * and skipv rows are the same bits in every instance, sparse voxels (DAGR_L1_SPARSE_NODES) included.  Returns DAGR_E_ARG with a
+ * message before launching anything on a null pointer (wl_hdr / wl_ids may be NULL) or N outside [0, 2^31). */
 int dagr_l1_conv_a_image_tc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
                             const float *x0, const int32_t *nbr, const uint16_t *off, const dagr_l1img_params_t *p_host,
                             const float *wfrag, float *xa, float *skipv, int32_t *wl_hdr, int32_t *wl_ids, int defer, void *stream);
