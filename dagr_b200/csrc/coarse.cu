@@ -810,7 +810,11 @@ extern "C" int dagr_sample_features(const float *img, int Bi, int C, int h, int 
                                     const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
                                     void *stream)
 {
-    if (n <= 0) return DAGR_OK;
+    DAGR_CHECK_ARG(img && posx && posy && bidx && out, "null argument");
+    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(Bi >= 1 && C >= 1 && h >= 1 && w >= 1, "the map must have Bi, C, h, w >= 1");
+    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
+    if (n == 0) return DAGR_OK;
     k_sample_features<false><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, Bi, C, h, w, posx, posy, bidx, n,
                                                                                 (float)width, (float)height, out, ldo, c0, ImgPlanes{});
     DAGR_CHECK_LAUNCH();
@@ -825,6 +829,8 @@ extern "C" int dagr_sample_features_planes(const float *img, int nplanes, const 
     DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
     DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
     DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(C >= 1 && h >= 1 && w >= 1, "the map must have C, h, w >= 1");
+    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
     if (n == 0) return DAGR_OK;
     k_sample_features<true><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, 1, C, h, w, posx, posy, bidx, n, (float)width,
                                                                                (float)height, out, ldo, c0,
@@ -841,6 +847,7 @@ extern "C" int dagr_sample_features_bf16(const void *img, int Bi, int C, int h, 
     DAGR_CHECK_ARG(img && posx && posy && bidx && out, "null argument");
     DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
     DAGR_CHECK_ARG(Bi >= 1 && C >= 1 && h >= 1 && w >= 1, "the map must have Bi, C, h, w >= 1");
+    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
     if (n == 0) return DAGR_OK;
     k_sample_features<false, __nv_bfloat16><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
         static_cast<const __nv_bfloat16 *>(img), Bi, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0, ImgPlanes{});
@@ -857,6 +864,7 @@ extern "C" int dagr_sample_features_planes_bf16(const void *img, int nplanes, co
     DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
     DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
     DAGR_CHECK_ARG(C >= 1 && h >= 1 && w >= 1, "the map must have C, h, w >= 1");
+    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
     if (n == 0) return DAGR_OK;
     k_sample_features<true, __nv_bfloat16><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
         static_cast<const __nv_bfloat16 *>(img), 1, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0,

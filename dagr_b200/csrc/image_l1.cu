@@ -86,7 +86,10 @@ extern "C" int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t 
                                 int h, int w, float *x0, void *stream)
 {
     (void)feat_s;
-    if (N <= 0) return DAGR_OK;
+    DAGR_CHECK_ARG(g && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the conv1 tap is [B, 16, h, w] with h, w >= 1");
+    if (N == 0) return DAGR_OK;
     k_l1_x0_image<false><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, nullptr, xyb, img0, h, w, x0, ImgPlanes{});
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
@@ -98,6 +101,7 @@ extern "C" int dagr_l1_x0_image_live(const dagr_geom_t *g, int64_t N, const int3
     (void)feat_s;
     DAGR_CHECK_ARG(g && start && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the conv1 tap is [B, 16, h, w] with h, w >= 1");
     if (N == 0) return DAGR_OK;
     k_l1_x0_image<false><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0, ImgPlanes{});
     DAGR_CHECK_LAUNCH();
@@ -113,6 +117,7 @@ extern "C" int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const in
     DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
     DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the conv1 tap is [nplanes, 16, h, w] with h, w >= 1");
     if (N == 0) return DAGR_OK;
     k_l1_x0_image<true><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0,
                                                                                  ImgPlanes{plane, plane_stride, nplanes});
@@ -180,7 +185,6 @@ extern "C" int dagr_l1_x0_image_planes_bf16(const dagr_geom_t *g, int64_t N, con
 // fp32 arithmetic are those of bilin_sample, i.e. of the oracle.  Windows that do not fit fall back to global taps.
 // ------------------------------------------------------------------------------------------------
 #define VS_THREADS 128
-#define VS_SMEM_FLOATS 10240                                            // 40 KB: e.g. 2 planes x 6 x 6 x 128 channels
 
 template <bool STAGED, typename MT>
 __device__ __forceinline__ float vs_sample(const MT *__restrict__ img, const float *s_patch, int Bi, int C, int h, int w,
@@ -229,7 +233,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
                    float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0, const ImgPlanes pl = ImgPlanes{})
 {
     __shared__ float s_m[VS_THREADS / 32][128];
-    __shared__ __align__(16) float s_patch[VS_SMEM_FLOATS];
+    __shared__ __align__(16) float s_patch[DAGR_VS_SMEM_FLOATS];
     const int cell = blockIdx.x;
     const int per = g.ny1 * g.nx1;
     const int b = cell / per, rem = cell % per, cy = rem / g.nx1, cx = rem % g.nx1;
@@ -271,7 +275,7 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
     const int xb = max(lo.x0, 0), yb = max(lo.y0, 0), zb = max(lo.z0, 0);
     const int xe = min(hi.x0 + 1, w - 1), ye = min(hi.y0 + 1, h - 1), ze = min(lo.z0 + 1, (PLANES ? 1 : g.B) - 1);
     const int pw = xe - xb + 1, ph = ye - yb + 1, pz = ze - zb + 1;
-    const bool staged = pw > 0 && ph > 0 && pz > 0 && (int64_t)pz * ph * pw * C <= VS_SMEM_FLOATS;   // block-uniform
+    const bool staged = pw > 0 && ph > 0 && pz > 0 && (int64_t)pz * ph * pw * C <= DAGR_VS_SMEM_FLOATS;   // block-uniform
     if (staged) {
         const int tot = pz * ph * pw * C;
         if constexpr (std::is_same<MT, float>::value) {
@@ -382,7 +386,10 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
 extern "C" int dagr_voxel_sample_max(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *img,
                                      int C, int h, int w, float *xg, int ldx, int c0, int pool_mean, void *stream)
 {
-    (void)N;
+    DAGR_CHECK_ARG(g && start && xyb && img && xg, "null argument");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
+    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
     const int cells = g->B * g->ny1 * g->nx1;
     if (pool_mean) k_voxel_sample_max<true, false><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
                                                                                                  nullptr, xg, ldx, c0);
@@ -399,6 +406,7 @@ extern "C" int dagr_voxel_sample_max_inc(const dagr_geom_t *g, int64_t N, const 
     DAGR_CHECK_ARG(g && start && xyb && ti && img && persist && xg, "null argument");
     DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
     DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
     DAGR_CHECK_ARG(!pool_mean, "pool_mean: the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
     const int cells = g->B * g->ny1 * g->nx1;
@@ -416,6 +424,7 @@ extern "C" int dagr_voxel_sample_max_planes(const dagr_geom_t *g, int64_t N, con
     DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
     DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
     DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
     const int cells = g->B * g->ny1 * g->nx1;
     const ImgPlanes pl{plane, plane_stride, nplanes};

@@ -53,6 +53,13 @@ extern "C" {
 #define DAGR_L1_CONV_DENSE        6144
 #define DAGR_L1_SPARSE_NODES        32
 
+/* Staging capacity (floats) of dagr_voxel_sample_max[_inc|_planes][_bf16]: a voxel stages the window of the map its events
+ * can touch -- pz planes x ph rows x pw columns x C channels, derived from the voxel's corner pixels -- in shared memory when
+ * pz * ph * pw * C <= DAGR_VS_SMEM_FLOATS, and reads its taps from global memory otherwise.  Staged voxels take the fast path
+ * (8 channels per lane) for C in {8, 16, 32, 64, 128} and the general path (one channel per lane, 128-channel blocks)
+ * otherwise.  40 KB: e.g. 2 planes x 6 x 6 x 128 channels. */
+#define DAGR_VS_SMEM_FLOATS      10240
+
 int         dagr_abi_version(void);
 const char *dagr_last_error(void);
 
@@ -209,7 +216,9 @@ int dagr_xa_permute(int64_t N, const int32_t *perm, int n_old, float *xa_sorted,
 
 /* ---- image fusion at the event level (use_image, net.py:117-131): conv_block1 = Layer(1+16+2 -> 16) ----
  * x0 f32[3][N][8] chunk-major = [polarity, 16 bilinear samples of image_feat[0] at the event, x/W, y/H, pad];
- * sampling follows net.py:193-221 (grid_sample, align_corners=True, batch as depth). */
+ * sampling follows net.py:193-221 (grid_sample, align_corners=True, batch as depth).  feat_s is not read and may be NULL; any
+ * other null pointer, N outside [0, 2^31) or h, w < 1 returns DAGR_E_ARG with a message before anything is launched (as for
+ * every image-sampling entry point below). */
 int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s,
                      const float *img0 /*[B,16,h,w]*/, int h, int w, float *x0, void *stream);
 /* Same kernel and results, bounded by the live total start[g->NK] that the sort wrote (device data): sorted positions at or
@@ -229,7 +238,9 @@ typedef struct {
 } dagr_l1img_params_t;
 
 /* per-voxel channel max (pool_mean = 0, every shipped config) or mean (pool_mean = 1, args.pooling_aggr) of image features
- * sampled at the voxel's events (sampling_skip before pool1, net.py:128-131): xg[cell*ldx + c0 + c], c < C, empty voxels -> 0 */
+ * sampled at the voxel's events (sampling_skip before pool1, net.py:128-131): xg[cell*ldx + c0 + c], c < C, empty voxels -> 0.
+ * Returns DAGR_E_ARG with a message before launching anything on a null pointer, N outside [0, 2^31), h or w < 1, C < 1,
+ * c0 < 0 or c0 + C > ldx. */
 int dagr_voxel_sample_max(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
                           const float *img /*[B,C,h,w]*/, int C, int h, int w, float *xg, int ldx, int c0, int pool_mean,
                           void *stream);
@@ -437,7 +448,9 @@ int dagr_postprocess_nms(const float *pred, int B, int A, int nc, float conf_thr
                          int width, int height, int filtering, float *det, int32_t *ndet, void *stream);
 
 /* a8 sample_features (net.py:193-221): bilinear, align_corners=True, batch as depth.
- * img f32[Bi,C,h,w]; positions given as normalised floats; out[n, ldo] columns [c0, c0+C) */
+ * img f32[Bi,C,h,w]; positions given as normalised floats; out[n, ldo] columns [c0, c0+C).  Every sample_features form
+ * (plain, _planes, _bf16) returns DAGR_E_ARG with a message before launching anything on a null pointer, n outside [0, 2^31),
+ * Bi, C, h or w < 1, c0 < 0 or c0 + C > ldo. */
 int dagr_sample_features(const float *img, int Bi, int C, int h, int w, const float *posx, const float *posy,
                          const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
                          void *stream);

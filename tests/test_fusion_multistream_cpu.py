@@ -43,19 +43,19 @@ def _geom(B=2):
     return Geometry(240, 180, B, device="cpu")
 
 
-def _x0(lib, a, N=1 << 10, nplanes=4, stride=4):
-    return lib.dagr_l1_x0_image_planes(a["g"], N, a["start"], a["xyb"], None, a["img"], 8, 8, nplanes, a["plane"], stride, a["out"],
+def _x0(lib, a, N=1 << 10, nplanes=4, stride=4, h=8, w=8, C=64, ld=80):
+    return lib.dagr_l1_x0_image_planes(a["g"], N, a["start"], a["xyb"], None, a["img"], h, w, nplanes, a["plane"], stride, a["out"],
                                        None)
 
 
-def _vox(lib, a, N=1 << 10, nplanes=4, stride=4):
-    return lib.dagr_voxel_sample_max_planes(a["g"], N, a["start"], a["xyb"], a["img"], 64, 8, 8, nplanes, a["plane"], stride, a["out"],
-                                            80, 16, 0, None)
+def _vox(lib, a, N=1 << 10, nplanes=4, stride=4, h=8, w=8, C=64, ld=80):
+    return lib.dagr_voxel_sample_max_planes(a["g"], N, a["start"], a["xyb"], a["img"], C, h, w, nplanes, a["plane"], stride, a["out"],
+                                            ld, 16, 0, None)
 
 
-def _sample(lib, a, N=1 << 10, nplanes=4, stride=4):
-    return lib.dagr_sample_features_planes(a["img"], nplanes, a["plane"], stride, 64, 8, 8, a["posx"], a["posy"], a["bidx"], N, 240,
-                                           180, a["out"], 80, 16, None)
+def _sample(lib, a, N=1 << 10, nplanes=4, stride=4, h=8, w=8, C=64, ld=80):
+    return lib.dagr_sample_features_planes(a["img"], nplanes, a["plane"], stride, C, h, w, a["posx"], a["posy"], a["bidx"], N, 240,
+                                           180, a["out"], ld, 16, None)
 
 
 def _head(lib, a, N=None, nplanes=4, stride=4):
@@ -92,9 +92,13 @@ def test_planes_entry_points_reject_null_pointers(name, null):
 
 COUNTS = [(dict(nplanes=0), "nplanes"), (dict(nplanes=-3), "nplanes"), (dict(stride=0), "plane_stride"), (dict(stride=-4), "plane_stride")]
 EVENTS = [(dict(N=-1), "N out of range"), (dict(N=1 << 31), "N out of range")]          # dagr_head_finish_planes takes no count
+# the sampling forms' maps and rows (c0 = 16): h, w >= 1 and the channels [c0, c0 + C) within the row stride
+MAPS = [(dict(h=0), "h, w >= 1"), (dict(w=0), "h, w >= 1")]
+ROWS = {"dagr_voxel_sample_max_planes": [(dict(ld=79), "ldx")], "dagr_sample_features_planes": [(dict(ld=79), "ldo"), (dict(C=0), "C, h, w")]}
 
 
-@pytest.mark.parametrize("name,kw,needle", [(n, kw, m) for n in sorted(ENTRY) for kw, m in COUNTS + (EVENTS if "head" not in n else [])])
+@pytest.mark.parametrize("name,kw,needle", [(n, kw, m) for n in sorted(ENTRY) for kw, m in COUNTS + (EVENTS if "head" not in n else [])]
+                         + [(n, kw, m) for n in sorted(ENTRY) for kw, m in (MAPS if "head" not in n else []) + ROWS.get(n, [])])
 def test_planes_entry_points_reject_bad_counts(name, kw, needle):
     from dagr_b200 import _lib
     lib = _lib.load()
