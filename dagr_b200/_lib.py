@@ -53,6 +53,10 @@ class PoolWs(C.Structure):
     _fields_ = [(k, i64) for k in ("acc", "possum", "ptmax", "pcnt", "pmask")]
 
 
+class EvalParams(C.Structure):
+    _fields_ = [("iou_thrs", C.c_double * 10), ("rec_thrs", C.c_double * 101), ("area_rng", C.c_double * 8)]
+
+
 class L1AParams(C.Structure):
     _fields_ = [("w", f32 * (KU * 3 * 16)), ("root", f32 * (3 * 16)),
                 ("scale", f32 * 16), ("shift", f32 * 16), ("relu", i32)]
@@ -139,6 +143,8 @@ _SIGS = {
     "dagr_masked_lin":(C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p]),
     "dagr_masked_inplace_bn": (C.c_int, [p, i64, p, p, p, p, p, p, C.c_int, f32, p]),
     "dagr_masked_isdiff": (C.c_int, [p, i64, p, p, C.c_int, f32, f32, p]),
+    "dagr_eval_workspace_bytes": (C.c_int, [i64, C.c_int, i64, i64, C.POINTER(i64)]),
+    "dagr_evaluate_bbox": (C.c_int, [p, p, p, p, p, p, p, i64, C.c_int, i64, i64, C.POINTER(EvalParams), p, i64, p, p, p]),
 }
 
 EXPORTS = tuple(_SIGS.keys())

@@ -5,7 +5,7 @@ Only the record format is in scope (the evaluation harness around it is not, SUR
   scripts/run_test_interframe.py:21-45  to_npy / save_detections
 plus `records_from_device`, which turns the batched device output of `Engine.postprocess` (det [B,A,6], ndet [B])
 into one record array per image with a single device->host copy (the reference loops over images and tensors).
-COCO evaluation itself (pycocotools, src/dagr/utils/coco_eval.py) is outside the hot path and not rebuilt.
+COCO evaluation (DetectionBuffer.compute, src/dagr/utils/coco_eval.py) runs on the device in dagr_b200.evaluation.
 """
 from __future__ import annotations
 

@@ -594,6 +594,37 @@ int dagr_stream_ingest(const int32_t *raw_stage, int streams, int max_raw, int f
 int dagr_frame_preprocess(const uint8_t *frames, int nframes, int src_h, int src_w, int scale, int out_h, int out_w,
                           uint8_t *out_u8, float *out_f32, const float *lut, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * COCO bbox evaluation: the reference's DetectionBuffer.compute / evaluate_detection (src/dagr/utils/buffers.py:118-123,
+ * coco_eval.py:64-230), i.e. pycocotools' COCOeval (evaluate + accumulate) with maxDets = 100, on the device.
+ *
+ *   gt_box f32[n_gt][4] / dt_box f32[n_det][4]  xyxy, 16-byte aligned; gt_label / dt_label i64 (the class index, taken
+ *         modulo 2^32 like the reference's uint32 class_id); dt_score f32[n_det].
+ *   gt_off / dt_off i64[n_images + 1]: image i owns GT rows [gt_off[i], gt_off[i+1]) and detection rows [dt_off[i], dt_off[i+1]).
+ *   params_host: the float64 thresholds and area ranges (np.linspace(.5, .95, 10), np.linspace(0, 1, 101), COCO areaRng).
+ *   precision f64[10][101][K][4] and recall f64[10][K][4] (out): COCOeval.eval['precision'|'recall'][..., maxDets = 100].
+ * Semantics: x, y, w = x2 - x1, h = y2 - y1 and area = w * h in float32; images without GT contribute nothing; per (image,
+ * class) the detections are ranked by descending score (stable) and the first 100 kept; IoU is bbIou in double; greedy
+ * matching per area range and IoU threshold as evaluateImg (GTs outside the range last, unmatched detections outside it
+ * ignored); per (class, area) the kept detections of every image, stably sorted by score, give cumulative tp / fp,
+ * rc = tp / npig, pr = tp / (fp + tp + 2^-52), the right-to-left max envelope and searchsorted(rc, rec_thrs, 'left').
+ * A class without a GT inside the area range keeps -1.  Boxes must be finite.  One warp per (image, class) stages up to 32
+ * GTs and their IoU table; more GTs of one class in one image take the same arithmetic from global memory.
+ * workspace: dagr_eval_workspace_bytes bytes, 256-byte aligned, no initialisation.
+ * Limits (DAGR_E_ARG before anything is launched): n_images >= 1, 1 <= K <= 65535, n_images * K < 2^31 - 1,
+ * n_det < 2^31, n_images < 2^31 / 100, no null pointer (row pointers may be NULL when their count is 0).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+    double iou_thrs[10];
+    double rec_thrs[101];
+    double area_rng[4][2];         /* all, small, medium, large: [lo, hi], a box is outside when area < lo or area > hi */
+} dagr_eval_params_t;
+int dagr_eval_workspace_bytes(int64_t n_images, int K, int64_t n_gt, int64_t n_det, int64_t *bytes);
+int dagr_evaluate_bbox(const float *gt_box, const int64_t *gt_label, const int64_t *gt_off, const float *dt_box,
+                       const float *dt_score, const int64_t *dt_label, const int64_t *dt_off, int64_t n_images, int K,
+                       int64_t n_gt, int64_t n_det, const dagr_eval_params_t *params_host, void *workspace,
+                       int64_t workspace_bytes, double *precision, double *recall, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
