@@ -59,6 +59,9 @@ extern "C" int dagr_check_config(const dagr_geom_t *g, int64_t N, int cin0, int 
     DAGR_UNSUPPORTED(g->ncell != (2 * g->r + 1) * (2 * g->r + 1), "ncell %d != (2r+1)^2", g->ncell);
     DAGR_UNSUPPORTED(g->r >= g->CW || g->r >= g->CH, "radius %d px must be smaller than a pool1 voxel (%dx%d px): coarse edges would leave the "
                      "8-neighbourhood the voxel-grid layers assume", g->r, g->CW, g->CH);
+    const int64_t nk = (int64_t)g->B * g->ny1 * g->nx1 * g->CP;
+    DAGR_UNSUPPORTED(nk >= (1ll << 31), "B*ny1*nx1*CP = %lld sort keys: the graph sort's 32-bit sort key holds fewer than 2^31", (long long)nk);
+    DAGR_UNSUPPORTED(g->NK != nk, "NK %d != B*ny1*nx1*CP = %lld", g->NK, (long long)nk);
     DAGR_UNSUPPORTED(N < 0 || N >= (1ll << 24), "N = %lld events per call: sorted positions are packed in 24 bits (N < 16.7 M)", (long long)N);
     DAGR_UNSUPPORTED(cout0 != 16 || (cin0 != 3 && cin0 != 19), "conv_block1 = Layer(%d -> %d): the event-level kernels implement 3 -> 16 (events "
                      "only) and 19 -> 16 (image fusion), i.e. base_width 0.5 as in every reference config", cin0, cout0);

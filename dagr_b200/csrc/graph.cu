@@ -227,6 +227,8 @@ static int graph_sort_impl(const dagr_geom_t *g, const int32_t *batch, const int
                            int32_t *flags, void *stream)
 {
     DAGR_CHECK_ARG(g && g->W <= 4096 && g->H <= 4096 && g->B <= 256, "geometry out of range (W,H<=4096, B<=256)");
+    const int64_t nk = (int64_t)g->B * g->ny1 * g->nx1 * g->CP;      // the keys and the count / start tables are int32
+    DAGR_CHECK_ARG(nk < (1ll << 31) && g->NK == nk, "geometry out of range (NK = B*ny1*nx1*CP must be < 2^31: 32-bit sort key)");
     DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
     cudaStream_t st = (cudaStream_t)stream;
     if (N > 0) {

@@ -169,6 +169,9 @@ class Geometry:
         self.xkey = (cx * self.CP + (torch.arange(W) - x0[cx])).int()
         self.ykey = (cy * self.nx1 * self.CP + (torch.arange(H) - y0[cy]) * self.CW).int()
         self.NK = B * self.ny1 * self.nx1 * self.CP
+        if self.NK >= 1 << 31:
+            raise ValueError(f"{B} x {self.ny1} x {self.nx1} pool1 voxels of {self.CP} pixels give {self.NK} sort keys: the "
+                             "graph sort's 32-bit sort key holds fewer than 2^31")
         self.cells1 = B * self.ny1 * self.nx1
         self.spiral = spiral_offsets(self.r)
 

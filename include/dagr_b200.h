@@ -128,6 +128,8 @@ int dagr_prepare_events(const float *pos /*[N,3]*/, const int64_t *batch /*[N]*/
  *                       xyb u32[N] = x | y<<12 | b<<24, feat_s f32[N]
  *                       work: key i32[N], tmp i32[N], count i32[NK+1] (MUST be zero on entry; is
  *                       zero again on exit), blocksums i32[dagr_scan_blocks(NK+1)+1]
+ *                       The sort keys are int32: every sort form (and dagr_check_config) refuses a geometry whose
+ *                       B*ny1*nx1*CP is >= 2^31 or differs from NK, before anything is launched.
  *   dagr_l1_build     : (below) -> nbr i32[16,N] COLUMN-MAJOR ELL: slot q of node p at [q*N+p]; slots 0..14 =
  *                       src positions in probe order, slot 15 = degree without the self loop;
  *                       off u16[16,N] (spiral cell index of each neighbour, same layout), cellmask u32[B*ny1*nx1] (bit (dcy+1)*3+(dcx+1) set when some
