@@ -75,16 +75,19 @@ extern "C" int dagr_downsample_events(const uint16_t *x, const uint16_t *y, cons
                                       int out_w, int out_h, float *change_map, int32_t *cell, int32_t *tmp, int32_t *sorted,
                                       int32_t *count, int32_t *start, int32_t *blocksums, uint8_t *mask, void *stream)
 {
-    DAGR_CHECK_ARG(fx >= 1 && fy >= 1 && out_w >= 1 && out_h >= 1, "bad down-sampling geometry");
-    DAGR_CHECK_ARG(N < (1ll << 31), "N must fit int32");
-    if (N <= 0) return DAGR_OK;
+    DAGR_CHECK_ARG(change_map && count && start && blocksums, "null argument");
+    DAGR_CHECK_ARG(N == 0 || (x && y && p && cell && tmp && sorted && mask), "null argument (the N-long rows may be NULL only when N = 0)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N must be in [0, 2^31)");
+    DAGR_CHECK_ARG(fx >= 1 && fy >= 1 && out_w >= 1 && out_h >= 1, "bad down-sampling geometry: fx, fy, out_w, out_h must be >= 1");
+    DAGR_CHECK_ARG((int64_t)out_w * out_h < (1ll << 31), "out_w * out_h must be < 2^31");
+    if (N == 0) return DAGR_OK;
     cudaStream_t st = (cudaStream_t)stream;
     const int cells = out_w * out_h;
     k_ds_hist<<<dagr_div_up(N, 256), 256, 0, st>>>(x, y, N, fx, fy, out_w, out_h, cell, count);
     scan_exclusive(count, start, (int64_t)cells, blocksums, st);          // start[cells] = N
     k_ds_scatter<<<dagr_div_up(N, 256), 256, 0, st>>>(cell, N, start, count, tmp);
     k_ds_rank<<<dagr_div_up(N, 256), 256, 0, st>>>(cell, tmp, N, start, sorted);
-    k_ds_walk<<<dagr_div_up(cells, 128), 128, 0, st>>>(p, start, sorted, cells, (double)(fx * fy), change_map, mask);
+    k_ds_walk<<<dagr_div_up(cells, 128), 128, 0, st>>>(p, start, sorted, cells, (double)fx * fy, change_map, mask);
     DAGR_CHECK_LAUNCH();
     return DAGR_OK;
 }
@@ -114,8 +117,13 @@ extern "C" int dagr_compact_events(const uint8_t *mask, int64_t N, const uint16_
                                    const int8_t *p, int fx, int fy, int32_t *flag, int32_t *pos, int32_t *blocksums,
                                    uint16_t *xo, uint16_t *yo, int64_t *to, int8_t *po, int32_t *n_out, void *stream)
 {
+    DAGR_CHECK_ARG(pos && blocksums && n_out, "null argument");
+    DAGR_CHECK_ARG(N == 0 || (mask && x && y && t && p && flag && xo && yo && to && po),
+                   "null argument (the N-long rows may be NULL only when N = 0)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N must be in [0, 2^31)");
+    DAGR_CHECK_ARG(fx >= 1 && fy >= 1, "fx and fy must be >= 1");
     cudaStream_t st = (cudaStream_t)stream;
-    if (N <= 0) { DAGR_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int32_t), st)); return DAGR_OK; }
+    if (N == 0) { DAGR_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int32_t), st)); return DAGR_OK; }
     k_mask_to_int<<<dagr_div_up(N, 256), 256, 0, st>>>(mask, N, flag);
     scan_exclusive(flag, pos, N, blocksums, st);
     k_compact<<<dagr_div_up(N, 256), 256, 0, st>>>(flag, pos, N, x, y, t, p, fx, fy, xo, yo, to, po);
@@ -129,31 +137,32 @@ extern "C" int dagr_compact_events(const uint8_t *mask, int64_t N, const uint16_
 // batch i32[M], pos i32[M,3], polarity f32[M]  (the arrays DAGR.forward derives from a formatted Batch)
 // ------------------------------------------------------------------------------------------------
 __global__ void k_ing_flag(const uint16_t *__restrict__ y, const int64_t *__restrict__ t, int64_t N, int H, long long t_cut,
-                           int32_t *__restrict__ flag, unsigned long long *__restrict__ tlast)
+                           int32_t *__restrict__ flag, unsigned long long *__restrict__ ilast)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     bool keep = false;
-    long long ti = 0;
-    if (i < N) { ti = t[i]; keep = (int)y[i] < H && ti < t_cut; flag[i] = keep ? 1 : 0; }
-    // t[-1] of the kept events (dsec_data.py:145): the stream is time-sorted, so the last kept event has the largest t.
-    // (raw timestamps are non-negative microseconds)
-    long long m = keep ? ti : -1;
+    if (i < N) { keep = (int)y[i] < H && t[i] < t_cut; flag[i] = keep ? 1 : 0; }
+    // t[-1] of the kept events (dsec_data.py:145) is the t of the last kept event in array order, whatever the order or
+    // sign of the timestamps: reduce the largest kept index (N < 2^31), -1 when nothing is kept
+    int m = keep ? (int)i : -1;
     for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
-    if ((threadIdx.x & 31) == 0 && m >= 0) atomicMax(tlast, (unsigned long long)m);
+    if ((threadIdx.x & 31) == 0 && m >= 0) atomicMax(reinterpret_cast<long long *>(ilast), (long long)m);
 }
 
 __global__ void k_ing_emit(const int32_t *__restrict__ flag, const int32_t *__restrict__ pos, int64_t N,
                            const uint16_t *__restrict__ x, const uint16_t *__restrict__ y, const int64_t *__restrict__ t,
                            const int8_t *__restrict__ p, int p_is_01, float W, float H, int T,
-                           const unsigned long long *__restrict__ tlast, int b, int32_t *__restrict__ batch_o,
+                           const unsigned long long *__restrict__ ilast, int b, int32_t *__restrict__ batch_o,
                            int32_t *__restrict__ pos_o, float *__restrict__ feat_o)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N || !flag[i]) return;
     const int j = pos[i];
     // data/utils.py:12-13: xy -> int16, t -> int32;  dsec_data.py:145: t = time_window + t - t[-1]
+    // (a kept event exists, so ilast >= 0; the int64 sum wraps as numpy's does, and the int32 cast keeps the low bits)
     const int xi = (int)(int16_t)x[i], yi = (int)(int16_t)y[i];
-    const int tr = (int)((long long)T + t[i] - (long long)*tlast);
+    const long long tlast = t[(long long)*ilast];
+    const int tr = (int)(long long)((unsigned long long)T + (unsigned long long)t[i] - (unsigned long long)tlast);
     // buffers.py:43: int / int -> fp32 true division;  ev_tgn.py:15-16: (pos * [W,H,T] + 1e-3).int()
     const float Tf = (float)T;
     const float px = __fdiv_rn((float)xi, W), py = __fdiv_rn((float)yi, H), pt = __fdiv_rn((float)tr, Tf);
@@ -170,10 +179,14 @@ extern "C" int dagr_ingest_events(const uint16_t *x, const uint16_t *y, const in
                                   int32_t *blocksums, unsigned long long *tlast, int32_t *batch_out, int32_t *pos_out,
                                   float *feat_out, int32_t *n_out, void *stream)
 {
+    DAGR_CHECK_ARG(pos && blocksums && tlast && n_out, "null argument");
+    DAGR_CHECK_ARG(N == 0 || (x && y && t && p && flag && batch_out && pos_out && feat_out),
+                   "null argument (the N-long rows may be NULL only when N = 0)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N must be in [0, 2^31)");
+    DAGR_CHECK_ARG(W >= 1 && H >= 1 && T >= 1, "W, H and T must be >= 1");
     cudaStream_t st = (cudaStream_t)stream;
-    DAGR_CHECK_ARG(N < (1ll << 31), "N must fit int32");
-    DAGR_CUDA(cudaMemsetAsync(tlast, 0, sizeof(unsigned long long), st));
-    if (N <= 0) { DAGR_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int32_t), st)); return DAGR_OK; }
+    DAGR_CUDA(cudaMemsetAsync(tlast, 0xff, sizeof(unsigned long long), st));   // -1: no kept event yet
+    if (N == 0) { DAGR_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int32_t), st)); return DAGR_OK; }
     k_ing_flag<<<dagr_div_up(N, 256), 256, 0, st>>>(y, t, N, H, (long long)t_cut, flag, tlast);
     scan_exclusive(flag, pos, N, blocksums, st);
     k_ing_emit<<<dagr_div_up(N, 256), 256, 0, st>>>(flag, pos, N, x, y, t, p, p_is_01, (float)W, (float)H, T, tlast, sample,

@@ -534,13 +534,20 @@ int dagr_masked_isdiff(int64_t *idx_inout, int64_t K, const float *a, const floa
  *       fx = int(in_w/out_w), fy = int(in_h/out_h); change_map f32[out_h*out_w] is the per-output-pixel accumulator that
  *       the script carries from chunk to chunk (in/out).  mask u8[N] (out) = 1 where the event passes.
  *       work: cell,tmp,sorted i32[N]; count i32[out_h*out_w] (MUST be zero on entry; is zero again on exit);
- *       start i32[out_h*out_w+1]; blocksums i32[dagr_scan_blocks(max(N, out_h*out_w))+2].
- *   dagr_compact_events   : events[mask] with x/fx, y/fy as (x / fx).astype(uint16) (:102-104); order preserved.
- *       work: flag i32[N], pos i32[N+1]; n_out i32[1] (device) = number kept.
- *   dagr_ingest_events    : one sample: keep t < t_cut (dsec_data.py:177-179) and y < H (:142-143), t = T + t - t[-1] of
- *       the kept events (:144-145), polarity 2p-1 when p_is_01 (:146), int16/int32 casts (data/utils.py:12-13), fp32
- *       normalisation by [W,H,T] (utils/buffers.py:41-43) and denormalisation (ev_tgn.py:15-16) -> batch i32[M] (= sample),
- *       pos i32[M,3], polarity f32[M]: the inputs of dagr_graph_sort.  work: flag i32[N], pos i32[N+1], tlast u64[1].
+ *       start i32[out_h*out_w+1]; blocksums i32[dagr_scan_blocks(max(N, out_h*out_w))+2].  Every mask byte is written.
+ *       Output cell (min(x / fx, out_w - 1), min(y / fy, out_h - 1)): the reference would index out of bounds.
+ *   dagr_compact_events   : events[mask] with x/fx, y/fy as (x / fx).astype(uint16) (:102-104); order preserved; any
+ *       non-zero mask byte keeps its event.  work: flag i32[N], pos i32[N+1], blocksums i32[dagr_scan_blocks(N)+2];
+ *       n_out i32[1] (device) = number kept.  Nothing is written to xo, yo, to, po past n_out.
+ *   dagr_ingest_events    : one sample: keep t < t_cut (dsec_data.py:177-179) and y < H (:142-143), t = T + t - t[-1]
+ *       (:144-145) where t[-1] is the t of the last kept event in array order (the events need not be time-sorted, and
+ *       t may be negative), polarity 2p-1 when p_is_01 (:146; else p as is), int16/int32 casts (data/utils.py:12-13:
+ *       x, y >= 2^15 and relative t outside int32 wrap), fp32 normalisation by [W,H,T] (utils/buffers.py:41-43) and
+ *       denormalisation (ev_tgn.py:15-16) -> batch i32[M] (= sample), pos i32[M,3], polarity f32[M]: the inputs of
+ *       dagr_graph_sort.  work: flag i32[N], pos i32[N+1], blocksums i32[dagr_scan_blocks(N)+2], tlast u64[1] (the
+ *       index of the last kept event, -1 when none).
+ * All three return DAGR_E_ARG with a message before anything is launched on a null pointer (the N-long rows may be NULL
+ * when N = 0), N outside [0, 2^31), fx or fy < 1, out_w or out_h < 1, out_w * out_h >= 2^31, or W, H or T < 1.
  * ------------------------------------------------------------------------------------------- */
 int dagr_downsample_events(const uint16_t *x, const uint16_t *y, const int8_t *p, int64_t N, int fx, int fy,
                            int out_w, int out_h, float *change_map, int32_t *cell, int32_t *tmp, int32_t *sorted,

@@ -9,8 +9,9 @@ Follows, line by line:
     fp32), src/dagr/model/layers/ev_tgn.py:11-16 ((pos*[W,H,T]+1e-3).int())
 
 Pinned by tests/golden/downsample_golden.npz, generated in the build container from the reference's own numba
-function (tests/golden/make_downsample_golden.py).  The preprocessing part has no reference-side fixture: its fixed
-points are the arithmetic identities tested in tests/test_oracle_cpu.py.
+function (tests/golden/make_downsample_golden.py), and by tests/golden/ingest_window_golden.npz, generated from the
+reference's own preprocess_events / to_data / format_data / denormalize_pos (tests/golden/make_ingest_window_golden.py);
+tests/test_ingest_kernels_cpu.py checks preprocess_window against it bit for bit.
 """
 import numpy as np
 
@@ -45,7 +46,8 @@ def downsample_events(events, input_height, input_width, output_height, output_w
 
 def preprocess_window(events, width, height, time_window, t_cut=None):
     """dsec_data.py:177-179 then :141-147 then data/utils.py:6-20, buffers.py:33-44 and ev_tgn.py:11-16:
-    raw (x, y, t us, p in {0,1}) -> pos_denorm int32[M,3], polarity float32[M]."""
+    raw (x, y, t us, p in {0,1}) -> pos_denorm int32[M,3], polarity float32[M].  t[-1] is the t of the last kept event in
+    array order, whatever the order or sign of the timestamps."""
     ev = dict(events)
     if t_cut is not None:
         keep = ev["t"] < t_cut

@@ -172,3 +172,17 @@ def image_branch_cpu(model, data):
         cnn_in = [torch.nn.functional.interpolate(o, size=tuple(sz)) for o, sz in zip(outs[-model.head.num_scales:], sizes)]
         image_outs = model.head.cnn_head(cnn_in)
     return [f.float().contiguous() for f in feats], {k: [t.float().contiguous() for t in v] for k, v in image_outs.items()}
+
+
+def downsample_golden_cases(g):
+    """the cases of tests/golden/downsample_golden.npz: [(case, (iw, ih, ow, oh), map0 float32[oh, ow] or None, chunks)],
+    where map0 is the change map the first chunk starts from (None: zeros) and chunks the number of chunks the map is
+    carried over."""
+    out = []
+    for case in sorted(int(k[1:-len("_shape")]) for k in g.files if k.endswith("_shape")):
+        n = 0
+        while f"c{case}_k{n}_map" in g.files:
+            n += 1
+        m0 = g[f"c{case}_map0"].copy() if f"c{case}_map0" in g.files else None
+        out.append((case, tuple(int(v) for v in g[f"c{case}_shape"]), m0, n))
+    return out

@@ -631,15 +631,17 @@ def test_masked_ops_vs_oracle_and_reference():
 
 def test_ingest_downsampler_vs_reference_golden_and_oracle():
     """csrc/ingest.cu vs (a) the golden vectors made by the reference's own numba down-sampler, chunk by chunk with the
-    change map carried over, and (b) the oracle on a larger random stream with hot pixels; bit-exact (mask, coordinates,
+    change map carried over from the case's initial map (every case of the fixture), and (b) the oracle on a larger random stream with hot pixels; bit-exact (mask, coordinates,
     accumulator map)."""
     from dagr_b200 import ingest
     from oracle import ref_ingest as R
+    from tests.helpers import downsample_golden_cases
     g = np.load(ROOT / "tests" / "golden" / "downsample_golden.npz")
-    for case in range(3):
-        iw, ih, ow, oh = (int(v) for v in g[f"c{case}_shape"])
-        cm = None
-        for k in range(3):
+    cases = downsample_golden_cases(g)
+    assert len(cases) >= 10
+    for case, (iw, ih, ow, oh), m0, chunks in cases:
+        cm = None if m0 is None else torch.from_numpy(m0).cuda()
+        for k in range(chunks):
             ev = {q: torch.from_numpy(g[f"c{case}_k{k}_in_{q}"].astype({"x": "int16", "y": "int16", "p": "int8", "t": "int64"}[q])).cuda()
                   for q in "xypt"}
             out, cm = ingest.downsample_events(ev, ih, iw, oh, ow, change_map=cm)

@@ -282,15 +282,17 @@ def test_oracle_reproduces_committed_golden_forward():
 
 def test_ingest_oracle_vs_reference_golden():
     """oracle/ref_ingest.py against tests/golden/downsample_golden.npz, which was produced by the reference's own numba
-    down-sampler (scripts/downsample_events.py:91-124) with the change map carried over three chunks."""
+    down-sampler (scripts/downsample_events.py:91-124) with the change map carried over each case's chunks: every case,
+    the seeded maps near +-1 at denominators 1, 2, 3, 8 and 9 included."""
     import numpy as np
     from pathlib import Path
     from oracle import ref_ingest as R
+    from tests.helpers import downsample_golden_cases
     g = np.load(Path(__file__).parent / "golden" / "downsample_golden.npz")
-    for case in range(3):
-        iw, ih, ow, oh = (int(v) for v in g[f"c{case}_shape"])
-        cm = None
-        for k in range(3):
+    cases = downsample_golden_cases(g)
+    assert len(cases) >= 10
+    for case, (iw, ih, ow, oh), cm, chunks in cases:
+        for k in range(chunks):
             ev = {q: g[f"c{case}_k{k}_in_{q}"] for q in "xypt"}
             out, cm = R.downsample_events(ev, ih, iw, oh, ow, change_map=cm)
             for q in "xypt":

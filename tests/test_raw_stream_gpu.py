@@ -89,18 +89,26 @@ def _ingest_call(raw_np, S, max_raw, fx, fy, ow, oh, crop, cmap, max_chunk):
 
 
 def test_ingest_kernel_equals_reference_golden_chunk_by_chunk():
-    """the three cases of downsample_golden.npz (the reference's own numba function, change map carried over three chunks)
-    through dagr_stream_ingest at S = 1, no crop, +-1 polarities: 640x480 -> 320x240; 64x48 -> 32x24 with a hot-pixel chunk;
-    96x48 -> 32x24 (fx = 3, fy = 2)."""
+    """every case of downsample_golden.npz (the reference's own numba function, change map carried over the case's chunks
+    from its initial map) through dagr_stream_ingest at S = 1, no crop, +-1 polarities: 640x480 -> 320x240; 64x48 -> 32x24
+    with a hot-pixel chunk; 96x48 -> 32x24 (fx = 3, fy = 2); fx x fy = 1x1, 2x1, 3x1, 3x3 and 4x2 from maps seeded near
+    +-1; more output cells than events; a 16384-event chunk with 7000 events in one cell."""
     from dagr_b200.streaming import pack_raw_stage
+    from tests.helpers import downsample_golden_cases
     g = np.load(GOLD_PATH)
-    MR = 6000                                                     # the largest golden chunk
-    for case in range(3):
-        iw, ih, ow, oh = (int(v) for v in g[f"c{case}_shape"])
+    cases = downsample_golden_cases(g)
+    assert len(cases) >= 10
+    MR = max(len(g[f"c{c}_k{k}_in_t"]) for c, _, _, n in cases for k in range(n))   # the largest golden chunk
+    assert MR <= 16384
+    for case, (iw, ih, ow, oh), m0, chunks in cases:
         fx, fy = iw // ow, ih // oh
+        if fx * fy == 1 and m0 is not None and m0.any():
+            continue                  # at 1x1 the stream's map is never walked and stays 0: a seeded map is not its state
         cmap = torch.zeros((1, oh, ow), dtype=torch.float32, device="cuda")
+        if m0 is not None:
+            cmap[0] = torch.from_numpy(m0)
         raw = np.zeros(4 + 2 * MR, np.int32)
-        for k in range(3):
+        for k in range(chunks):
             x, y, p, t = (g[f"c{case}_k{k}_in_{q}"] for q in "xypt")
             pack_raw_stage(raw, [(x, y, t, p)], [-123], MR, planes=[5])
             hdr, rows = _ingest_call(raw, 1, MR, fx, fy, ow, oh, oh, cmap, MR)
