@@ -38,6 +38,7 @@ own init + update criterion.
 """
 from __future__ import annotations
 
+import gc
 import time
 
 import numpy as np
@@ -62,12 +63,17 @@ def _pow2_at_least(n: int) -> int:
 
 
 class _RingDetector:
-    """What StreamingDetector and MultiStreamDetector share: the device rings of `streams` x `cap` slots, a pinned stage
+    """The streaming detector of S event cameras that every class below is: S device rings of `cap` slots, a pinned stage
     and its device copy, and the step itself -- H2D of the stage, push, forward over the live windows, NMS, D2H of the
     detections and of the control block.  The first two steps run eagerly (they allocate every buffer of the step); the
     second is followed by one capture, and every later step is one replay of that CUDA graph.  A detector whose steps read
     different buffers (FusionStreamingDetector's two frame slots) keeps one graph per _graph_key(); a key first used after
     the warm-up is captured right after its first (eager) step.
+
+    The step pushes the S rings with dagr_stream_push_multi and sorts them with dagr_graph_sort_rings.  The one-camera
+    classes (_one_ring) are S = 1 on their own step: dagr_stream_push on an i32[8] control block, dagr_graph_sort_ring and
+    the single-ring image taps (ring_streams=None).  Their stage {n_new, t_cut, 0, 0, events} is the S = 1 packed stage, so
+    everything on the host is shared.
 
     Raw sensor mode (`sensor=(width, height)`): the detector takes the camera's own events and runs the reference's 2x
     down-sampler (scripts/downsample_events.py), the crop to the model's height (dsec_data.py:142-143), the polarity 2p - 1
@@ -76,42 +82,52 @@ class _RingDetector:
     output.  Each stream keeps its down-sampler's change map on the device and its time base (the first raw timestamp
     after a reset) on the host."""
 
+    _one_ring = False
+
     def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device, sensor=None, p_is_01=True):
+        S = int(streams)
+        if not 1 <= S <= MAX_STREAMS:
+            raise ValueError(f"streams={streams}: 1 <= streams <= {MAX_STREAMS}")
+        cap = _pow2_at_least(capacity)
+        if S * cap >= MAX_RING_SLOTS:
+            raise ValueError(f"streams * capacity = {S} * {cap} must be < 2^24 (sorted positions are packed in 24 bits)")
+        if not 1 <= int(max_chunk) <= cap:
+            raise ValueError(f"max_chunk={max_chunk} must be in [1, capacity={cap}]")
+        self.S = self._B = S
+        self._ring_streams = None if self._one_ring else S
         self.model, self.eng = model, model.engine
         self.lib = self.eng.lib
         self.W, self.H = int(model.width), int(model.height)
         self.window_us, self.max_chunk = int(window_us), int(max_chunk)
-        self.cap = _pow2_at_least(capacity)
+        self.cap = cap
         self._check_sensor(sensor, p_is_01)
         dev = torch.device(device) if device is not None else next(model.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("dagr_b200: streaming needs a CUDA device (no CPU fallback)")
         self.dev = dev
-        n = streams * self.cap
+        n = S * cap
         self.batch = torch.zeros(n, dtype=torch.int32, device=dev)
         self.pos = torch.zeros((n, 3), dtype=torch.int32, device=dev)
         self.feat = torch.zeros(n, dtype=torch.float32, device=dev)
-        nstage = 4 * streams + 4 * streams * self.max_chunk
+        nstage = 4 * S + 4 * S * self.max_chunk
         self.stage_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
-        if self.sensor is None:
-            self.stage_h = torch.zeros(nstage, dtype=torch.int32).pin_memory()
-            self._stage_np = self.stage_h.numpy()
-        else:
-            nraw = 4 * streams + 2 * streams * self.max_chunk
-            self.stage_h = torch.zeros(nraw, dtype=torch.int32).pin_memory()        # the raw stage
-            self.raw_d = torch.zeros(nraw, dtype=torch.int32, device=dev)
-            self._raw_np = self.stage_h.numpy()
+        if self.sensor is not None:
+            nstage = 4 * S + 2 * S * self.max_chunk                            # the pinned stage holds the raw chunks
+            self.raw_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
             ow, oh = self.grid
-            self._cmap = torch.zeros((streams, oh, ow), dtype=torch.float32, device=dev)
-            self._tbase = [None] * streams    # per stream: raw timestamp of rebased time 0
-            self._tend = [None] * streams     # per stream: raw t_end of its last step
-            self._nraw = [0] * streams        # per stream: raw events of the last submitted chunk
-        self._nstreams = streams
+            self._cmap = torch.zeros((S, oh, ow), dtype=torch.float32, device=dev)
+            self._tbase = [None] * S          # per stream: raw timestamp of rebased time 0
+            self._tend = [None] * S           # per stream: raw t_end of its last step
+            self._nraw = [0] * S              # per stream: raw events of the last submitted chunk
+        self.stage_h = torch.zeros(nstage, dtype=torch.int32).pin_memory()
+        self._stage_np = self.stage_h.numpy()
+        self.stage_bytes = 4 * nstage
         self.stream = torch.cuda.Stream(device=dev)
         self.graphs = {}                      # _graph_key() -> captured step
         self._res_h = None
         self._done = None
         self._warm = 0
+        self.ctl = torch.zeros(RING_CTL if self._one_ring else (S + 1) * RING_CTL, dtype=torch.int32, device=dev)
 
     @property
     def graph(self):
@@ -135,7 +151,9 @@ class _RingDetector:
         return None
 
     def _push(self):
-        raise NotImplementedError
+        _lib.check(self.lib.dagr_stream_push_multi(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
+                                                   _lib.ptr(self.feat), self.cap, self.S, self.max_chunk, _lib.stream_ptr()),
+                   "stream_push_multi")
 
     def _check_sensor(self, sensor, p_is_01):
         """raw sensor mode: the down-sampling factor and grid of a `sensor` = (width, height) stream for this model."""
@@ -161,7 +179,7 @@ class _RingDetector:
 
     def _ingest(self):
         ow, oh = self.grid
-        self.eng._run("stream_ingest", self.lib.dagr_stream_ingest, _lib.ptr(self.raw_d), self._nstreams, self.max_chunk, self.scale,
+        self.eng._run("stream_ingest", self.lib.dagr_stream_ingest, _lib.ptr(self.raw_d), self.S, self.max_chunk, self.scale,
                       self.scale, ow, oh, self.H, _lib.ptr(self._cmap), _lib.ptr(self.stage_d), self.max_chunk, _lib.stream_ptr())
 
     def _enqueue(self):
@@ -213,6 +231,63 @@ class _RingDetector:
             ev.record(self.stream)
         self._done = ev
 
+    def _submit(self, chunks, t_end):
+        """enqueue one step: chunks[s] = (x, y, t, p) host arrays of stream s or None, t_end None or t_end[s] = end of stream
+        s's time slice or None (see MultiStreamDetector.submit).  Every chunk is checked (raw sensor mode: and rebased) before
+        the stage is written: a refused step does no device work and leaves every time base as it was."""
+        S = self.S
+        if len(chunks) != S:
+            raise ValueError(f"{len(chunks)} chunks for {S} streams")
+        if t_end is not None and len(t_end) != S:
+            raise ValueError(f"{len(t_end)} t_end values for {S} streams")
+        if self.sensor is None:
+            rows = [None if c is None or len(c[2]) == 0 else tuple(np.asarray(a) for a in c) for c in chunks]
+            for s, c in enumerate(rows):
+                if c is not None and len(c[2]) > self.max_chunk:
+                    raise ValueError(f"stream {s}: chunk of {len(c[2])} events exceeds max_chunk={self.max_chunk}")
+            hdr = self._stage_np[:4 * S].reshape(S, 4)
+            t_cut = []
+            for s, c in enumerate(rows):
+                te = None if t_end is None else t_end[s]
+                if te is None:
+                    te = int(c[2][-1]) if c is not None else int(hdr[s, 1]) + self.window_us
+                t_cut.append(int(te) - self.window_us)
+        else:
+            rows, t_cut, bases, ends = self._raw_rows(chunks, t_end)
+        if self._done is not None:
+            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
+        if self.sensor is None:
+            pack_stage(self._stage_np, rows, t_cut, self.max_chunk, planes=self._stage_planes())
+        else:
+            self._nraw = pack_raw_stage(self._stage_np, rows, t_cut, self.max_chunk, planes=self._stage_planes())
+            self._tbase, self._tend = bases, ends
+        self._step()
+
+    def result(self):
+        """detections of the last step, one dict(boxes f32[n,4] xyxy px, scores f32[n], labels i64[n]) per stream (host tensors)."""
+        self._done.synchronize()
+        return [self._dets(s) for s in range(self.S)]
+
+    def reset(self, stream=None):
+        """forget the live window of one stream (the others keep theirs) or of all streams (raw sensor mode: and its change
+        map and time base)."""
+        if self._done is not None:
+            self._done.synchronize()
+        if stream is None:
+            streams = range(self.S)
+            self.ctl.zero_()
+        else:
+            s = int(stream)
+            if not 0 <= s < self.S:
+                raise IndexError(f"stream {stream} out of range [0, {self.S})")
+            streams = [s]
+            self.ctl[RING_CTL * s:RING_CTL * (s + 1)].zero_()
+        if self.sensor is not None:
+            for s in streams:
+                self._cmap[s].zero_()
+                self._tbase[s] = self._tend[s] = None
+                self._nraw[s] = 0
+
     def _dets(self, s: int):
         det_h, ndet_h, _ = self._res_h
         n = int(ndet_h[s])
@@ -235,7 +310,7 @@ class _RingDetector:
         return self.pos[idx], self.feat[idx]
 
     # ---- raw sensor mode ---------------------------------------------------------------------------------------------
-    def _raw_rows(self, s, c):
+    def _raw_chunk(self, s, c):
         """check one raw chunk (x, y, t int64 us, p) of stream s and rebase its time; raises ValueError, touches nothing."""
         x, y, t, p = (np.asarray(a) for a in c)
         n = len(t)
@@ -256,14 +331,13 @@ class _RingDetector:
                              f"base {base} us (reset the stream to start a new base)")
         return base, (x, y, tr, p)
 
-    def _submit_raw(self, chunks, t_end):
-        """raw sensor mode: check and rebase every chunk, then fill the raw stage and step.  Nothing is touched (no device
-        work, no time base) when a chunk is refused."""
+    def _raw_rows(self, chunks, t_end):
+        """check and rebase every raw chunk: (rows, t_cut, time bases, raw t_end per stream) of the step, nothing touched."""
         rows, t_cut, bases, ends = [], [], list(self._tbase), list(self._tend)
         for s, c in enumerate(chunks):
             row = None
             if c is not None and len(c[2]) > 0:
-                bases[s], row = self._raw_rows(s, c)
+                bases[s], row = self._raw_chunk(s, c)
             rows.append(row)
             te = None if t_end is None else t_end[s]
             if te is None:
@@ -273,20 +347,7 @@ class _RingDetector:
             if cut > _I32_MAX:
                 raise ValueError(f"stream {s}: t_end {te} us leaves the int32 range of the stream's time base {bases[s]} us")
             t_cut.append(max(cut, _I32_MIN))
-        if self._done is not None:
-            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
-        self._nraw = pack_raw_stage(self._raw_np, rows, t_cut, self.max_chunk, planes=self._stage_planes())
-        self._tbase, self._tend = bases, ends
-        self._step()
-
-    def _forget(self, s=None):
-        """raw sensor mode: stream s (every stream when None) starts over: zero change map, no time base."""
-        if self.sensor is None:
-            return
-        for k in (range(self._nstreams) if s is None else [s]):
-            self._cmap[k].zero_()
-            self._tbase[k] = self._tend[k] = None
-            self._nraw[k] = 0
+        return rows, t_cut, bases, ends
 
     def _change_map(self, s: int):
         if self.sensor is None:
@@ -303,41 +364,26 @@ class StreamingDetector(_RingDetector):
     p in {0, 1}, or +-1 with p_is_01=False), down-sampled, cropped and rebased inside the step (see _RingDetector); the
     model's width must divide the sensor's.  max_chunk then bounds the raw events of a chunk (<= 16384)."""
 
-    _B, _ring_streams = 1, None
+    _one_ring = True
 
     def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None, sensor=None,
                  p_is_01: bool = True):
         if model.backbone.use_image:
             raise NotImplementedError("streaming mode drives the events-only model")
         self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
-
-    # ------------------------------------------------------------------------------------------------------------
-    def reset(self):
-        """forget the live window (raw sensor mode: and the change map and time base)."""
-        if self._done is not None:
-            self._done.synchronize()
-        self.ctl.zero_()
-        self._forget()
-
-    def change_map(self):
-        """raw sensor mode: host copy of the down-sampler's accumulators f32[h, w] after the last step (for tests)."""
-        return self._change_map(0)
 
     def _push(self):
         _lib.check(self.lib.dagr_stream_push(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
                                              _lib.ptr(self.feat), self.cap, self.max_chunk, 0, _lib.stream_ptr()), "stream_push")
 
-    def _fill_stage(self, x, y, t, p, t_end):
-        n = int(len(t))
-        if n > self.max_chunk:
-            raise ValueError(f"chunk of {n} events exceeds max_chunk={self.max_chunk}")
-        st = self._stage_np
-        st[0] = n
-        st[1] = int(t_end) - self.window_us
-        if n:
-            ev = st[4:4 + 4 * n].reshape(n, 4)
-            ev[:, 0] = x; ev[:, 1] = y; ev[:, 2] = t; ev[:, 3] = p
+    # ------------------------------------------------------------------------------------------------------------
+    def reset(self):
+        """forget the live window (raw sensor mode: and the change map and time base)."""
+        super().reset()
+
+    def change_map(self):
+        """raw sensor mode: host copy of the down-sampler's accumulators f32[h, w] after the last step (for tests)."""
+        return self._change_map(0)
 
     @torch.no_grad()
     def submit(self, x, y, t, p, t_end=None):
@@ -347,20 +393,7 @@ class StreamingDetector(_RingDetector):
         Raw sensor mode: x, y at the sensor's resolution, t int64 us, p in {0, 1} (or +-1, p_is_01=False), t_end in raw
         time; a chunk over max_chunk, outside the sensor or whose rebased time leaves int32 raises ValueError before any
         device work."""
-        if self.sensor is not None:
-            self._submit_raw([(x, y, t, p)], None if t_end is None else [t_end])
-            return
-        if self._done is not None:
-            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
-        if t_end is None:
-            t_end = int(t[-1]) if len(t) else int(self._stage_np[1]) + self.window_us
-        self._fill_stage(np.asarray(x), np.asarray(y), np.asarray(t), np.asarray(p), t_end)
-        self._step()
-
-    def result(self):
-        """detections of the last submitted chunk: [dict(boxes f32[n,4] xyxy px, scores f32[n], labels i64[n])] (host tensors)."""
-        self._done.synchronize()
-        return [self._dets(0)]
+        self._submit([(x, y, t, p)], None if t_end is None else [t_end])
 
     def push(self, x, y, t, p, t_end=None):
         self.submit(x, y, t, p, t_end)
@@ -390,15 +423,6 @@ def _check_raw_frames(raw_frames, sensor):
         raise ValueError("raw_frames takes the camera's own frames: it needs sensor=(width, height)")
 
 
-def _frame_setup(det, raw_frames):
-    """frame handling of the fusion detectors after _setup: the frame stream, the image branch precision (read once from the
-    model: a later change of model.image_precision does not reach the detector), and with raw_frames the u8 -> f32 table."""
-    det.frame_stream = torch.cuda.Stream(device=det.dev)
-    det.image_precision = det.model.image_precision
-    det.raw_frames = bool(raw_frames)
-    det._frame_lut = ingest.frame_lut(det.dev) if det.raw_frames else None
-
-
 class _CameraFrames:
     """The frames of one hybrid camera, for the fusion detectors: two frame slots, the frame pending in the trunk, the frame
     in use, and the done-event of the last step that read each slot.
@@ -419,6 +443,7 @@ class _CameraFrames:
         self.cur_frame = None                 # (id, t_us) of that frame
         self.pending = None                   # frame whose trunk may still run: dict(slot, id, t_us, ready, trunk)
         self.step_frame = (None, None)        # (id, t_us) of the frame the last submitted step used
+        self.overlapped = False               # the last submitted step ran while a newer frame's trunk was in flight
         self.nframes = 0
         self.img_h = self.h2d = None
 
@@ -507,10 +532,11 @@ class _CameraFrames:
 
     def take_newest(self):
         """before a step: the newest frame whose trunk has finished becomes current (a non-blocking query; the first frame is
-        taken whatever its state, the step waits for it on the device).  Returns whether a newer frame is still in flight."""
+        taken whatever its state, the step waits for it on the device).  `overlapped`: whether a newer frame is still in
+        flight."""
         if self.pending is not None and (self.cur is None or self.pending["ready"].query()):
             self.promote()
-        return self.pending is not None
+        self.overlapped = self.pending is not None
 
     def stepped(self, done):
         """after a step was enqueued: it reads the current slot until `done`."""
@@ -522,7 +548,48 @@ class _CameraFrames:
         return dict(frame=fid, t_us=t_us, pending=None if self.pending is None else self.pending["id"])
 
 
-class FusionStreamingDetector(StreamingDetector):
+class _FusionDetector:
+    """What the two fusion detectors add to their ring detector: the cameras `_cams` (one _CameraFrames each; the one-camera
+    detector has a list of one) and the frame policy of a step.  A step is refused before any device work while some
+    camera has never had a frame; before the step each camera's newest frame whose copy has finished becomes current (a
+    non-blocking query; a camera's first frame is waited for on the device), and after it the step reads that frame's slot
+    until it is done."""
+
+    def _frame_setup(self, raw_frames, slot_dsts):
+        """after _setup: the frame stream, the image branch precision (read once from the model: a later change of
+        model.image_precision does not reach the detector), with raw_frames the u8 -> f32 table, and one camera per entry of
+        slot_dsts (its _CameraFrames.slot_dst)."""
+        self.frame_stream = torch.cuda.Stream(device=self.dev)
+        self.image_precision = self.model.image_precision
+        self.raw_frames = bool(raw_frames)
+        self._frame_lut = ingest.frame_lut(self.dev) if self.raw_frames else None
+        self._cams = [_CameraFrames(self, dst) for dst in slot_dsts]
+
+    def _camera(self, s):
+        s = int(s)
+        if not 0 <= s < self.S:
+            raise IndexError(f"camera {s} out of range [0, {self.S})")
+        return self._cams[s]
+
+    def _submit(self, chunks, t_end):
+        missing = [s for s, c in enumerate(self._cams) if c.cur is None and c.pending is None]
+        if missing:
+            raise RuntimeError(f"{type(self).__name__}: set_frame() must be called for every camera before the first step "
+                               f"(no frame yet: cameras {missing})")
+        for c in self._cams:
+            c.take_newest()
+        super()._submit(chunks, t_end)
+        for c in self._cams:
+            c.stepped(self._done)
+
+    def _frame_state(self, s):
+        cam = self._camera(s)
+        if self._done is not None:
+            self._done.synchronize()
+        return cam.state()
+
+
+class FusionStreamingDetector(_FusionDetector, StreamingDetector):
     """Streaming detection with the hybrid (image + events) model: camera frames at frame rate, event chunks in between.
 
         det = FusionStreamingDetector(model, window_us=50_000)
@@ -535,8 +602,9 @@ class FusionStreamingDetector(StreamingDetector):
 
     Which frame a step uses: the newest frame whose trunk has finished when the chunk is submitted (a non-blocking event
     query).  Chunks keep flowing on the previous frame while the next frame's trunk runs; sync_frame() blocks until the
-    pending frame is usable, so the next step uses it.  The first step waits for the first frame.  After every step the
-    detections equal model(data) over the live window with the image of the frame that frame_state reports.
+    pending frame is usable, so the next step uses it.  The first step waits for the first frame; submit raises
+    RuntimeError before any device work while no frame was set.  After every step the detections equal model(data) over
+    the live window with the image of the frame that frame_state reports.
 
     raw_frames=True (with sensor=(width, height)): set_frame takes the camera's own frame, u8 [height, width, 3] (HWC, the
     camera's channel order), and the reference's crop + cv2.resize(INTER_CUBIC) by the integer factor width / W
@@ -548,11 +616,8 @@ class FusionStreamingDetector(StreamingDetector):
         _check_fusion_model(model, "FusionStreamingDetector", "StreamingDetector")
         _check_raw_frames(raw_frames, sensor)
         self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self.ctl = torch.zeros(RING_CTL, dtype=torch.int32, device=self.dev)
-        _frame_setup(self, raw_frames)
         self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
-        self._cam = _CameraFrames(self, self._slot_dst)
-        self._overlapped = False              # the last submitted step ran while a newer frame's trunk was in flight
+        self._frame_setup(raw_frames, [self._slot_dst])
 
     def _slot_dst(self, slot, feats, outs):
         if self._slots is None:
@@ -561,8 +626,17 @@ class FusionStreamingDetector(StreamingDetector):
         return self._slots[slot]
 
     @property
+    def _cam(self):
+        return self._cams[0]
+
+    @property
     def _cur(self):
         return self._cam.cur
+
+    @property
+    def _overlapped(self):
+        """the last submitted step ran while a newer frame's trunk was in flight."""
+        return self._cam.overlapped
 
     # ------------------------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -583,30 +657,19 @@ class FusionStreamingDetector(StreamingDetector):
     def _image_inputs(self):
         return self._slots[self._cam.cur]
 
-    @torch.no_grad()
-    def submit(self, x, y, t, p, t_end=None):
-        """as StreamingDetector.submit; the step uses the newest frame whose trunk has finished (see the class docstring)."""
-        self._overlapped = self._cam.take_newest()
-        if self._cam.cur is None:
-            raise RuntimeError("FusionStreamingDetector: set_frame() must be called before the first chunk")
-        super().submit(x, y, t, p, t_end)
-        self._cam.stepped(self._done)
-
     @property
     def frame_state(self):
         """dict(frame=id of the frame the last finished step used, t_us=its timestamp, pending=id of a frame not yet in use
         or None)."""
-        if self._done is not None:
-            self._done.synchronize()
-        return self._cam.state()
+        return self._frame_state(0)
 
 
 def pack_stage(stage: np.ndarray, chunks, t_cut, max_chunk: int, planes=None):
     """write the packed multi-stream stage of dagr_stream_push_multi into the int32 array `stage` (>= 4*S + 4*S*max_chunk
     entries): header [S][4] = {n_new, t_cut, event offset, plane}, then the (x, y, t, polarity) rows of all streams back to
-    back.  chunks[s] = (x, y, t, p) host arrays or None (no events).  planes[s] = the frame plane stream s's step reads (image
-    fusion, read by the *_planes kernels; the push ignores the word), 0 when `planes` is None.  Returns the per-stream event
-    counts."""
+    back; S = 1 is the stage of dagr_stream_push.  chunks[s] = (x, y, t, p) host arrays or None (no events).  planes[s] =
+    the frame plane stream s's step reads (image fusion, read by the *_planes kernels; the push ignores the word), 0 when
+    `planes` is None.  Returns the per-stream event counts."""
     S = len(chunks)
     ns = [0 if c is None else len(c[2]) for c in chunks]
     for s, n in enumerate(ns):
@@ -674,41 +737,7 @@ class MultiStreamDetector(_RingDetector):
                  sensor=None, p_is_01: bool = True):
         if model.backbone.use_image:
             raise NotImplementedError("streaming mode drives the events-only model")
-        self._setup_streams(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
-
-    def _setup_streams(self, model, streams, window_us, max_chunk, capacity, device, sensor=None, p_is_01=True):
-        S = int(streams)
-        if not 1 <= S <= MAX_STREAMS:
-            raise ValueError(f"streams={streams}: 1 <= streams <= {MAX_STREAMS}")
-        cap = _pow2_at_least(capacity)
-        if S * cap >= MAX_RING_SLOTS:
-            raise ValueError(f"streams * capacity = {S} * {cap} must be < 2^24 (sorted positions are packed in 24 bits)")
-        if not 1 <= int(max_chunk) <= cap:
-            raise ValueError(f"max_chunk={max_chunk} must be in [1, capacity={cap}]")
-        self.S = self._B = self._ring_streams = S
-        self._setup(model, S, window_us, max_chunk, cap, device, sensor, p_is_01)
-        self.ctl = torch.zeros((S + 1) * RING_CTL, dtype=torch.int32, device=self.dev)
-        self.stage_bytes = 4 * self.stage_h.numel()
-
-    def _push(self):
-        _lib.check(self.lib.dagr_stream_push_multi(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
-                                                   _lib.ptr(self.feat), self.cap, self.S, self.max_chunk, _lib.stream_ptr()),
-                   "stream_push_multi")
-
-    def reset(self, stream=None):
-        """forget the live window of one stream (the others keep theirs) or of all streams (raw sensor mode: and its change
-        map and time base)."""
-        if self._done is not None:
-            self._done.synchronize()
-        if stream is None:
-            self.ctl.zero_()
-            self._forget()
-        else:
-            s = int(stream)
-            if not 0 <= s < self.S:
-                raise IndexError(f"stream {stream} out of range [0, {self.S})")
-            self.ctl[RING_CTL * s:RING_CTL * (s + 1)].zero_()
-            self._forget(s)
+        self._setup(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
 
     def change_map(self, s: int):
         """raw sensor mode: host copy of stream s's down-sampler accumulators f32[h, w] after the last step (for tests)."""
@@ -720,34 +749,7 @@ class MultiStreamDetector(_RingDetector):
         t_end[s] = end of stream s's time slice (None, or t_end=None: its last timestamp, or for an empty chunk the previous
         end).  Returns immediately; `result()` blocks on the step.  Raw sensor mode: raw chunks and raw t_end, as
         StreamingDetector.submit."""
-        S = self.S
-        if len(chunks) != S:
-            raise ValueError(f"{len(chunks)} chunks for {S} streams")
-        if t_end is not None and len(t_end) != S:
-            raise ValueError(f"{len(t_end)} t_end values for {S} streams")
-        if self.sensor is not None:
-            self._submit_raw(chunks, t_end)
-            return
-        cs =[None if c is None or len(c[2]) == 0 else tuple(np.asarray(a) for a in c) for c in chunks]
-        for s, c in enumerate(cs):
-            if c is not None and len(c[2]) > self.max_chunk:
-                raise ValueError(f"stream {s}: chunk of {len(c[2])} events exceeds max_chunk={self.max_chunk}")
-        if self._done is not None:
-            self._done.synchronize()                                  # the stage / result buffers of the previous step are free
-        hdr = self._stage_np[:4 * S].reshape(S, 4)
-        t_cut = []
-        for s, c in enumerate(cs):
-            te = None if t_end is None else t_end[s]
-            if te is None:
-                te = int(c[2][-1]) if c is not None else int(hdr[s, 1]) + self.window_us
-            t_cut.append(int(te) - self.window_us)
-        pack_stage(self._stage_np, cs, t_cut, self.max_chunk, planes=self._stage_planes())
-        self._step()
-
-    def result(self):
-        """detections of the last step, one dict(boxes f32[n,4] xyxy px, scores f32[n], labels i64[n]) per stream (host tensors)."""
-        self._done.synchronize()
-        return [self._dets(s) for s in range(self.S)]
+        self._submit(chunks, t_end)
 
     def push(self, chunks, t_end=None):
         self.submit(chunks, t_end)
@@ -762,7 +764,7 @@ class MultiStreamDetector(_RingDetector):
         return self._live(s)
 
 
-class FusionMultiStreamDetector(MultiStreamDetector):
+class FusionMultiStreamDetector(_FusionDetector, MultiStreamDetector):
     """S hybrid (image + events) cameras on one GPU: MultiStreamDetector with a camera frame per stream.
 
         det = FusionMultiStreamDetector(model, streams=S, window_us=50_000)
@@ -791,11 +793,9 @@ class FusionMultiStreamDetector(MultiStreamDetector):
                  sensor=None, p_is_01: bool = True, raw_frames: bool = False):
         _check_fusion_model(model, "FusionMultiStreamDetector", "MultiStreamDetector")
         _check_raw_frames(raw_frames, sensor)
-        self._setup_streams(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        _frame_setup(self, raw_frames)
+        self._setup(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
         self._planes = None                   # (image_feats, image_outs) as plane arrays [2S, ...]
-        self._cams = [_CameraFrames(self, lambda j, f, o, s=s: self._plane_dst(2 * s + j, f, o)) for s in range(self.S)]
-        self._overlapped = [False] * self.S   # per camera: the last step ran while a newer frame of it was in flight
+        self._frame_setup(raw_frames, [lambda j, f, o, s=s: self._plane_dst(2 * s + j, f, o) for s in range(self.S)])
 
     def _plane_dst(self, k, feats, outs):
         if self._planes is None:
@@ -808,11 +808,10 @@ class FusionMultiStreamDetector(MultiStreamDetector):
         pf, po = self._planes
         return [f[k:k + 1] for f in pf], {key: [t[k:k + 1] for t in v] for key, v in po.items()}
 
-    def _camera(self, s):
-        s = int(s)
-        if not 0 <= s < self.S:
-            raise IndexError(f"camera {s} out of range [0, {self.S})")
-        return self._cams[s]
+    @property
+    def _overlapped(self):
+        """per camera: the last submitted step ran while a newer frame of it was in flight."""
+        return [c.overlapped for c in self._cams]
 
     @torch.no_grad()
     def set_frame(self, s: int, image, t_us=None):
@@ -834,25 +833,10 @@ class FusionMultiStreamDetector(MultiStreamDetector):
     def _stage_planes(self):
         return [2 * s + c.cur for s, c in enumerate(self._cams)]
 
-    @torch.no_grad()
-    def submit(self, chunks, t_end=None):
-        """as MultiStreamDetector.submit; each camera's step uses its newest frame whose copy has finished."""
-        missing = [s for s, c in enumerate(self._cams) if c.cur is None and c.pending is None]
-        if missing:
-            raise RuntimeError(f"FusionMultiStreamDetector: set_frame() must be called for every camera before the first step "
-                               f"(no frame yet: cameras {missing})")
-        self._overlapped = [c.take_newest() for c in self._cams]
-        super().submit(chunks, t_end)
-        for c in self._cams:
-            c.stepped(self._done)
-
     def frame_state(self, s: int):
         """camera s after the last finished step: dict(frame=id of the frame the step used, t_us=its timestamp, pending=id of a
         frame of camera s not yet in use or None)."""
-        cam = self._camera(s)
-        if self._done is not None:
-            self._done.synchronize()
-        return cam.state()
+        return self._frame_state(s)
 
 
 def synth_stream(rate_ev_s: int, seconds: float, width: int, height: int, seed: int = 99, kind: str = "uniform"):
@@ -864,56 +848,145 @@ def synth_stream(rate_ev_s: int, seconds: float, width: int, height: int, seed: 
     return x.numpy(), y.numpy(), t.numpy(), p.numpy()
 
 
-def stream_benchmark(dev, size="l", width=640, height=480, rate_ev_s=1_000_000, chunk_us=1000, window_us=50_000, seconds=2.0,
-                     kind="uniform", model=None):
-    """config 5: per-chunk latency (host submit -> detections on the host) and sustained rate of ONE stream on ONE GPU.
-    Latency mode: a chunk is submitted, its detections are awaited, then the next chunk is submitted (a real-time consumer);
-    the wall clock per chunk is what a 1 ms chunk period has to accommodate."""
+# ---- benchmarks ----------------------------------------------------------------------------------------------------
+def _bench_setup(dev, model, size, width, height, streams, rate_ev_s, chunk_us, window_us, seconds, kind, **image):
+    """what the stream benchmarks set up: the seeded model (unless `model` is given; `image` = use_image / img_net of the
+    hybrid model), `streams` synthetic streams (seeds 99, 100, ...) of seconds + window + 20 ms, each stream's bounds on
+    the chunk grid, and the detectors' max_chunk (four mean chunks, at least 4096)."""
     from .model.dagr import DAGR
     from .utils.args import default_args
     if model is None:
         from tests.helpers import randomize_bn
         torch.manual_seed(0)
-        model = randomize_bn(DAGR(default_args(size, batch_size=1), height=height, width=width).eval()).to(dev)
+        model = randomize_bn(DAGR(default_args(size, batch_size=1, **image), height=height, width=width).eval()).to(dev)
     total_s = seconds + window_us * 1e-6 + 0.02
-    x, y, t, p = synth_stream(rate_ev_s, total_s, width, height, kind=kind)
-    det = StreamingDetector(model, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)))
-    bounds = np.searchsorted(t, np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us))
-    nchunks = len(bounds) - 1
-    lat, dev_ms, evs = [], [], []
-    warm = int(window_us / chunk_us) + 20                                # fill the live window first (+ graph capture)
-    import gc
+    evs = [synth_stream(rate_ev_s, total_s, width, height, seed=99 + s, kind=kind) for s in range(streams)]
+    grid = np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us)
+    return model, evs, [np.searchsorted(e[2], grid) for e in evs], max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4))
+
+
+def _timed_steps(det, submit, evs, bounds, chunk_us, window_us, frames=None):
+    """the latency loop of the stream benchmarks: step k submits every stream's events of [k, k + 1) * chunk_us with t_end =
+    (k + 1) * chunk_us through `submit(chunks, t_end)` and awaits the detections of all streams on the host before the next
+    step is submitted (a real-time consumer).  The first window_us / chunk_us + 20 steps fill the live windows (and capture
+    the graphs); each later step is timed: host wall clock from submit to the detections, and CUDA events around the submit
+    on the detector's stream.  `frames` (_FrameFeed, fusion) sets camera frames between two steps and records what a step
+    used.  Returns host ms, device ms and events of each timed step."""
+    S = len(evs)
+    lat, dev_ms, nev = [], [], []
+    warm = int(window_us / chunk_us) + 20                                # fill the live windows first (+ graph captures)
     gc_was = gc.isenabled()
     gc.collect()
     gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
-    for k in range(nchunks):
-        a, b = int(bounds[k]), int(bounds[k + 1])
-        t_end = (k + 1) * chunk_us
+    for k in range(len(bounds[0]) - 1):
+        if frames is not None:
+            frames.between(k, k >= warm)
+        chunks = []
+        for (x, y, t, p), bd in zip(evs, bounds):
+            a, b = int(bd[k]), int(bd[k + 1])
+            chunks.append((x[a:b], y[a:b], t[a:b], p[a:b]))
+        t_end = [(k + 1) * chunk_us] * S
         if k >= warm:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0 = time.perf_counter()
             e0.record(det.stream)
-            det.submit(x[a:b], y[a:b], t[a:b], p[a:b], t_end)
+            submit(chunks, t_end)
             e1.record(det.stream)
-            out = det.result()
-            lat.append((time.perf_counter() - t0) * 1e3)
+            det.result()
+            t1 = time.perf_counter()
+            lat.append((t1 - t0) * 1e3)
             dev_ms.append(e0.elapsed_time(e1))
-            evs.append(b - a)
+            nev.append(sum(len(c[2]) for c in chunks))
+            if frames is not None:
+                frames.stepped(t1)
         else:
-            det.push(x[a:b], y[a:b], t[a:b], p[a:b], t_end)
+            submit(chunks, t_end)
+            det.result()
     if gc_was:
         gc.enable()
-    st = det.window_state
+    return lat, dev_ms, nev
+
+
+class _FrameFeed:
+    """the cameras of the fusion benchmarks: camera s delivers frame s at stream time 0, before the first step, and frame
+    s + j (of four seeded random u8 images; the trunk's cost does not depend on the pixels) at offset[s] + j * frame_us,
+    set between two steps and, with sync_frames, waited for.  For the frames of the timed steps it records the host time
+    of set_frame (+ sync_frame), the CUDA events around the trunk, and the host time from set_frame until the detections
+    of the first step that used the frame are on the host; for each timed step whether some camera's newer frame was in
+    flight."""
+
+    def __init__(self, det, set_frame, frame_us, chunk_us, offset, sync_frames=False):
+        g = torch.Generator().manual_seed(0)
+        self.images = [torch.randint(0, 256, (3, det.H, det.W), generator=g, dtype=torch.uint8) for _ in range(4)]
+        self.det, self.set_frame, self.frame_us, self.chunk_us, self.offset = det, set_frame, frame_us, chunk_us, offset
+        self.sync_frames = sync_frames
+        self.set_ms, self.trunk, self.overlapped, self.waiting = [], [], [], {}   # waiting: (camera, frame id) -> set_frame time
+        self.first_use = [[] for _ in offset]
+        for s in range(len(offset)):                                     # every camera needs a frame before the first step
+            self._set(s, s, 0, False)
+
+    def _set(self, s, image, t_us, timed):
+        ts = time.perf_counter()
+        fid = self.set_frame(s, self.images[image % len(self.images)], t_us)
+        cam = self.det._cams[s]
+        trunk = cam.pending["trunk"]
+        if self.sync_frames:
+            cam.sync()
+        if timed:
+            self.set_ms.append((time.perf_counter() - ts) * 1e3)
+            self.trunk.append(trunk)
+            self.waiting[(s, fid)] = ts
+
+    def between(self, k, timed):
+        tk = k * self.chunk_us
+        for s, o in enumerate(self.offset):
+            if tk > o and (tk - o) % self.frame_us == 0:                 # camera s delivers a frame at stream time tk
+                self._set(s, s + (tk - o) // self.frame_us, tk, timed)
+
+    def stepped(self, t1):
+        self.overlapped.append(any(c.overlapped for c in self.det._cams))
+        for s, cam in enumerate(self.det._cams):
+            key = (s, cam.step_frame[0])
+            if key in self.waiting:
+                self.first_use[s].append((t1 - self.waiting.pop(key)) * 1e3)
+
+    def trunk_ms(self):
+        torch.cuda.synchronize(self.det.dev)
+        return [a.elapsed_time(b) for a, b in self.trunk]
+
+
+def _q(v, f):
+    """the f-quantile of the sorted list v."""
+    return v[min(len(v) - 1, int(f * len(v)))]
+
+
+def _dist(v):
+    v = sorted(v)
+    return dict(n=len(v), p50=_q(v, 0.5), p99=_q(v, 0.99), max=v[-1]) if v else dict(n=0)
+
+
+def _latency(lat, dev_ms, nev, chunk_us):
+    """the latency fields of the events-only stream benchmarks."""
     lat_s, dev_s = sorted(lat), sorted(dev_ms)
-    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
     busy = sum(lat) * 1e-3
+    return dict(latency_ms=dict(p50=_q(lat_s, 0.5), p90=_q(lat_s, 0.9), p99=_q(lat_s, 0.99), max=lat_s[-1]),
+                device_ms=dict(p50=_q(dev_s, 0.5), p99=_q(dev_s, 0.99)),
+                sustained_mev_s=sum(nev) / busy / 1e6, realtime=bool(_q(lat_s, 0.99) * 1e3 <= chunk_us),
+                realtime_margin=chunk_us / (_q(lat_s, 0.5) * 1e3))
+
+
+def stream_benchmark(dev, size="l", width=640, height=480, rate_ev_s=1_000_000, chunk_us=1000, window_us=50_000, seconds=2.0,
+                     kind="uniform", model=None):
+    """config 5: per-chunk latency (host submit -> detections on the host) and sustained rate of ONE stream on ONE GPU.
+    Latency mode: a chunk is submitted, its detections are awaited, then the next chunk is submitted (a real-time consumer);
+    the wall clock per chunk is what a 1 ms chunk period has to accommodate."""
+    model, evs, bounds, max_chunk = _bench_setup(dev, model, size, width, height, 1, rate_ev_s, chunk_us, window_us, seconds, kind)
+    det = StreamingDetector(model, window_us=window_us, max_chunk=max_chunk)
+    lat, dev_ms, nev = _timed_steps(det, lambda c, te: det.submit(*c[0], te[0]), evs, bounds, chunk_us, window_us)
+    st = det.window_state
     return dict(model=f"dagr-{size}", stream_rate_mev_s=rate_ev_s / 1e6, chunk_us=chunk_us, window_us=window_us,
-                stream_seconds=len(lat) * chunk_us * 1e-6, chunks=len(lat), events_per_chunk=float(np.mean(evs)),
-                live_events=st["live"], overflow=st["overflow"],
-                latency_ms=dict(p50=q(lat_s, 0.5), p90=q(lat_s, 0.9), p99=q(lat_s, 0.99), max=lat_s[-1]),
-                device_ms=dict(p50=q(dev_s, 0.5), p99=q(dev_s, 0.99)),
-                sustained_mev_s=sum(evs) / busy / 1e6, realtime=bool(q(lat_s, 0.99) * 1e3 <= chunk_us),
-                realtime_margin=chunk_us / (q(lat_s, 0.5) * 1e3),
+                stream_seconds=len(lat) * chunk_us * 1e-6, chunks=len(lat), events_per_chunk=float(np.mean(nev)),
+                live_events=st["live"], overflow=st["overflow"], **_latency(lat, dev_ms, nev, chunk_us),
                 note="one stream on one GPU; every chunk: H2D of the chunk from pinned memory, eviction by watermark + append into the "
                      "device ring, full forward over the live window, NMS, D2H of the detections -- one CUDA graph replay; latency = host "
                      "wall clock from submit() to the detections being readable on the host, chunks submitted back to back "
@@ -926,57 +999,15 @@ def multistream_benchmark(dev, streams, size="l", width=640, height=480, rate_ev
     """config 5 with S cameras on ONE GPU: S independent synthetic streams (seeds 99, 100, ...) at `rate_ev_s` each, all
     advanced by one MultiStreamDetector step per chunk period.  Latency mode as in stream_benchmark: a step is submitted,
     the detections of all S streams are awaited on the host, then the next step is submitted."""
-    from .model.dagr import DAGR
-    from .utils.args import default_args
     S = int(streams)
-    if model is None:
-        from tests.helpers import randomize_bn
-        torch.manual_seed(0)
-        model = randomize_bn(DAGR(default_args(size, batch_size=1), height=height, width=width).eval()).to(dev)
-    total_s = seconds + window_us * 1e-6 + 0.02
-    evs_s = [synth_stream(rate_ev_s, total_s, width, height, seed=99 + s, kind=kind) for s in range(S)]
-    det = MultiStreamDetector(model, streams=S, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)),
-                              capacity=capacity)
-    grid = np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us)
-    bounds = [np.searchsorted(e[2], grid) for e in evs_s]
-    nchunks = len(grid) - 1
-    lat, dev_ms, evs = [], [], []
-    warm = int(window_us / chunk_us) + 20                                # fill the live windows first (+ graph capture)
-    import gc
-    gc_was = gc.isenabled()
-    gc.collect()
-    gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
-    for k in range(nchunks):
-        chunks = []
-        for (x, y, t, p), bd in zip(evs_s, bounds):
-            a, b = int(bd[k]), int(bd[k + 1])
-            chunks.append((x[a:b], y[a:b], t[a:b], p[a:b]))
-        t_end = [(k + 1) * chunk_us] * S
-        if k >= warm:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            t0 = time.perf_counter()
-            e0.record(det.stream)
-            det.submit(chunks, t_end)
-            e1.record(det.stream)
-            det.result()
-            lat.append((time.perf_counter() - t0) * 1e3)
-            dev_ms.append(e0.elapsed_time(e1))
-            evs.append(sum(len(c[2]) for c in chunks))
-        else:
-            det.push(chunks, t_end)
-    if gc_was:
-        gc.enable()
+    model, evs, bounds, max_chunk = _bench_setup(dev, model, size, width, height, S, rate_ev_s, chunk_us, window_us, seconds, kind)
+    det = MultiStreamDetector(model, streams=S, window_us=window_us, max_chunk=max_chunk, capacity=capacity)
+    lat, dev_ms, nev = _timed_steps(det, det.submit, evs, bounds, chunk_us, window_us)
     st = [det.window_state(s) for s in range(S)]
-    lat_s, dev_s = sorted(lat), sorted(dev_ms)
-    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
-    busy = sum(lat) * 1e-3
     return dict(model=f"dagr-{size}", streams=S, kind=kind, stream_rate_mev_s=rate_ev_s / 1e6, chunk_us=chunk_us, window_us=window_us,
-                stream_seconds=len(lat) * chunk_us * 1e-6, steps=len(lat), events_per_step=float(np.mean(evs)),
+                stream_seconds=len(lat) * chunk_us * 1e-6, steps=len(lat), events_per_step=float(np.mean(nev)),
                 stage_bytes=det.stage_bytes, live_events=[x["live"] for x in st], overflow=[x["overflow"] for x in st],
-                latency_ms=dict(p50=q(lat_s, 0.5), p90=q(lat_s, 0.9), p99=q(lat_s, 0.99), max=lat_s[-1]),
-                device_ms=dict(p50=q(dev_s, 0.5), p99=q(dev_s, 0.99)),
-                sustained_mev_s=sum(evs) / busy / 1e6, realtime=bool(q(lat_s, 0.99) * 1e3 <= chunk_us),
-                realtime_margin=chunk_us / (q(lat_s, 0.5) * 1e3),
+                **_latency(lat, dev_ms, nev, chunk_us),
                 note=f"{S} independent streams on one GPU, one MultiStreamDetector step per chunk period: H2D of the packed stage "
                      "(fixed size), per-stream eviction + append into S device rings, one batched forward over the S live windows, "
                      "NMS, D2H of the detections -- one CUDA graph replay; latency = host wall clock from submit() until the "
@@ -992,77 +1023,24 @@ def fusion_stream_benchmark(dev, size="s", img_net="resnet50", width=640, height
     its detections are awaited, then the next one); frames are set between two chunks, followed by sync_frame() when
     `sync_frames`.  Frames are seeded random u8 images on the host (the trunk's cost does not depend on the pixels).
     step_priority < 0 runs the steps on a higher-priority stream than the trunk's (an experiment: does it shield the chunks?)."""
-    from .model.dagr import DAGR
-    from .utils.args import default_args
-    if model is None:
-        from tests.helpers import randomize_bn
-        torch.manual_seed(0)
-        model = randomize_bn(DAGR(default_args(size, batch_size=1, use_image=True, img_net=img_net), height=height, width=width).eval()).to(dev)
-    total_s = seconds + window_us * 1e-6 + 0.02
-    x, y, t, p = synth_stream(rate_ev_s, total_s, width, height, kind=kind)
-    g = torch.Generator().manual_seed(0)
-    frames = [torch.randint(0, 256, (3, height, width), generator=g, dtype=torch.uint8) for _ in range(4)]
-    det = FusionStreamingDetector(model, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)))
+    model, evs, bounds, max_chunk = _bench_setup(dev, model, size, width, height, 1, rate_ev_s, chunk_us, window_us, seconds, kind,
+                                                 use_image=True, img_net=img_net)
+    det = FusionStreamingDetector(model, window_us=window_us, max_chunk=max_chunk)
     if step_priority:
         det.stream = torch.cuda.Stream(device=det.dev, priority=step_priority)      # before the first step: captures inherit it
-    bounds = np.searchsorted(t, np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us))
-    nchunks = len(bounds) - 1
-    lat, dev_ms, evs, overlapped, set_ms, trunk, first_use = [], [], [], [], [], [], []
-    waiting = {}                                                         # frame id -> host time of its set_frame
-    warm = int(window_us / chunk_us) + 20                                # fill the live window first (+ both graph captures)
-    import gc
-    gc_was = gc.isenabled()
-    gc.collect()
-    gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
-    for k in range(nchunks):
-        a, b = int(bounds[k]), int(bounds[k + 1])
-        t_end = (k + 1) * chunk_us
-        if (k * chunk_us) % frame_us == 0:                              # the camera delivers a frame at stream time k * chunk_us
-            ts = time.perf_counter()
-            fid = det.set_frame(frames[(k * chunk_us // frame_us) % len(frames)], t_us=k * chunk_us)
-            tr = det._cam.pending["trunk"]
-            if sync_frames:
-                det.sync_frame()
-            if k >= warm:
-                set_ms.append((time.perf_counter() - ts) * 1e3)
-                trunk.append(tr)
-                waiting[fid] = ts
-        if k >= warm:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            t0 = time.perf_counter()
-            e0.record(det.stream)
-            det.submit(x[a:b], y[a:b], t[a:b], p[a:b], t_end)
-            e1.record(det.stream)
-            det.result()
-            t1 = time.perf_counter()
-            lat.append((t1 - t0) * 1e3)
-            dev_ms.append(e0.elapsed_time(e1))
-            evs.append(b - a)
-            overlapped.append(det._overlapped)
-            fid = det._cam.step_frame[0]
-            if fid in waiting:
-                first_use.append((t1 - waiting.pop(fid)) * 1e3)
-        else:
-            det.push(x[a:b], y[a:b], t[a:b], p[a:b], t_end)
-    if gc_was:
-        gc.enable()
-    torch.cuda.synchronize(dev)
-    trunk_ms = [a.elapsed_time(b) for a, b in trunk]
+    frames = _FrameFeed(det, lambda s, image, t_us: det.set_frame(image, t_us=t_us), frame_us, chunk_us, [0], sync_frames)
+    lat, dev_ms, nev = _timed_steps(det, lambda c, te: det.submit(*c[0], te[0]), evs, bounds, chunk_us, window_us, frames)
+    trunk_ms = frames.trunk_ms()
     st = det.window_state
-    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
-
-    def dist(v):
-        v = sorted(v)
-        return dict(n=len(v), p50=q(v, 0.5), p99=q(v, 0.99), max=v[-1]) if v else dict(n=0)
-
+    overlapped = frames.overlapped
     busy = sum(lat) * 1e-3
     return dict(model=f"dagr-{size} + {img_net}", width=width, height=height, stream_rate_mev_s=rate_ev_s / 1e6, chunk_us=chunk_us,
                 window_us=window_us, frame_us=frame_us, sync_frames=bool(sync_frames), step_priority=step_priority, stream_seconds=len(lat) * chunk_us * 1e-6,
-                chunks=len(lat), frames=len(trunk_ms), events_per_chunk=float(np.mean(evs)), live_events=st["live"], overflow=st["overflow"],
-                latency_ms=dist(lat), latency_ms_trunk_in_flight=dist([v for v, o in zip(lat, overlapped) if o]),
-                latency_ms_no_trunk=dist([v for v, o in zip(lat, overlapped) if not o]),
-                device_ms=dist(dev_ms), trunk_device_ms=dist(trunk_ms), set_frame_host_ms=dist(set_ms),
-                frame_to_first_use_ms=dist(first_use), sustained_mev_s=sum(evs) / busy / 1e6,
+                chunks=len(lat), frames=len(trunk_ms), events_per_chunk=float(np.mean(nev)), live_events=st["live"], overflow=st["overflow"],
+                latency_ms=_dist(lat), latency_ms_trunk_in_flight=_dist([v for v, o in zip(lat, overlapped) if o]),
+                latency_ms_no_trunk=_dist([v for v, o in zip(lat, overlapped) if not o]),
+                device_ms=_dist(dev_ms), trunk_device_ms=_dist(trunk_ms), set_frame_host_ms=_dist(frames.set_ms),
+                frame_to_first_use_ms=_dist(frames.first_use[0]), sustained_mev_s=sum(nev) / busy / 1e6,
                 note="one hybrid stream on one GPU: every chunk is one CUDA graph replay of the step of the current frame slot; every "
                      "frame_us of stream time a host u8 frame goes through the ResNet trunk + CNN head (captured ImageBranch graphs) on "
                      "a side stream and is copied into the free slot.  latency = host wall clock from submit() to the detections on the "
@@ -1083,85 +1061,25 @@ def fusion_multistream_benchmark(dev, streams, size="s", img_net="resnet50", wid
     camera, camera s's frames offset by s * frame_us / S (rounded down to the chunk grid) so that the trunks spread out.
     Latency mode as in multistream_benchmark: a step is submitted, the detections of all S cameras are awaited, then the next
     step is submitted; frames are set between two steps and never waited for."""
-    from .model.dagr import DAGR
-    from .utils.args import default_args
     S = int(streams)
-    if model is None:
-        from tests.helpers import randomize_bn
-        torch.manual_seed(0)
-        model = randomize_bn(DAGR(default_args(size, batch_size=1, use_image=True, img_net=img_net), height=height, width=width).eval()).to(dev)
-    total_s = seconds + window_us * 1e-6 + 0.02
-    evs_s = [synth_stream(rate_ev_s, total_s, width, height, seed=99 + s, kind=kind) for s in range(S)]
-    g = torch.Generator().manual_seed(0)
-    frames = [torch.randint(0, 256, (3, height, width), generator=g, dtype=torch.uint8) for _ in range(4)]
-    det = FusionMultiStreamDetector(model, streams=S, window_us=window_us, max_chunk=max(4096, int(rate_ev_s * chunk_us * 1e-6 * 4)),
-                                    capacity=capacity)
+    model, evs, bounds, max_chunk = _bench_setup(dev, model, size, width, height, S, rate_ev_s, chunk_us, window_us, seconds, kind,
+                                                 use_image=True, img_net=img_net)
+    det = FusionMultiStreamDetector(model, streams=S, window_us=window_us, max_chunk=max_chunk, capacity=capacity)
     offset = [(s * frame_us // S) // chunk_us * chunk_us for s in range(S)]
-    grid = np.arange(0, int(total_s * 1e6) + chunk_us, chunk_us)
-    bounds = [np.searchsorted(e[2], grid) for e in evs_s]
-    nchunks = len(grid) - 1
-    lat, dev_ms, evs, overlapped, trunk = [], [], [], [], []
-    first_use = [[] for _ in range(S)]
-    waiting = {}                                                         # (camera, frame id) -> host time of its set_frame
-    warm = int(window_us / chunk_us) + 20                                # fill the live windows first (+ graph capture)
-    for s in range(S):                                                   # every camera needs a frame before the first step
-        det.set_frame(s, frames[s % len(frames)], t_us=0)
-    import gc
-    gc_was = gc.isenabled()
-    gc.collect()
-    gc.disable()                                                         # a collector pause inside a 1 ms chunk period is a latency spike
-    for k in range(nchunks):
-        tk = k * chunk_us
-        for s in range(S):
-            if tk > offset[s] and (tk - offset[s]) % frame_us == 0:      # camera s delivers a frame at stream time tk
-                ts = time.perf_counter()
-                fid = det.set_frame(s, frames[(s + (tk - offset[s]) // frame_us) % len(frames)], t_us=tk)
-                if k >= warm:
-                    trunk.append(det._cams[s].pending["trunk"])
-                    waiting[(s, fid)] = ts
-        chunks = []
-        for (x, y, t, p), bd in zip(evs_s, bounds):
-            a, b = int(bd[k]), int(bd[k + 1])
-            chunks.append((x[a:b], y[a:b], t[a:b], p[a:b]))
-        t_end = [(k + 1) * chunk_us] * S
-        if k >= warm:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            t0 = time.perf_counter()
-            e0.record(det.stream)
-            det.submit(chunks, t_end)
-            e1.record(det.stream)
-            det.result()
-            t1 = time.perf_counter()
-            lat.append((t1 - t0) * 1e3)
-            dev_ms.append(e0.elapsed_time(e1))
-            evs.append(sum(len(c[2]) for c in chunks))
-            overlapped.append(any(det._overlapped))
-            for s, cam in enumerate(det._cams):
-                key = (s, cam.step_frame[0])
-                if key in waiting:
-                    first_use[s].append((t1 - waiting.pop(key)) * 1e3)
-        else:
-            det.push(chunks, t_end)
-    if gc_was:
-        gc.enable()
-    torch.cuda.synchronize(dev)
-    trunk_ms = [a.elapsed_time(b) for a, b in trunk]
+    frames = _FrameFeed(det, det.set_frame, frame_us, chunk_us, offset)
+    lat, dev_ms, nev = _timed_steps(det, det.submit, evs, bounds, chunk_us, window_us, frames)
+    trunk_ms = frames.trunk_ms()
     st = [det.window_state(s) for s in range(S)]
-    q = lambda v, f: v[min(len(v) - 1, int(f * len(v)))]
-
-    def dist(v):
-        v = sorted(v)
-        return dict(n=len(v), p50=q(v, 0.5), p99=q(v, 0.99), max=v[-1]) if v else dict(n=0)
-
+    overlapped = frames.overlapped
     busy = sum(lat) * 1e-3
     return dict(model=f"dagr-{size} + {img_net}", streams=S, width=width, height=height, stream_rate_mev_s=rate_ev_s / 1e6,
                 chunk_us=chunk_us, window_us=window_us, frame_us=frame_us, frame_offset_us=offset, stream_seconds=len(lat) * chunk_us * 1e-6,
-                steps=len(lat), frames=len(trunk_ms), events_per_step=float(np.mean(evs)), live_events=[x["live"] for x in st],
-                overflow=[x["overflow"] for x in st], graphs=len(det.graphs), latency_ms=dist(lat),
-                latency_ms_trunk_in_flight=dist([v for v, o in zip(lat, overlapped) if o]),
-                latency_ms_no_trunk=dist([v for v, o in zip(lat, overlapped) if not o]), steps_trunk_in_flight=int(sum(overlapped)),
-                device_ms=dist(dev_ms), trunk_device_ms=dist(trunk_ms), frame_to_first_use_ms=[dist(v) for v in first_use],
-                sustained_mev_s=sum(evs) / busy / 1e6,
+                steps=len(lat), frames=len(trunk_ms), events_per_step=float(np.mean(nev)), live_events=[x["live"] for x in st],
+                overflow=[x["overflow"] for x in st], graphs=len(det.graphs), latency_ms=_dist(lat),
+                latency_ms_trunk_in_flight=_dist([v for v, o in zip(lat, overlapped) if o]),
+                latency_ms_no_trunk=_dist([v for v, o in zip(lat, overlapped) if not o]),
+                steps_trunk_in_flight=int(sum(overlapped)), device_ms=_dist(dev_ms), trunk_device_ms=_dist(trunk_ms),
+                frame_to_first_use_ms=[_dist(v) for v in frames.first_use], sustained_mev_s=sum(nev) / busy / 1e6,
                 note=f"{S} hybrid cameras on one GPU, one FusionMultiStreamDetector step (one CUDA graph replay) per chunk period; every "
                      "frame_us of stream time each camera's host u8 frame goes through the ResNet trunk + CNN head at B = 1 (captured "
                      "ImageBranch graphs) on the frame stream and is copied into the camera's free plane; latency = host wall clock "

@@ -13,7 +13,7 @@ BAD = C.c_void_p(256)          # never dereferenced: every call below fails its 
 
 
 def test_fusion_multistream_detector_refuses_events_only_no_events_and_bad_limits():
-    from dagr_b200.streaming import FusionMultiStreamDetector
+    from dagr_b200.streaming import FusionMultiStreamDetector, FusionStreamingDetector
     events_only, _ = make_model("n", 180, 240)
     with pytest.raises(ValueError, match="MultiStreamDetector"):
         FusionMultiStreamDetector(events_only, streams=2)
@@ -29,6 +29,13 @@ def test_fusion_multistream_detector_refuses_events_only_no_events_and_bad_limit
         FusionMultiStreamDetector(model, streams=64, capacity=1 << 18)
     with pytest.raises(ValueError, match="max_chunk"):
         FusionMultiStreamDetector(model, streams=2, capacity=1 << 10, max_chunk=4096)
+    # the one-camera detector takes the same construction checks
+    with pytest.raises(ValueError, match="2\\^24"):
+        FusionStreamingDetector(model, capacity=1 << 24)
+    with pytest.raises(ValueError, match="2\\^24"):
+        FusionStreamingDetector(model, capacity=(1 << 23) + 1)            # rounds up to 2^24
+    with pytest.raises(ValueError, match="max_chunk"):
+        FusionStreamingDetector(model, capacity=1 << 10, max_chunk=4096)
 
 
 def test_multistream_detector_still_refuses_fusion_models():

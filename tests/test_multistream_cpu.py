@@ -80,7 +80,7 @@ def test_pack_stage_header_offsets_and_empty_chunks():
 
 
 def test_multistream_detector_rejects_image_fusion_and_oversized_rings():
-    from dagr_b200.streaming import MultiStreamDetector
+    from dagr_b200.streaming import MultiStreamDetector, StreamingDetector
     img, _ = make_model("n", 180, 240, use_image=True, img_net="resnet18")
     with pytest.raises(NotImplementedError, match="events-only"):
         MultiStreamDetector(img, streams=2)
@@ -93,3 +93,10 @@ def test_multistream_detector_rejects_image_fusion_and_oversized_rings():
         MultiStreamDetector(model, streams=0)
     with pytest.raises(ValueError, match="max_chunk"):
         MultiStreamDetector(model, streams=2, capacity=1 << 10, max_chunk=4096)
+    # the one-camera detector takes the same construction checks
+    with pytest.raises(ValueError, match="2\\^24"):
+        StreamingDetector(model, capacity=1 << 24)
+    with pytest.raises(ValueError, match="2\\^24"):
+        StreamingDetector(model, capacity=(1 << 23) + 1)                  # rounds up to 2^24
+    with pytest.raises(ValueError, match="max_chunk"):
+        StreamingDetector(model, capacity=1 << 10, max_chunk=4096)

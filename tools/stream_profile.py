@@ -8,7 +8,7 @@ import torch
 
 sys.path.insert(0, ".")
 from dagr_b200.model.dagr import DAGR
-from dagr_b200.streaming import StreamingDetector, synth_stream
+from dagr_b200.streaming import StreamingDetector, pack_stage, synth_stream
 from dagr_b200.utils.args import default_args
 from tests.helpers import randomize_bn
 
@@ -27,7 +27,7 @@ eng = model.engine
 eng.prof = {}
 for k in range(80, 110):
     a, b = int(bounds[k]), int(bounds[k + 1])
-    det._fill_stage(x[a:b], y[a:b], t[a:b], p[a:b], (k + 1) * 1000)
+    pack_stage(det._stage_np, [(x[a:b], y[a:b], t[a:b], p[a:b])], [(k + 1) * 1000 - det.window_us], det.max_chunk)
     det._enqueue()
 torch.cuda.synchronize()
 prof = eng.prof_summary()
