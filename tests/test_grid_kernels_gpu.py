@@ -115,8 +115,12 @@ def conv_params(rng, tier, cells, Cin, Cout, flags):
     return p, 2.0 ** -13 * (0.5 if p["scale"] is not None else 1.0)
 
 
-def conv_case(Cin, Cout, size, block=False, flags=("bias", "scale", "skip"), seed=0):
-    """run both tiers of one grid-conv case; asserts; returns {tier: (instance, error / bound ratio or 0)}"""
+def conv_case(Cin, Cout, size, block=False, flags=("bias", "scale", "skip"), seed=0, off=0, ldin=0):
+    """run both tiers of one grid-conv case; asserts; returns {tier: (instance, error / bound ratio or 0)}.  The kernel
+    reads columns [off, off + Cin) of a [cells, ldin] array whose other columns are NaN (ldin = 0: a dense [cells, Cin]
+    input); block = True is the second half of [cells, 2 Cin]."""
+    if block:
+        off, ldin = Cin, 2 * Cin
     nsm = n_sm()
     B = 4 if size == "v1" else batch_for(size, nsm)
     cells = B * NX * NY
@@ -132,14 +136,14 @@ def conv_case(Cin, Cout, size, block=False, flags=("bias", "scale", "skip"), see
         g = dict(nx=NX, ny=NY, B=B, cnt=cnt, pxy=pxy, mask=mask, den_x=den[0], den_y=den[1])
         x = dyadic(rng, (cells, Cin), 2, 2) if tier == "exact" else rng.standard_normal((cells, Cin)).astype(np.float32)
         p, step = conv_params(rng, tier, cells, Cin, Cout, flags)
-        if block:                                 # the second half of a [cells, 2 Cin] array; the first half is NaN
-            xfull, off, ldin = np.concatenate([np.full_like(x, np.nan), x], 1), Cin, 2 * Cin
-        else:
-            xfull, off, ldin = x, 0, 0
+        xfull = x
+        if ldin:                                  # a column block of a wider array; the other columns are NaN
+            xfull = np.full((cells, ldin), np.nan, np.float32)
+            xfull[:, off:off + Cin] = x
         out, seen = run_grid_conv(g, xfull, off, ldin, Cin, Cout, p)
         assert seen == {want}, f"{Cin}x{Cout} on {cells} cells: ran {seen}, expected {want}"
         ref, S, n = ref_grid_conv(g, x, p["w"], p["root"], p["bias"], p["scale"], p["shift"], p["skip"], p["relu"])
-        what = f"{Cin}x{Cout} {want} {tier} (B = {B}, flags {'/'.join(flags) or '-'})"
+        what = f"{Cin}x{Cout} {want} {tier} (B = {B}, columns {off}.. of {ldin or Cin}, flags {'/'.join(flags) or '-'})"
         if tier == "exact":
             cells_v, edges = export_grid(NX, NY, B, cnt, mask)
             a = edge_attr(pxy, cells_v, edges, *den)
@@ -157,8 +161,9 @@ def conv_case(Cin, Cout, size, block=False, flags=("bias", "scale", "skip"), see
     return res
 
 
-# (Cin, Cout, column block): the shipped layer / head convs, 18 -> 128 (<16> with a separate partial-sum buffer) and
-# 16 -> 6400 (too wide for every split-K instance: k_grid_conv)
+# (Cin, Cout, column block): a few layer / head convs, 18 -> 128 (<16> with a separate partial-sum buffer) and 16 -> 6400
+# (too wide for every split-K instance: k_grid_conv).  Every shape the shipped configurations launch, derived from the
+# models, runs in tests/test_coarse_shapes_gpu.py.
 SHAPES = [(18, 64, False), (66, 64, False), (64, 64, False), (66, 128, False), (130, 128, False), (128, 256, False),
           (96, 192, False), (32, 100, True), (64, 5, True)]
 CASES = ([(ci, co, blk, "big") for ci, co, blk in SHAPES if instance(ci, co, 10 ** 6, 132) == "sk16"]
@@ -206,6 +211,11 @@ def run_linear_bn(cnt, x, wT, scale, shift):
                                                (7, 130, 13, True), (96, 192, 9, False), (1536, 3, 21, True)])
 def test_grid_linear_bn_vs_float64(Cin, Cout, cells, bn):
     """Cin not a multiple of 8 (clamped rows), cells not a multiple of 8, Cout above 128, scale = NULL"""
+    linear_bn_case(Cin, Cout, cells, bn)
+
+
+def linear_bn_case(Cin, Cout, cells, bn):
+    """both tiers of dagr_grid_linear_bn on `cells` rows, 70 % of them valid, against the float64 matmul"""
     rng = np.random.default_rng([Cin, Cout, cells])
     cnt = (rng.random(cells) < 0.7).astype(np.int32)
     for tier in ("exact", "realistic"):
@@ -354,19 +364,23 @@ def test_grid_pool_flags_a_coarse_edge_over_two_voxels():
     assert int(run_grid_pool(s, 1, 0)["err"][0]) == 0
 
 
-def run_head_finish(s, B, a0=13, tail=6, stride=16):
-    """cls: columns [3, 3 + NC) of a [cells, NC + 7] array; regobj: columns [2, 7) of a [cells, 9] array; out rows outside
-    [a0, a0 + cells per sample) must stay untouched"""
+def run_head_finish(s, B, a0=13, tail=6, stride=16, nc=NC, maps=True):
+    """cls: columns [3, 3 + nc) of a [cells, NC + 7] array; regobj: columns [2, 7) of a [cells, 9] array; the CNN maps
+    add_* (maps = False: all three NULL, as in every events-only model); out rows outside [a0, a0 + cells per sample) must
+    stay untouched"""
     from dagr_b200 import _lib
     lib = _lib.load()
     per = CNX * CNY
     A = a0 + per + tail
-    d = {k: dev(s[k]) for k in ("cnt", "cls", "regobj", "add_cls", "add_reg", "add_obj")}
-    out = torch.full((B, A, 5 + NC), 7.0, device="cuda")
+    d = {k: dev(s[k]) for k in ("cnt", "cls", "regobj", "add_reg", "add_obj")}
+    d["add_cls"] = dev(s["add_cls"][:, :nc])
+    if not maps:
+        d["add_cls"] = d["add_reg"] = d["add_obj"] = None
+    out = torch.full((B, A, 5 + nc), 7.0, device="cuda")
     out[:, a0:a0 + per] = float("nan")
     _lib.check(lib.dagr_head_finish(grid(CNX, CNY, B), _lib.ptr(d["cnt"]), _lib.ptr(d["cls"][:, 3:]), NC + 7,
                                     _lib.ptr(d["regobj"][:, 2:]), 9, _lib.ptr(d["add_cls"]), _lib.ptr(d["add_reg"]),
-                                    _lib.ptr(d["add_obj"]), NC, stride, a0, A, _lib.ptr(out), _lib.stream_ptr()),
+                                    _lib.ptr(d["add_obj"]), nc, stride, a0, A, _lib.ptr(out), _lib.stream_ptr()),
                "dagr_head_finish")
     torch.cuda.synchronize()
     return out.cpu()
@@ -376,8 +390,12 @@ def test_head_finish_vs_float64_and_torch():
     """nc = 100 on column blocks with CNN maps on every cell (empty cells read 0 + map).  xy exactly as torch fp32;
     exp within CUDA's documented 2 ulp of expf (relative 4u), sigmoid 1 / (1 + expf(-v)) within 6u (4u through the
     quotient, one rounding each for the sum and the division); exp overflow to inf and sigmoid saturation equal torch fp32"""
-    B, stride, a0 = 3, 16, 13
-    s = batch([sample(7), sample(8), sample(9)])
+    head_finish_case(NC, True)
+
+
+def head_finish_case(nc, maps, B=3, stride=16, a0=13):
+    """the checks of test_head_finish_vs_float64_and_torch with nc classes, with the CNN maps or with all three NULL"""
+    s = batch([sample(7), sample(8), sample(9)][:B])
     per = CNX * CNY
     # (cell, r, exp overflows or underflows, sigmoid saturates); -20 and -80 are ordinary values far out in the tails
     specials = [(0, 89.0, True, True), (1, 88.7, True, True), (2, 40.0, False, True), (3, -120.0, True, True),
@@ -385,17 +403,20 @@ def test_head_finish_vs_float64_and_torch():
     for i, v, _, _ in specials:                               # on valid cells, with zero maps: r is v itself
         s["cnt"][i] = 1
         s["regobj"][i, 2 + 2:2 + 5] = v
-        s["cls"][i, 3:3 + NC] = v
+        s["cls"][i, 3:3 + nc] = v
         s["add_reg"][0, 2:, 0, i], s["add_obj"][0, 0, 0, i], s["add_cls"][0, :, 0, i] = 0, 0, 0
-    out = run_head_finish(s, B, a0=a0, stride=stride)
+    if not maps:
+        for k in ("add_cls", "add_reg", "add_obj"):
+            s[k] = np.zeros_like(s[k])
+    out = run_head_finish(s, B, a0=a0, stride=stride, nc=nc, maps=maps)
     assert (out[:, :a0] == 7).all() and (out[:, a0 + per:] == 7).all()
-    o = out[:, a0:a0 + per].reshape(B * per, 5 + NC)
+    o = out[:, a0:a0 + per].reshape(B * per, 5 + nc)
     valid = torch.from_numpy(s["cnt"] > 0)[:, None]
     def col(a, lo, hi):
         return torch.where(valid, torch.from_numpy(a[:, lo:hi]), torch.zeros(1))
-    maps = lambda m: torch.from_numpy(m).permute(0, 2, 3, 1).reshape(B * per, -1)     # noqa: E731
-    r = col(s["regobj"], 2, 7) + torch.cat([maps(s["add_reg"]), maps(s["add_obj"])], 1)
-    v = col(s["cls"], 3, 3 + NC) + maps(s["add_cls"])
+    rows = lambda m: torch.from_numpy(np.ascontiguousarray(m)).permute(0, 2, 3, 1).reshape(B * per, -1)     # noqa: E731
+    r = col(s["regobj"], 2, 7) + torch.cat([rows(s["add_reg"]), rows(s["add_obj"])], 1)
+    v = col(s["cls"], 3, 3 + nc) + rows(s["add_cls"][:, :nc])
     a = torch.arange(B * per) % per
     gy, gx = a // CNX, a % CNX
     assert torch.equal(o[:, 0], (r[:, 0] + gx.float()) * stride) and torch.equal(o[:, 1], (r[:, 1] + gy.float()) * stride)
