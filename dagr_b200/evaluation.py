@@ -44,17 +44,22 @@ def workspace_bytes(n_images: int, num_classes: int, n_gt: int, n_det: int) -> i
 
 
 def accumulate(gt_boxes_list: Sequence[Dict[str, torch.Tensor]], dt_boxes_list: Sequence[Dict[str, torch.Tensor]],
-               num_classes: int):
+               num_classes: int, workspace: torch.Tensor = None):
     """COCOeval evaluate + accumulate of the images that have GT, on the device.  Returns (precision f64[10, 101, K, 4],
-    recall f64[10, K, 4]) as CUDA tensors without synchronising, or None when those images hold no detection."""
+    recall f64[10, K, 4]) as CUDA tensors without synchronising, or None when those images hold no detection.
+    `workspace`: a uint8 CUDA tensor of at least workspace_bytes(...) to run in (its contents do not matter); by default
+    one is allocated."""
     pairs = [(g, d) for g, d in zip(gt_boxes_list, dt_boxes_list) if len(g["boxes"]) > 0]
     n_det = sum(len(d["boxes"]) for _, d in pairs)
     if n_det == 0:
         return None
     if not torch.cuda.is_available():
         raise RuntimeError("dagr_b200: detection evaluation runs on a CUDA device (there is no CPU path)")
+    if workspace is not None and (not workspace.is_cuda or workspace.dtype != torch.uint8 or not workspace.is_contiguous()):
+        raise ValueError("workspace must be a contiguous uint8 CUDA tensor")
     lib = _lib.load()
-    dev = next((t.device for g, d in pairs for t in (g["boxes"], d["boxes"]) if t.is_cuda), torch.device("cuda"))
+    dev = next((t.device for g, d in pairs for t in (g["boxes"], d["boxes"]) if t.is_cuda),
+               workspace.device if workspace is not None else torch.device("cuda"))
     K, n = int(num_classes), len(pairs)
 
     def rows(key, dicts, dtype, width=None):
@@ -69,7 +74,13 @@ def accumulate(gt_boxes_list: Sequence[Dict[str, torch.Tensor]], dt_boxes_list: 
     gt_off = torch.tensor(np.cumsum([0] + [len(g["boxes"]) for g in gts]), dtype=torch.int64).to(dev)
     dt_off = torch.tensor(np.cumsum([0] + [len(d["boxes"]) for d in dts]), dtype=torch.int64).to(dev)
     with torch.cuda.device(dev):
-        ws = torch.empty(workspace_bytes(n, K, len(gt_box), len(dt_box)), dtype=torch.uint8, device=dev)
+        need = workspace_bytes(n, K, len(gt_box), len(dt_box))
+        if workspace is None:
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        else:
+            if workspace.device != dev or workspace.numel() < need:
+                raise ValueError(f"workspace must be on {dev} and hold at least {need} bytes")
+            ws = workspace
         precision = torch.empty((len(IOU_THRS), len(REC_THRS), K, len(AREA_RNG)), dtype=torch.float64, device=dev)
         recall = torch.empty((len(IOU_THRS), K, len(AREA_RNG)), dtype=torch.float64, device=dev)
         _lib.check(lib.dagr_evaluate_bbox(_lib.ptr(gt_box), _lib.ptr(gt_lab), _lib.ptr(gt_off), _lib.ptr(dt_box), _lib.ptr(dt_score),

@@ -516,6 +516,13 @@ int dagr_sample_features_planes_bf16(const void *img /*bf16 [nplanes,h,w,C]*/, i
  * a14  asy_tools (src/dagr/asynchronous/asy_tools/main.cu:239-244), same argument meaning.
  * masked_isdiff writes kept[i] = idx[i] or -1 (the reference clobbers `indices` in place, :30-37);
  * compaction is the caller's job exactly as in main.cu:124.
+ * The outputs equal the reference kernels' bit for bit as nvcc builds them (FMA contraction on):
+ * masked_lin accumulates with fmaf in channel order and adds the bias last; masked_inplace_bn ends
+ * in one fmaf(d, weight, bias); masked_isdiff tests |a - b| > fmaf(rtol, b, atol) with b signed.
+ * Precondition: the K indices are distinct.  With duplicates, masked_lin with add = 1 (and every
+ * op writing the same row twice) races, as the reference kernels do.
+ * DAGR_E_ARG before any launch: K < 0, Cin / Cout / C < 1, or a NULL pointer when K > 0 (only
+ * masked_lin's bias may be NULL).
  * ------------------------------------------------------------------------------------------- */
 int dagr_masked_lin(const int64_t *idx, int64_t K, const float *x_in, float *x_out, const float *weight,
                     const float *bias /*or NULL*/, int Cin, int Cout, int add, void *stream);

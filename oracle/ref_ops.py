@@ -484,9 +484,11 @@ def masked_isdiff(indices, x_old, x_new, atol, rtol):
 
 
 def masked_inplace_bn(indices, x, x_out, mean, var, weight, bias, eps):
-    """main.cu:43-67."""
+    """main.cu:43-67.  nvcc contracts `* weight + bias` there to one fma.rn, so d * w + b is rounded once: the product of
+    two float32 values is exact in float64, and the float64 sum is cast to float32."""
     r = indices.long()
-    x_out[r] = (x[r] - mean) / torch.sqrt(var + eps) * weight + bias
+    d = (x[r] - mean) / torch.sqrt(var + eps)
+    x_out[r] = (d.double() * weight.double() + bias.double()).to(x_out.dtype)
     return x_out
 
 

@@ -131,3 +131,61 @@ def test_eval_symbols_exported_declared_and_sized():
     for bad in ((0, 2, 1, 1), (10, 0, 1, 1), (10, 70000, 1, 1), (10, 2, 1, -1)):
         with pytest.raises(RuntimeError):
             evaluation.workspace_bytes(*bad)
+
+
+# ---- the case builders of tests/eval_cases.py (the sets tests/test_eval_kernels_gpu.py runs) -----------------------------
+def test_eval_case_builders_reach_the_kernel_switches():
+    from tests import eval_cases as E
+    for n in (2047, 2048, 2049, 4097):
+        gts, dts, K = E.CASES[f"kept_{n}"]()
+        assert E.kept_total(gts, dts, K) == n
+        assert sum(len(d["boxes"]) for d in dts) > n                      # some detections are dropped
+    gts, dts, K = E.CASES["equal_scores_many_tiles"]()
+    assert E.kept_total(gts, dts, K) > 5 * E.RS_TILE and torch.cat([d["scores"] for d in dts]).unique().tolist() == [0.5]
+    for K in (255, 256, 257, 300):
+        gts, dts, k = E.CASES[f"radix_k{K}"]()
+        labels = torch.cat([d["labels"] for d in dts])
+        assert k == K and int(labels.max()) == K - 1 and (K <= 256 or int(labels.min()) >= 256)
+    for name, pair in (("radix_k257_bit8", (0, 256)), ("radix_k300_bit8", (43, 299))):
+        counts = E.class_counts(*E.CASES[name]())
+        assert counts[pair[0]] > 0 and counts[pair[1]] > 0
+    for ng, nk in ((32, 25), (32, 26), (33, 10), (8, 100), (9, 89)):
+        gts, dts, _ = E.CASES[f"match_ng{ng}_nk{nk}"]()
+        assert int((gts[0]["labels"] == 0).sum()) == ng and E.class_counts(gts, dts, 2)[0] == nk
+    fast = {(ng, nk): ng <= 32 and ng * nk <= E.EV_IOU_CAP for ng, nk in ((32, 25), (32, 26), (33, 10), (8, 100), (9, 89))}
+    assert fast == {(32, 25): True, (32, 26): False, (33, 10): False, (8, 100): True, (9, 89): False}
+    gts, dts, K = E.CASES["rank_ties"]()
+    assert sorted(len(d["boxes"]) for d in dts) == [100, 101, 102, 130, 140]
+    for d in dts:
+        s = np.sort(d["scores"].numpy())[::-1]
+        if len(s) > 100:
+            assert s[99] == s[100] or s[100] == s[101]                        # a tie straddles the cut at 100
+    counts = E.class_counts(*E.CASES["acc_tiles"]())
+    assert counts.tolist()[:4] == [E.AC_TILE - 1, E.AC_TILE, E.AC_TILE + 1, 2 * E.AC_TILE + 5]
+    assert counts[4] == 0 and counts[5] == 30 and counts[6] == 0
+    gts, _, _ = E.CASES["acc_tiles"]()
+    glab = torch.cat([g["labels"] for g in gts])
+    assert int((glab == 4).sum()) > 0 and int((glab == 5).sum()) == 0 and int((glab == 6).sum()) == 0
+    gts, dts, _ = E.CASES["slow_path_thresholds"]()
+    assert len(gts[0]["boxes"]) > 32
+
+
+def test_eval_case_score_keys_and_oracle_order():
+    from tests import eval_cases as E
+    gts, dts, K = E.score_keys()
+    s = torch.cat([d["scores"] for d in dts]).numpy()
+    bits = s.view(np.uint32)
+    assert np.isnan(s).any() and np.isposinf(s).any() and np.isneginf(s).any() and (s < 0).any()
+    assert (bits == 0x80000000).any() and (bits == 0).any()                # -0.0 and +0.0
+    assert ((bits & 0x7F800000) == 0).sum() > (bits & 0x7FFFFFFF == 0).sum()   # denormals
+    # numpy's order, which the device's score key restates: -0.0 ties +0.0, NaN last
+    assert list(ref_coco._order([-0.0, 0.0, np.nan, 1.0, np.inf])) == [4, 3, 0, 1, 2]
+    ev = ref_coco.evaluate_lists(gts, dts, K)
+    assert ev is not None and ev.stats[0] > 0
+
+
+def test_eval_case_wide_scan_passes_one_chunk():
+    from tests import eval_cases as E
+    gts, dts, K = E.wide_scan()
+    assert len(gts) * K > E.SCAN_CHUNK and all(len(g["boxes"]) == 1 for g in gts)
+    assert len(set(torch.cat([d["labels"] for d in dts]).tolist())) == K
