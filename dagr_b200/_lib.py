@@ -83,6 +83,8 @@ _SIGS = {
     "dagr_downsample_events": (C.c_int, [p, p, p, i64, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, p, p, p, p, p, p]),
     "dagr_compact_events": (C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, p, p, p, p, p, p, p, p, p]),
     "dagr_ingest_events": (C.c_int, [p, p, p, p, i64, C.c_int, C.c_int, C.c_int, C.c_int, i64, C.c_int, p, p, p, p, p, p, p, p, p]),
+    "dagr_window_bounds": (C.c_int, [p, i64, p, p, i64, p, p, p]),
+    "dagr_window_gather": (C.c_int, [p, p, p, p, i64, p, p, C.c_int, i64, C.c_int, i64, p, p, p, p, p]),
     "dagr_stream_ingest": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int, p]),
     "dagr_frame_preprocess": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, p]),
     "dagr_denormalize_pos": (C.c_int, [p, i64, C.c_int, C.c_int, C.c_int, p, p]),

@@ -309,6 +309,107 @@ extern "C" int dagr_stream_ingest(const int32_t *raw_stage, int streams, int max
 }
 
 // ------------------------------------------------------------------------------------------------
+// windows of one recording (dagr_b200.sequence): the live-window rule of the rings applied to a time-sorted recording,
+// then a block of G windows gathered as the G samples of one batched forward.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int lower_bound_i64(const int64_t *__restrict__ t, int n, long long v)
+{
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (int)(((unsigned)lo + (unsigned)hi) >> 1);
+        if (__ldg(t + mid) < v) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void k_window_bounds(const int64_t *__restrict__ t, int n, const int64_t *__restrict__ t_begin,
+                                const int64_t *__restrict__ t_end, int64_t Q, int32_t *__restrict__ begin, int32_t *__restrict__ end)
+{
+    const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= Q) return;
+    begin[q] = lower_bound_i64(t, n, (long long)t_begin[q]);
+    end[q] = lower_bound_i64(t, n, (long long)t_end[q]);
+}
+
+extern "C" int dagr_window_bounds(const int64_t *t, int64_t N, const int64_t *t_begin, const int64_t *t_end, int64_t Q,
+                                  int32_t *begin, int32_t *end, void *stream)
+{
+    DAGR_CHECK_ARG(N == 0 || t, "null t (it may be NULL only when N = 0)");
+    DAGR_CHECK_ARG(Q == 0 || (t_begin && t_end && begin && end), "null argument (the Q-long rows may be NULL only when Q = 0)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N must be in [0, 2^31)");
+    DAGR_CHECK_ARG(Q >= 0 && Q < (1ll << 31), "Q must be in [0, 2^31)");
+    if (Q == 0) return DAGR_OK;
+    k_window_bounds<<<dagr_div_up(Q, 256), 256, 0, (cudaStream_t)stream>>>(t, (int)N, t_begin, t_end, Q, begin, end);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+// One CTA per WG_ROWS consecutive output rows.  Every CTA scans the G window sizes itself (G <= 255: one value per thread;
+// two int block scans of the high and low bits give the exact 64-bit offsets of any begin / end), then each thread finds
+// the window of its row by a binary search over the offsets in shared memory and copies one event: consecutive threads
+// read consecutive events of one window and write consecutive rows, and no two CTAs write the same row, so there are no
+// atomics.
+#define WG_THREADS 256
+#define WG_ROWS (WG_THREADS * 4)
+
+__global__ void __launch_bounds__(WG_THREADS) k_window_gather(const uint16_t *__restrict__ x, const uint16_t *__restrict__ y,
+                                                               const int64_t *__restrict__ t, const int8_t *__restrict__ p,
+                                                               const int32_t *__restrict__ begin, const int32_t *__restrict__ end,
+                                                               int G, long long t_base, int p_is_01, int total,
+                                                               int32_t *__restrict__ batch_o, int32_t *__restrict__ pos_o,
+                                                               float *__restrict__ feat_o, int64_t *__restrict__ offsets)
+{
+    __shared__ long long off[WG_THREADS];
+    __shared__ int src[WG_THREADS];
+    __shared__ int sm[32];
+    __shared__ int tot_hi, tot_lo;
+    const int tid = threadIdx.x;
+    int b = 0, n = 0;
+    if (tid < G) { b = begin[tid]; n = max(end[tid] - b, 0); }
+    const int o_hi = block_exclusive_scan(n >> 12, &tot_hi, sm);         // <= 2^19 per window: no int overflow
+    const int o_lo = block_exclusive_scan(n & 4095, &tot_lo, sm);
+    off[tid] = (long long)o_hi * 4096 + o_lo;
+    src[tid] = b;
+    __syncthreads();
+    const long long tot = (long long)tot_hi * 4096 + tot_lo;
+    if (blockIdx.x == 0 && tid <= G) offsets[tid] = tid < G ? off[tid] : tot;
+    const int rows = (int)min(tot, (long long)total);                    // the caller's rows bound every write
+    for (int r = blockIdx.x * WG_ROWS + tid; r < min(rows, (int)(blockIdx.x + 1) * WG_ROWS); r += WG_THREADS) {
+        int lo = 0, hi = G - 1;                                          // the last window w with off[w] <= r
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (off[mid] <= r) lo = mid;
+            else hi = mid - 1;
+        }
+        const int64_t i = (int64_t)src[lo] + (r - off[lo]);
+        batch_o[r] = lo;
+        pos_o[3 * (int64_t)r] = (int)__ldg(x + i);
+        pos_o[3 * (int64_t)r + 1] = (int)__ldg(y + i);
+        pos_o[3 * (int64_t)r + 2] = (int)((long long)__ldg(t + i) - t_base);
+        const int pv = (int)__ldg(p + i);
+        feat_o[r] = (float)(p_is_01 ? 2 * pv - 1 : pv);
+    }
+}
+
+extern "C" int dagr_window_gather(const uint16_t *x, const uint16_t *y, const int64_t *t, const int8_t *p, int64_t N,
+                                  const int32_t *begin, const int32_t *end, int G, int64_t t_base, int p_is_01, int64_t total,
+                                  int32_t *batch_out, int32_t *pos_out, float *feat_out, int64_t *offsets, void *stream)
+{
+    DAGR_CHECK_ARG(begin && end && offsets, "null argument");
+    DAGR_CHECK_ARG(N == 0 || (x && y && t && p), "null argument (the N-long rows may be NULL only when N = 0)");
+    DAGR_CHECK_ARG(total == 0 || (batch_out && pos_out && feat_out), "null argument (the output rows may be NULL only when total = 0)");
+    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N must be in [0, 2^31)");
+    DAGR_CHECK_ARG(G >= 1 && G <= 255, "G must be in [1, 255] (the windows of a block are the samples of one forward)");
+    DAGR_CHECK_ARG(total >= 0 && total < (1ll << 24), "the block total must be in [0, 2^24) (sorted positions are packed in 24 bits)");
+    const int ctas = total > 0 ? dagr_div_up(total, WG_ROWS) : 1;
+    k_window_gather<<<ctas, WG_THREADS, 0, (cudaStream_t)stream>>>(x, y, t, p, begin, end, G, (long long)t_base, p_is_01, (int)total,
+                                                                  batch_out, pos_out, feat_out, offsets);
+    DAGR_CHECK_LAUNCH();
+    return DAGR_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // camera frames (dsec_data.py:149-154): crop to scale * H rows, cv2.resize(INTER_CUBIC) by the integer factor `scale`,
 // HWC -> CHW, in one pass.  At an integer factor the cubic is integer arithmetic (oracle/ref_frame.py): the source
 // coordinate of output pixel d is (d + 0.5) * s - 0.5.  Odd s: fraction 0, the output is source pixel s * d + (s - 1) / 2.

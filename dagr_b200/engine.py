@@ -162,7 +162,7 @@ class Engine:
         self._out_slot = {}
 
     # kernels enqueued by each C-ABI call (see csrc/*.cu)
-    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_stream_ingest=1, dagr_l1_build=2, dagr_l1_build_tc=2, dagr_graph_export=5, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
+    _NKERNELS = dict(dagr_graph_sort=6, dagr_graph_sort_ring=6, dagr_stream_push=2, dagr_graph_sort_rings=6, dagr_stream_push_multi=2, dagr_stream_ingest=1, dagr_window_gather=1, dagr_l1_build=2, dagr_l1_build_tc=2, dagr_graph_export=5, dagr_l1_conv_b_pool_voxel_tc=2, dagr_l1_x0_image=1, dagr_l1_x0_image_live=1, dagr_xa_permute=1, dagr_l1_conv_a_image_tc=2, dagr_voxel_sample_max=1,
                      dagr_l1_conv_a_image_inc=2, dagr_voxel_sample_max_inc=1,
                      dagr_l1_x0_image_planes=1, dagr_voxel_sample_max_planes=1, dagr_sample_features_planes=1, dagr_head_finish_planes=1,
                      dagr_grid_cat_pos=1, dagr_grid_conv=1, dagr_grid_linear_bn=1, dagr_grid_pool=1,
@@ -544,10 +544,11 @@ class Engine:
         depends on a host-side count and the whole call can sit inside one captured CUDA graph (dagr_b200.streaming).
         ring_streams = S: `ring` is the int32[S+1][8] block of S rings of N / S slots each (dagr_graph_sort_rings), stream s
         being sample s of B = S.
-        image_planes = (plane table int32 on the device, stride), with ring_streams and image fusion: image_feats / image_outs
-        are plane arrays [P, C, h, w] and sample b reads plane table[b * stride] alone, sampled as a batch of one (the
-        *_planes kernels), so each stream gets the bits of a B = 1 forward with its own frame.  The table may be device
-        data written inside the step (the stage header, dagr_b200.streaming.FusionMultiStreamDetector)."""
+        image_planes = (plane table int32 on the device, stride), with image fusion: image_feats / image_outs are plane arrays
+        [P, C, h, w] and sample b reads plane table[b * stride] alone, sampled as a batch of one (the *_planes kernels), so
+        each sample gets the bits of a B = 1 forward with its own frame.  The table may be device data written inside the
+        step (the stage header, dagr_b200.streaming.FusionMultiStreamDetector).  A plain batch (ring None) takes it too: the
+        windows of one recording, each with its own frame (dagr_b200.sequence)."""
         for n, t in (("batch", batch_i32), ("pos", pos_i32), ("x", feat)):
             _lib.require_cuda(t, n)
         dev = pos_i32.device
@@ -556,9 +557,8 @@ class Engine:
             raise ValueError(f"ring_streams={ring_streams} needs a ring control block, B == ring_streams and N a multiple of it "
                              f"(B={B}, N={N})")
         if image_planes is not None:
-            if ring_streams is None or image_feats is None or image_outs is None:
-                raise ValueError("image_planes selects per-stream frames of a multi-ring step: it needs ring_streams, image_feats "
-                                 "and image_outs")
+            if image_feats is None or image_outs is None:
+                raise ValueError("image_planes selects a frame per sample: it needs image_feats and image_outs")
             if self.keep_node_features:
                 raise ValueError("keep_node_features: the dense head maps (dagr_grid_to_dense) have no plane mode")
             plane_tab, plane_stride = image_planes

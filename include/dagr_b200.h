@@ -568,6 +568,31 @@ int dagr_ingest_events(const uint16_t *x, const uint16_t *y, const int64_t *t, c
                        float *feat_out, int32_t *n_out, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Windows of one recording (dagr_b200.sequence): many time windows of a time-sorted recording as the samples of batched
+ * forwards.
+ *
+ *   dagr_window_bounds : t i64[N] sorted (non-decreasing); window q = [t_begin[q], t_end[q]) (i64[Q] each, on the device)
+ *       -> begin[q] = lower_bound(t, t_begin[q]), end[q] = lower_bound(t, t_end[q]) (i32[Q]), one thread per window.  This
+ *       is the live-window rule of the streaming rings: an event with t == t_end - window_us is live, one with t == t_end is
+ *       not.  Returns DAGR_E_ARG with a message before anything is launched on a null pointer (t may be NULL when N = 0,
+ *       the Q-long rows when Q = 0), N outside [0, 2^31) or Q outside [0, 2^31).
+ *   dagr_window_gather : the G windows {begin[g], end[g]} (i32[G] on the device, G in [1, 255]; end < begin counts as
+ *       empty) of the recording x, y u16[N], t i64[N], p i8[N] -> the inputs of dagr_graph_sort, window g's events in
+ *       recording order at rows [offsets[g], offsets[g + 1]): batch i32 = g, pos i32[., 3] = (x, y, t - t_base) (t - t_base
+ *       is kept in its low 32 bits), feat f32 = 2p - 1 when p_is_01, else p as is.  offsets i64[G + 1] (out) = the exclusive
+ *       scan of the window sizes, offsets[G] their total.  Windows may overlap, repeat or be empty.  `total` = the rows the
+ *       outputs hold (the block total the caller read back): no row at or past it is written.  One CTA per 1024 rows, no
+ *       atomics.  Returns DAGR_E_ARG with a message before anything is launched on a null pointer (the N-long rows may be
+ *       NULL when N = 0, the output rows when total = 0), N outside [0, 2^31), G outside [1, 255] or total outside [0, 2^24)
+ *       (dagr_graph_sort packs sorted positions in 24 bits).
+ * ------------------------------------------------------------------------------------------- */
+int dagr_window_bounds(const int64_t *t, int64_t N, const int64_t *t_begin, const int64_t *t_end, int64_t Q, int32_t *begin,
+                       int32_t *end, void *stream);
+int dagr_window_gather(const uint16_t *x, const uint16_t *y, const int64_t *t, const int8_t *p, int64_t N, const int32_t *begin,
+                       const int32_t *end, int G, int64_t t_base, int p_is_01, int64_t total, int32_t *batch_out, int32_t *pos_out,
+                       float *feat_out, int64_t *offsets, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Streaming ingest: raw sensor chunks of S cameras -> the stage of dagr_stream_push / dagr_stream_push_multi, as one
  * launch of S CTAs whose grid depends on no count (capturable in the streaming step's CUDA graph; no host sync).
  *
