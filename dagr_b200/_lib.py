@@ -147,6 +147,11 @@ _SIGS = {
     "dagr_masked_isdiff": (C.c_int, [p, i64, p, p, C.c_int, f32, f32, p]),
     "dagr_eval_workspace_bytes": (C.c_int, [i64, C.c_int, i64, i64, C.POINTER(i64)]),
     "dagr_evaluate_bbox": (C.c_int, [p, p, p, p, p, p, p, i64, C.c_int, i64, i64, C.POINTER(EvalParams), p, i64, p, p, p]),
+    "dagr_interframe_targets_workspace_bytes": (C.c_int, [i64, i64, C.POINTER(i64)]),
+    "dagr_interframe_targets": (C.c_int, [p, p, p, p, p, i64, i64, p, p, p, i64, C.c_int, C.c_int, C.c_int, f32, f32, i64, p, i64,
+                                          p, p, p, p]),
+    "dagr_eval_pack_workspace_bytes": (C.c_int, [i64, C.POINTER(i64)]),
+    "dagr_eval_pack_detections": (C.c_int, [p, p, i64, C.c_int, p, p, C.c_int, p, i64, p, p, p, p, p]),
 }
 
 EXPORTS = tuple(_SIGS.keys())

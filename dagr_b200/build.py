@@ -10,7 +10,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libdagr_b200.so"
-SOURCES = ["capi.cu", "graph.cu", "build_l1.cu", "conv_l1.cu", "image_l1.cu", "coarse.cu", "masked.cu", "ingest.cu", "evaluate.cu"]
+SOURCES = ["capi.cu", "graph.cu", "build_l1.cu", "conv_l1.cu", "image_l1.cu", "coarse.cu", "masked.cu", "ingest.cu", "evaluate.cu", "labels.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17"] + GENCODE + ["-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]

@@ -666,6 +666,47 @@ int dagr_evaluate_bbox(const float *gt_box, const int64_t *gt_label, const int64
                        int64_t n_gt, int64_t n_det, const dagr_eval_params_t *params_host, void *workspace,
                        int64_t workspace_bytes, double *precision, double *recall, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Interframe evaluation (the reference's scripts/run_test_interframe.py): the ground truth of every window and the
+ * detections of every window in the layout of dagr_evaluate_bbox, with one category block per group (offset), so that
+ * one evaluate call over K' = n_groups * K categories equals one call per group.
+ *
+ * dagr_interframe_targets: window w = (pair win_pair[w], time win_t[w], group win_group[w]).
+ *   box0 / box1 f32[n_labels][4] xywh (16-byte aligned): the preprocessed labels of the pair's first and second frame,
+ *         paired row by row and sorted by track id; pair p owns rows [pair_off[p], pair_off[p+1]); cls i64[n_labels] the
+ *         class index (from the first frame); pair_t i64[n_pairs][2] = (t0, t1), t0 < t1.
+ *   Per window and row, as dsec_data.interpolate_tracks under NumPy 1 promotion: r = (t - t0) / (t1 - t0) in double, r and
+ *   1 - r rounded to float, v = v0 * (1 - r) + v1 * r in float for x, y, w, h; then augment.Crop([0, 0], [1, 1]) (both
+ *   corners clamped to [0, width-1] x [0, height-1]), filter_small_bboxes (float sqrt(h*h + w*w) > min_bbox_diag,
+ *   w > min_bbox_height, h > min_bbox_height) and x2 = x + w, y2 = y + h.  Every operation is correctly rounded.
+ *   Out: the kept rows of every window in window order, each window's rows in table order: gt_box f32[n_rows][4] xyxy
+ *   (16-byte aligned), gt_label i64[n_rows] = win_group * K + cls, gt_off i64[n_windows + 1].
+ *   n_rows: the capacity, the sum over the windows of their pairs' row counts (rows past it are not evaluated).
+ *   win_pair and pair_off are device data the launch cannot check: a pair index is clamped to [0, n_pairs) and a row
+ *   index to [0, n_labels).
+ *   workspace: dagr_interframe_targets_workspace_bytes bytes, 256-byte aligned, no initialisation.
+ *   Limits (DAGR_E_ARG before anything is launched): counts >= 0, K >= 1, n_windows and n_rows < 2^31 - 1,
+ *   n_labels < 2^31, n_pairs >= 1 when n_windows > 0, 1 <= width, height <= 2^24, no null pointer where a count is > 0.
+ *
+ * dagr_eval_pack_detections: det f32[n_windows][A][6] (x1, y1, x2, y2, score, label) and ndet i32[n_windows] as
+ *   Engine.postprocess / SequenceDetector return them.  A window with ground truth (gt_off[w+1] > gt_off[w]) keeps its
+ *   first min(max(ndet, 0), A) detections, one without keeps none (an image without GT contributes nothing).
+ *   Out: dt_box f32[n_windows * A][4] (16-byte aligned), dt_score f32[.], dt_label i64[.] = win_group * K + (long)label,
+ *   or -1 (no category) for a label outside [0, K); dt_off i64[n_windows + 1].
+ *   workspace: dagr_eval_pack_workspace_bytes bytes, 256-byte aligned, no initialisation.
+ *   Limits (DAGR_E_ARG): n_windows >= 0, A >= 1, K >= 1, n_windows * A < 2^31 - 1, no null pointer when n_windows > 0.
+ * ------------------------------------------------------------------------------------------- */
+int dagr_interframe_targets_workspace_bytes(int64_t n_windows, int64_t n_rows, int64_t *bytes);
+int dagr_interframe_targets(const float *box0, const float *box1, const int64_t *cls, const int64_t *pair_off,
+                            const int64_t *pair_t, int64_t n_pairs, int64_t n_labels, const int64_t *win_pair,
+                            const int64_t *win_t, const int32_t *win_group, int64_t n_windows, int K, int width, int height,
+                            float min_bbox_height, float min_bbox_diag, int64_t n_rows, void *workspace,
+                            int64_t workspace_bytes, float *gt_box, int64_t *gt_label, int64_t *gt_off, void *stream);
+int dagr_eval_pack_workspace_bytes(int64_t n_windows, int64_t *bytes);
+int dagr_eval_pack_detections(const float *det, const int32_t *ndet, int64_t n_windows, int A, const int32_t *win_group,
+                              const int64_t *gt_off, int K, void *workspace, int64_t workspace_bytes, float *dt_box,
+                              float *dt_score, int64_t *dt_label, int64_t *dt_off, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
