@@ -97,7 +97,8 @@ class AsyncDAGR:
         self.B = self.W = self.H = None
         self._image = None                  # the frame: the caller's tensor (identity test) and a copy (content test)
         self._image_copy = None
-        self._feats = self._outs = None     # the frame's feature maps / CNN head maps, copied out of the branch's graph buffers
+        self._frames = self._frame_shape = None   # FrameStore(1) of the frame's branch outputs, and the image shape it holds
+        self._feats = self._outs = None     # its frame(0)
         self.frames = 0                     # frames run through the trunk since construction
 
     def reset(self):
@@ -108,28 +109,14 @@ class AsyncDAGR:
         self._image = self._image_copy = None
 
     def _new_frame(self, image):
-        """run the frame through the model's own ImageBranch and copy its outputs into buffers of this wrapper: the branch's
-        outputs are static graph buffers that the next model(data) overwrites."""
-        from .model.image_branch import ImageBranch
-        m = self.model
-        if m._image_branch is None:
-            m._image_branch = ImageBranch(m)
-        br = m._image_branch
-        cur = torch.cuda.current_stream(image.device)
-        feats, outs, (_, ev2) = br.run(image, use_graph=m.image_graph, precision=self.image_precision)
-        cur.wait_event(ev2)                                          # the copy waits for the whole branch
-        if (self._feats is None or [tuple(f.shape) for f in feats] != [tuple(f.shape) for f in self._feats]
-                or {k: [tuple(t.shape) for t in v] for k, v in outs.items()} != {k: [tuple(t.shape) for t in v] for k, v in self._outs.items()}):
-            self._feats = [torch.empty_like(f) for f in feats]
-            self._outs = {k: [torch.empty_like(t) for t in v] for k, v in outs.items()}
-        for d, s in zip(self._feats, feats):
-            d.copy_(s)
-        for k, v in outs.items():
-            for d, s in zip(self._outs[k], v):
-                d.copy_(s)
-        copied = torch.cuda.Event()
-        copied.record(cur)
-        br.stream.wait_event(copied)                                 # the branch's buffers outlive the copy
+        """run the frame through the model's own ImageBranch into this wrapper's frame store: the branch's outputs are static
+        graph buffers that the next model(data) overwrites.  The store is re-created when the image's shape, and so the
+        shapes of the branch's outputs, changes."""
+        from .model.image_branch import FrameStore, run_frame
+        if self._frames is None or self._frame_shape != image.shape:
+            self._frames, self._frame_shape = FrameStore(1), image.shape
+        run_frame(self.model, self._frames, 0, image, self.image_precision)
+        self._feats, self._outs = self._frames.frame(0)
         self._image, self._image_copy = image, image.clone()
         self.frames += 1
 

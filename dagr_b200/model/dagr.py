@@ -11,6 +11,7 @@ import numpy as np
 import torch
 from torch import nn
 
+from .image_branch import branch_of
 from .layers import ConvBlock, SplineConvToDense
 from .net import Net
 from .yolox_compat import YOLOX, YOLOXHead
@@ -242,11 +243,8 @@ class DAGR(YOLOX):
         if self.backbone.use_image:
             # dense image trunk + CNN head stay torch/cuDNN (tensor cores allowed here only), net.py:110, dagr.py:205-206;
             # they run on a side stream, concurrently with the sort + radius-graph kernels below
-            if self._image_branch is None:
-                from .image_branch import ImageBranch
-                self._image_branch = ImageBranch(self)
-            image_feats, image_outs, image_event = self._image_branch.run(x.image, use_graph=self.image_graph,
-                                                                          precision=self.image_precision)
+            image_feats, image_outs, image_event = branch_of(self).run(x.image, use_graph=self.image_graph,
+                                                                       precision=self.image_precision)
             self.last_image_outs, self.last_image_feats = image_outs, image_feats
             if self.head.no_events:
                 # --no_events (dagr.py:284): detections from the image branch alone -- collect_outputs + decode_outputs on

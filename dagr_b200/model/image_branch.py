@@ -145,3 +145,64 @@ class ImageBranch:
             for t in v:
                 t.record_stream(cur)
         return feats, outs, (ev1, ev2)
+
+
+def branch_of(model) -> ImageBranch:
+    """the model's ImageBranch, created on first use."""
+    if model._image_branch is None:
+        model._image_branch = ImageBranch(model)
+    return model._image_branch
+
+
+class FrameStore:
+    """n frames of the image branch's outputs, in the taps' own format: fp32 NCHW feature maps, or bf16 channels_last ones
+    (the engine's bf16 sampling kernels read NHWC); the CNN head maps are fp32 contiguous.  The arrays are planes [n * b,
+    ...], allocated by the first put(), where b is the batch of the branch's output; frame k is rows [k * b, (k + 1) * b).
+    A slice along dim 0 keeps the channels_last layout, so a frame is what the engine's non-plane kernels take, and the
+    whole arrays are what its *_planes kernels take."""
+
+    def __init__(self, n: int):
+        self.n = int(n)
+        self.b = None
+        self.feats = self.outs = None
+
+    def put(self, k: int, feats, outs):
+        """copy one frame of branch outputs into frame k, on the current stream."""
+        if self.feats is None:
+            self.b = b = int(feats[0].shape[0])
+            fmt = torch.channels_last if feats[0].dtype == torch.bfloat16 else torch.contiguous_format
+            self.feats = [torch.empty((self.n * b,) + tuple(f.shape[1:]), dtype=f.dtype, device=f.device, memory_format=fmt)
+                          for f in feats]
+            self.outs = {key: [torch.empty((self.n * b,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device) for t in v]
+                         for key, v in outs.items()}
+        dst_f, dst_o = self.frame(k)
+        for d, s in zip(dst_f, feats):
+            d.copy_(s)
+        for key, v in outs.items():
+            for d, s in zip(dst_o[key], v):
+                d.copy_(s)
+
+    def frame(self, k: int):
+        """-> (image_feats, image_outs) views of frame k."""
+        a, b = k * self.b, (k + 1) * self.b
+        return [f[a:b] for f in self.feats], {key: [t[a:b] for t in v] for key, v in self.outs.items()}
+
+
+def run_frame(model, store: FrameStore, k: int, image, precision: str, after=None, trunk_done=None):
+    """run `image` through the model's ImageBranch and copy its outputs into frame k of `store`, on the current stream.
+    The copy waits for the branch and, when given, for the event `after` (the last reader of frame k); the branch's next
+    run, which overwrites its outputs, waits for the copy.  `trunk_done`, when given, is recorded once the branch has
+    finished, before the copy.  Returns the event of the finished copy."""
+    br = branch_of(model)
+    cur = torch.cuda.current_stream(image.device)
+    feats, outs, (_, ev2) = br.run(image, use_graph=model.image_graph, precision=precision)
+    cur.wait_event(ev2)
+    if trunk_done is not None:
+        trunk_done.record(cur)
+    if after is not None:
+        cur.wait_event(after)
+    store.put(k, feats, outs)
+    copied = torch.cuda.Event()
+    copied.record(cur)
+    br.stream.wait_event(copied)
+    return copied

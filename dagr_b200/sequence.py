@@ -118,7 +118,7 @@ class SequenceDetector:
         self.dev = torch.device(device) if device is not None else next(model.parameters()).device
         self._check_sensor(sensor, p_is_01)
         self._frame_lut = None
-        self._cam = _CameraFrames(self, None)          # frame checks and the u8 -> f32 conversion of the fusion detectors
+        self._cam = _CameraFrames(self, 0)             # frame checks and the u8 -> f32 conversion of the fusion detectors
         self.last = None
 
     def _check_sensor(self, sensor, p_is_01):
@@ -214,7 +214,7 @@ class SequenceDetector:
     def _planes(self, fi, checked, blocks, G):
         """every frame the call uses through the model's ImageBranch at B = 1, once, into plane arrays; -> (image_feats,
         image_outs, plane table i32[blocks, G] on the device)."""
-        from .model.image_branch import ImageBranch
+        from .model.image_branch import FrameStore, branch_of, run_frame
         m, dev = self.model, self.dev
         used = np.array(sorted(checked), dtype=np.int64)
         tab = np.zeros((len(blocks), G), dtype=np.int32)
@@ -222,28 +222,12 @@ class SequenceDetector:
             tab[i, :q1 - q0] = np.searchsorted(used, fi[q0:q1])
         if self.raw_frames and self._frame_lut is None:
             self._frame_lut = ingest.frame_lut(dev)
-        if m._image_branch is None:
-            m._image_branch = ImageBranch(m)
-        br = m._image_branch
-        cur = torch.cuda.current_stream(dev)
-        pf = po = None
+        store = FrameStore(len(used))
         for k, f in enumerate(used.tolist()):
             img = self._cam.to_float(checked[f].to(dev))
-            feats, outs, (_, ev2) = br.run(img, use_graph=m.image_graph, precision=self.image_precision)
-            img.record_stream(br.stream)
-            cur.wait_event(ev2)
-            if pf is None:
-                n = len(used)
-                # bf16 taps are NHWC (channels_last), and so are their plane arrays, as in FusionMultiStreamDetector
-                fmt = torch.channels_last if feats[0].dtype == torch.bfloat16 else torch.contiguous_format
-                pf = [torch.empty((n,) + tuple(a.shape[1:]), dtype=a.dtype, device=dev, memory_format=fmt) for a in feats]
-                po = {key: [torch.empty((n,) + tuple(a.shape[1:]), dtype=a.dtype, device=dev) for a in v] for key, v in outs.items()}
-            for d, s in zip(pf, feats):
-                d[k:k + 1].copy_(s)
-            for key, v in outs.items():
-                for d, s in zip(po[key], v):
-                    d[k:k + 1].copy_(s)
-        return pf, po, torch.from_numpy(tab).to(dev)
+            run_frame(m, store, k, img, self.image_precision)
+            img.record_stream(branch_of(m).stream)
+        return store.feats, store.outs, torch.from_numpy(tab).to(dev)
 
     def _run_blocks(self, ev, begin, end, blocks, totals, G, planes):
         """the block loop: gather, forward, NMS and the copy of each block's detections, all enqueued without a host sync.

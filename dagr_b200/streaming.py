@@ -429,15 +429,15 @@ class _CameraFrames:
 
     set() runs a frame through the model's own ImageBranch (ResNet trunk + CNN head, the captured graphs that model(data)
     replays) on the detector's frame stream and copies its five feature maps and CNN head maps into the slot the steps do
-    not use; `slot_dst(slot, feats, outs)` names the destination tensors of a slot (allocating them on first use).  Two
-    hazards are ordered on the device: the copy into a slot waits for the last step that read that slot, and the branch's
-    static output buffers are overwritten (by the next frame or a model(data) call) only after the copy out of them.
+    not use: slot j of camera s is frame 2s + j of the detector's FrameStore `_frames`.  Two hazards are ordered on the
+    device (run_frame): the copy into a slot waits for the last step that read that slot, and the branch's static output
+    buffers are overwritten (by the next frame or a model(data) call) only after the copy out of them.
 
     With the detector's raw_frames a frame is the camera's u8 [sensor_h, sensor_w, 3]; the pinned stage is sized for it,
     and dagr_frame_preprocess turns it into the trunk's f32 [1, 3, H, W] where `.float() / 255.0` runs otherwise."""
 
-    def __init__(self, det, slot_dst):
-        self.det, self.slot_dst = det, slot_dst
+    def __init__(self, det, s):
+        self.det, self.s = det, s
         self.reader = [None, None]            # per slot: done-event of the last step that read it
         self.cur = None                       # slot of the newest usable frame
         self.cur_frame = None                 # (id, t_us) of that frame
@@ -484,15 +484,12 @@ class _CameraFrames:
             self.promote()
 
     def set(self, image, t_us):
-        from .model.image_branch import ImageBranch
+        from .model.image_branch import branch_of, run_frame
         det = self.det
         img = self.check(image)
         self.sync()
         slot = 0 if self.cur is None else 1 - self.cur
-        m, fs = det.model, det.frame_stream
-        if m._image_branch is None:
-            m._image_branch = ImageBranch(m)
-        br = m._image_branch
+        fs = det.frame_stream
         cur = torch.cuda.current_stream(det.dev)
         if img.is_cuda:
             x = self.to_float(img.to(det.dev))                         # on the caller's stream, ordered with its writes
@@ -509,22 +506,10 @@ class _CameraFrames:
                 self.h2d.record(fs)
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record(fs)
-            feats, outs, (_, ev2) = br.run(x, use_graph=m.image_graph, precision=det.image_precision)
+            ready = run_frame(det.model, det._frames, 2 * self.s + slot, x, det.image_precision, after=self.reader[slot],
+                              trunk_done=t1)
             x.record_stream(fs)
-            x.record_stream(br.stream)
-            fs.wait_event(ev2)
-            t1.record(fs)
-            if self.reader[slot] is not None:
-                fs.wait_event(self.reader[slot])                      # the last step that read this slot is done
-            dst_f, dst_o = self.slot_dst(slot, feats, outs)
-            for d, s in zip(dst_f, feats):
-                d.copy_(s)
-            for k, v in outs.items():
-                for d, s in zip(dst_o[k], v):
-                    d.copy_(s)
-            ready = torch.cuda.Event()
-            ready.record(fs)
-        br.stream.wait_event(ready)                                   # the branch's static outputs outlive the copy
+            x.record_stream(branch_of(det.model).stream)
         fid = self.nframes
         self.nframes += 1
         self.pending = dict(slot=slot, id=fid, t_us=t_us, ready=ready, trunk=(t0, t1))
@@ -555,15 +540,17 @@ class _FusionDetector:
     non-blocking query; a camera's first frame is waited for on the device), and after it the step reads that frame's slot
     until it is done."""
 
-    def _frame_setup(self, raw_frames, slot_dsts):
+    def _frame_setup(self, raw_frames):
         """after _setup: the frame stream, the image branch precision (read once from the model: a later change of
-        model.image_precision does not reach the detector), with raw_frames the u8 -> f32 table, and one camera per entry of
-        slot_dsts (its _CameraFrames.slot_dst)."""
+        model.image_precision does not reach the detector), with raw_frames the u8 -> f32 table, the frame store of the S
+        cameras' two slots each, and one _CameraFrames per camera."""
+        from .model.image_branch import FrameStore
         self.frame_stream = torch.cuda.Stream(device=self.dev)
         self.image_precision = self.model.image_precision
         self.raw_frames = bool(raw_frames)
         self._frame_lut = ingest.frame_lut(self.dev) if self.raw_frames else None
-        self._cams = [_CameraFrames(self, dst) for dst in slot_dsts]
+        self._frames = FrameStore(2 * self.S)
+        self._cams = [_CameraFrames(self, s) for s in range(self.S)]
 
     def _camera(self, s):
         s = int(s)
@@ -616,14 +603,7 @@ class FusionStreamingDetector(_FusionDetector, StreamingDetector):
         _check_fusion_model(model, "FusionStreamingDetector", "StreamingDetector")
         _check_raw_frames(raw_frames, sensor)
         self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self._slots = None                    # per slot: (image_feats, image_outs) copies of the branch outputs
-        self._frame_setup(raw_frames, [self._slot_dst])
-
-    def _slot_dst(self, slot, feats, outs):
-        if self._slots is None:
-            self._slots = [([torch.empty_like(f) for f in feats], {k: [torch.empty_like(t) for t in v] for k, v in outs.items()})
-                           for _ in range(2)]
-        return self._slots[slot]
+        self._frame_setup(raw_frames)
 
     @property
     def _cam(self):
@@ -655,7 +635,7 @@ class FusionStreamingDetector(_FusionDetector, StreamingDetector):
         return self._cam.cur
 
     def _image_inputs(self):
-        return self._slots[self._cam.cur]
+        return self._frames.frame(self._cam.cur)
 
     @property
     def frame_state(self):
@@ -794,19 +774,7 @@ class FusionMultiStreamDetector(_FusionDetector, MultiStreamDetector):
         _check_fusion_model(model, "FusionMultiStreamDetector", "MultiStreamDetector")
         _check_raw_frames(raw_frames, sensor)
         self._setup(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self._planes = None                   # (image_feats, image_outs) as plane arrays [2S, ...]
-        self._frame_setup(raw_frames, [lambda j, f, o, s=s: self._plane_dst(2 * s + j, f, o) for s in range(self.S)])
-
-    def _plane_dst(self, k, feats, outs):
-        if self._planes is None:
-            n = 2 * self.S
-            # bf16 feature maps are NHWC (channels_last), and so are their plane arrays: [2S, h, w, C] in memory
-            fmt = torch.channels_last if feats[0].dtype == torch.bfloat16 else torch.contiguous_format
-            self._planes = ([torch.empty((n,) + tuple(f.shape[1:]), dtype=f.dtype, device=self.dev, memory_format=fmt) for f in feats],
-                            {key: [torch.empty((n,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev) for t in v]
-                             for key, v in outs.items()})
-        pf, po = self._planes
-        return [f[k:k + 1] for f in pf], {key: [t[k:k + 1] for t in v] for key, v in po.items()}
+        self._frame_setup(raw_frames)
 
     @property
     def _overlapped(self):
@@ -825,7 +793,7 @@ class FusionMultiStreamDetector(_FusionDetector, MultiStreamDetector):
             c.sync()
 
     def _image_inputs(self):
-        return self._planes
+        return self._frames.feats, self._frames.outs
 
     def _image_planes(self):
         return self.stage_d[3:], 4

@@ -185,7 +185,7 @@ def test_bf16_fusion_stream_equals_dense_forward_with_its_frame():
         want = _dense(model, pos, feat, frames[fs["frame"]])
         model.image_precision = "tf32"
         assert _same(out, want), (k, fs, len(out["boxes"]), len(want["boxes"]))
-        slot = det._slots[det._cur][0]
+        slot = det._frames.frame(det._cur)[0]
         assert all(f.dtype == torch.bfloat16 and f.is_contiguous(memory_format=torch.channels_last) for f in slot)
     assert set(det.graphs) == {0, 1} and det.frame_state["frame"] == 2
 
@@ -211,7 +211,7 @@ def test_bf16_fusion_multistream_equals_dense_forward_of_each_camera():
             pos, feat = det.live_window(s)
             want = _dense(model, pos, feat, frames[s][fs["frame"]])
             assert _same(out[s], want), (k, s, fs)
-    pf = det._planes[0]
+    pf = det._frames.feats
     assert all(f.dtype == torch.bfloat16 and f.shape[0] == 2 * S and f.is_contiguous(memory_format=torch.channels_last) for f in pf)
     assert len(det.graphs) == 1
 
@@ -256,7 +256,7 @@ def test_bf16_raw_frames_equal_host_prepared_frames():
         out = det.push(*c, t_end=_rt_end(ev, k))[0]
         want = ref.push(*c, t_end=_rt_end(ev, k))[0]
         assert _same(out, want) and det.frame_state == ref.frame_state, k
-    assert det._slots[det._cur][0][0].dtype == torch.bfloat16
+    assert det._frames.frame(det._cur)[0][0].dtype == torch.bfloat16
 
 
 def test_bf16_no_events_runs():

@@ -84,7 +84,7 @@ def test_fusion_stream_equals_dense_forward_with_its_frame():
         fs = _check(det, model, out, frames)
         assert fs == dict(frame=fid, t_us=FRAMES_AT[fid] * CHUNK, pending=None), (k, fs)
         # the slot holds exactly what the branch computes for this frame (the dense forward above just ran it)
-        feats, outs = det._slots[det._cur]
+        feats, outs = det._frames.frame(det._cur)
         assert all(torch.equal(a, b) for a, b in zip(feats, model.last_image_feats))
         assert all(torch.equal(a, b) for key in outs for a, b in zip(outs[key], model.last_image_outs[key]))
     assert set(det.graphs) == {0, 1} and all(g is not None for g in det.graphs.values())

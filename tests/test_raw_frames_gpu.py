@@ -124,7 +124,7 @@ def test_raw_frames_streaming_detector_equals_host_prepared_frames():
         assert det.frame_state == ref.frame_state, (k, det.frame_state, ref.frame_state)
         assert det.window_state == ref.window_state, k
         if k in (1, 7, 13):
-            assert all(torch.equal(_bits(a), _bits(b)) for a, b in zip(det._slots[det._cur][0], ref._slots[ref._cur][0])), k
+            assert all(torch.equal(_bits(a), _bits(b)) for a, b in zip(det._frames.frame(det._cur)[0], ref._frames.frame(ref._cur)[0])), k
     assert set(det.graphs) == {0, 1} and det.frame_state["frame"] == 5
 
 
@@ -184,4 +184,4 @@ def test_refused_raw_frames_leave_no_trace():
     m = FusionMultiStreamDetector(model, streams=2, raw_frames=True, **kw)
     with pytest.raises(ValueError, match="480, 640, 3"):
         m.set_frame(0, frames[0][:, :, :2])
-    assert m._cams[0].nframes == 0 and m._cams[0].pending is None and m._planes is None
+    assert m._cams[0].nframes == 0 and m._cams[0].pending is None and m._frames.feats is None
