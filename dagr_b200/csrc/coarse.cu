@@ -759,7 +759,7 @@ extern "C" int dagr_postprocess_nms(const float *pred, int B, int A, int nc, flo
 // PLANES: img_in is a plane array [pl.n][C][h][w]; node i samples plane img_plane(pl, bidx[i]) as a batch of one.
 // MT: the map format (common.cuh: float = NCHW, __nv_bfloat16 = NHWC, where the lanes' channels of a tap are one coalesced run).
 // ------------------------------------------------------------------------------------------------
-template <bool PLANES, typename MT = float>
+template <bool PLANES, typename MT>
 __global__ void k_sample_features(const MT *__restrict__ img_in, int Bi_in, int C, int h, int w,
                                   const float *__restrict__ posx, const float *__restrict__ posy,
                                   const int32_t *__restrict__ bidx, int64_t n, float width, float height,
@@ -770,73 +770,50 @@ __global__ void k_sample_features(const MT *__restrict__ img_in, int Bi_in, int 
     if (i >= n) return;
     const int Bi = PLANES ? 1 : Bi_in;
     const MT *__restrict__ img = PLANES ? img_in + (int64_t)img_plane(pl, bidx[i]) * C * h * w : img_in;
-    // normalise exactly as _sample_features does, then unnormalise as grid_sample(align_corners=True)
-    float gx = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posx[i], width)), width - 1.f), 1.f);
-    float gy = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posy[i], height)), height - 1.f), 1.f);
-    const float bs = (float)(Bi > 1 ? Bi : 2);
-    float gz = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, PLANES ? 0.f : (float)bidx[i]), bs - 1.f), 1.f);
-    const float ix = __fmul_rn(__fmul_rn(__fadd_rn(gx, 1.f), 0.5f), (float)(w - 1));
-    const float iy = __fmul_rn(__fmul_rn(__fadd_rn(gy, 1.f), 0.5f), (float)(h - 1));
-    const float iz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.f), 0.5f), (float)(Bi - 1));
-    const float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
-    const int x0 = (int)x0f, y0 = (int)y0f, z0 = (int)z0f;
-    const float tx = ix - x0f, ty = iy - y0f, tz = iz - z0f;
+    const Bilin q = bilin_setup(posx[i], posy[i], PLANES ? 0 : bidx[i], width, height, Bi, h, w);
     for (int c = lane; c < C; c += 32) {
         float acc = 0.f;
-#pragma unroll
-        for (int dz = 0; dz < 2; dz++) {
-            const int z = z0 + dz;
-            const float wz = dz ? tz : 1.f - tz;
-            if (z < 0 || z >= Bi) continue;
-#pragma unroll
-            for (int dy = 0; dy < 2; dy++) {
-                const int y = y0 + dy;
-                const float wy = dy ? ty : 1.f - ty;
-                if (y < 0 || y >= h) continue;
-#pragma unroll
-                for (int dx = 0; dx < 2; dx++) {
-                    const int x = x0 + dx;
-                    const float wx = dx ? tx : 1.f - tx;
-                    if (x < 0 || x >= w) continue;
-                    acc += map_ld(img, C, h, w, z, c, y, x) * (wx * wy * wz);
-                }
-            }
-        }
+        bilin_taps(q, Bi, h, w, [&](const BilinTap &t) { acc += map_ld(img, C, h, w, t.z, c, t.y, t.x) * t.w(); });
         out[i * ldo + c0 + c] = acc;
     }
+}
+
+// The checks and the launch of every sample_features form; the plane forms pass Bi = 1.
+template <bool PLANES, typename MT>
+static int sample_features(const char *who, const void *img, int Bi, const ImgPlanes pl, int C, int h, int w, const float *posx,
+                           const float *posy, const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
+                           void *stream)
+{
+    DAGR_CHECK_ARG_AS(who, img && posx && posy && bidx && out && (pl.plane || !PLANES), "null argument");
+    if (PLANES) {
+        DAGR_CHECK_ARG_AS(who, pl.n >= 1, "nplanes must be >= 1");
+        DAGR_CHECK_ARG_AS(who, pl.stride >= 1, "plane_stride must be >= 1");
+    }
+    DAGR_CHECK_ARG_AS(who, n >= 0 && n < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG_AS(who, Bi >= 1 && C >= 1 && h >= 1 && w >= 1,
+                      PLANES ? "the map must have C, h, w >= 1" : "the map must have Bi, C, h, w >= 1");
+    DAGR_CHECK_ARG_AS(who, c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
+    if (n == 0) return DAGR_OK;
+    k_sample_features<PLANES, MT><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
+        static_cast<const MT *>(img), Bi, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0, pl);
+    DAGR_CHECK_LAUNCH_AS(who);
+    return DAGR_OK;
 }
 
 extern "C" int dagr_sample_features(const float *img, int Bi, int C, int h, int w, const float *posx, const float *posy,
                                     const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
                                     void *stream)
 {
-    DAGR_CHECK_ARG(img && posx && posy && bidx && out, "null argument");
-    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(Bi >= 1 && C >= 1 && h >= 1 && w >= 1, "the map must have Bi, C, h, w >= 1");
-    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
-    if (n == 0) return DAGR_OK;
-    k_sample_features<false><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, Bi, C, h, w, posx, posy, bidx, n,
-                                                                                (float)width, (float)height, out, ldo, c0, ImgPlanes{});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return sample_features<false, float>(__func__, img, Bi, ImgPlanes{}, C, h, w, posx, posy, bidx, n, width, height, out, ldo, c0,
+                                         stream);
 }
 
 extern "C" int dagr_sample_features_planes(const float *img, int nplanes, const int32_t *plane, int plane_stride, int C, int h, int w,
                                            const float *posx, const float *posy, const int32_t *bidx, int64_t n, int width, int height,
                                            float *out, int ldo, int c0, void *stream)
 {
-    DAGR_CHECK_ARG(img && posx && posy && bidx && out && plane, "null argument");
-    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
-    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
-    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(C >= 1 && h >= 1 && w >= 1, "the map must have C, h, w >= 1");
-    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
-    if (n == 0) return DAGR_OK;
-    k_sample_features<true><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(img, 1, C, h, w, posx, posy, bidx, n, (float)width,
-                                                                               (float)height, out, ldo, c0,
-                                                                               ImgPlanes{plane, plane_stride, nplanes});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return sample_features<true, float>(__func__, img, 1, ImgPlanes{plane, plane_stride, nplanes}, C, h, w, posx, posy, bidx, n, width,
+                                        height, out, ldo, c0, stream);
 }
 
 // bf16 NHWC forms (include/dagr_b200.h): the same kernel with MT = __nv_bfloat16
@@ -844,31 +821,14 @@ extern "C" int dagr_sample_features_bf16(const void *img, int Bi, int C, int h, 
                                          const int32_t *bidx, int64_t n, int width, int height, float *out, int ldo, int c0,
                                          void *stream)
 {
-    DAGR_CHECK_ARG(img && posx && posy && bidx && out, "null argument");
-    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(Bi >= 1 && C >= 1 && h >= 1 && w >= 1, "the map must have Bi, C, h, w >= 1");
-    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
-    if (n == 0) return DAGR_OK;
-    k_sample_features<false, __nv_bfloat16><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
-        static_cast<const __nv_bfloat16 *>(img), Bi, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0, ImgPlanes{});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return sample_features<false, __nv_bfloat16>(__func__, img, Bi, ImgPlanes{}, C, h, w, posx, posy, bidx, n, width, height, out, ldo,
+                                                 c0, stream);
 }
 
 extern "C" int dagr_sample_features_planes_bf16(const void *img, int nplanes, const int32_t *plane, int plane_stride, int C, int h, int w,
                                                 const float *posx, const float *posy, const int32_t *bidx, int64_t n, int width,
                                                 int height, float *out, int ldo, int c0, void *stream)
 {
-    DAGR_CHECK_ARG(img && posx && posy && bidx && out && plane, "null argument");
-    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
-    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
-    DAGR_CHECK_ARG(n >= 0 && n < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(C >= 1 && h >= 1 && w >= 1, "the map must have C, h, w >= 1");
-    DAGR_CHECK_ARG(c0 >= 0 && c0 + C <= ldo, "the channels [c0, c0 + C) must lie within the row stride ldo");
-    if (n == 0) return DAGR_OK;
-    k_sample_features<true, __nv_bfloat16><<<dagr_div_up(n, 4), 128, 0, (cudaStream_t)stream>>>(
-        static_cast<const __nv_bfloat16 *>(img), 1, C, h, w, posx, posy, bidx, n, (float)width, (float)height, out, ldo, c0,
-        ImgPlanes{plane, plane_stride, nplanes});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return sample_features<true, __nv_bfloat16>(__func__, img, 1, ImgPlanes{plane, plane_stride, nplanes}, C, h, w, posx, posy, bidx, n,
+                                                width, height, out, ldo, c0, stream);
 }

@@ -13,13 +13,17 @@
 
 void dagr_set_error(const char *fmt, ...);
 
-#define DAGR_CHECK_ARG(cond, msg)                                              \
-    do { if (!(cond)) { dagr_set_error("%s: %s", __func__, msg); return DAGR_E_ARG; } } while (0)
+// The _AS forms name `who` in the error instead of the enclosing function: a launcher shared by several entry points passes
+// the entry point's __func__, so dagr_last_error() names the function the caller called.
+#define DAGR_CHECK_ARG_AS(who, cond, msg)                                      \
+    do { if (!(cond)) { dagr_set_error("%s: %s", who, msg); return DAGR_E_ARG; } } while (0)
+#define DAGR_CHECK_ARG(cond, msg) DAGR_CHECK_ARG_AS(__func__, cond, msg)
 
-#define DAGR_CHECK_LAUNCH()                                                    \
+#define DAGR_CHECK_LAUNCH_AS(who)                                              \
     do { cudaError_t e__ = cudaGetLastError();                                 \
-         if (e__ != cudaSuccess) { dagr_set_error("%s: %s", __func__, cudaGetErrorString(e__)); \
+         if (e__ != cudaSuccess) { dagr_set_error("%s: %s", who, cudaGetErrorString(e__)); \
                                    return DAGR_E_CUDA; } } while (0)
+#define DAGR_CHECK_LAUNCH() DAGR_CHECK_LAUNCH_AS(__func__)
 
 #define DAGR_CUDA(call)                                                        \
     do { cudaError_t e__ = (call);                                             \
@@ -70,6 +74,62 @@ __device__ __forceinline__ float map_ldg(const float *__restrict__ m, int C, int
 __device__ __forceinline__ float map_ldg(const __nv_bfloat16 *__restrict__ m, int C, int h, int w, int z, int c, int y, int x)
 {
     return __bfloat162float(__ldg(m + (((int64_t)z * h + y) * w + x) * C + c));
+}
+
+// grid_sample(align_corners=True) of one (x, y, batch) position: weights and corner offsets, mirroring
+// _sample_features (net.py:207-221): normalise with the event resolution, unnormalise with the map size.
+struct Bilin {
+    int x0, y0, z0;
+    float tx, ty, tz;
+};
+__device__ __forceinline__ Bilin bilin_setup(float posx, float posy, int b, float width, float height, int Bi, int h, int w)
+{
+    const float gx = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posx, width)), width - 1.f), 1.f);
+    const float gy = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posy, height)), height - 1.f), 1.f);
+    const float bs = (float)(Bi > 1 ? Bi : 2);
+    const float gz = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, (float)b), bs - 1.f), 1.f);
+    const float ix = __fmul_rn(__fmul_rn(__fadd_rn(gx, 1.f), 0.5f), (float)(w - 1));
+    const float iy = __fmul_rn(__fmul_rn(__fadd_rn(gy, 1.f), 0.5f), (float)(h - 1));
+    const float iz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.f), 0.5f), (float)(Bi - 1));
+    Bilin r;
+    const float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
+    r.x0 = (int)x0f; r.y0 = (int)y0f; r.z0 = (int)z0f;
+    r.tx = ix - x0f; r.ty = iy - y0f; r.tz = iz - z0f;
+    return r;
+}
+// One in-bounds corner of a trilinear sample: map element (z, y, x) and its weight's factors.  w() is the weight in the
+// oracle's association; each kernel calls it where its arithmetic has always had it (after the load in the per-channel loops,
+// before the loads in the voxel kernel's 8-channel path), so the shared loop leaves every kernel's instruction order as it was.
+struct BilinTap {
+    int z, y, x;
+    float wx, wy, wz;
+    __device__ __forceinline__ float w() const { return wx * wy * wz; }
+};
+// The trilinear taps of q in a [Bi][h][w] map with zero padding: f(tap) for each in-bounds corner, in the order dz, dy, dx.
+// Every image-sampling kernel walks its taps here and accumulates acc += v * tap.w(), so all of them (and the oracle) share
+// one tap order and one fp32 arithmetic; only the loader of v differs.
+template <typename F>
+__device__ __forceinline__ void bilin_taps(const Bilin &q, int Bi, int h, int w, F &&f)
+{
+#pragma unroll
+    for (int dz = 0; dz < 2; dz++) {
+        const int z = q.z0 + dz;
+        const float wz = dz ? q.tz : 1.f - q.tz;
+        if (z < 0 || z >= Bi) continue;
+#pragma unroll
+        for (int dy = 0; dy < 2; dy++) {
+            const int y = q.y0 + dy;
+            const float wy = dy ? q.ty : 1.f - q.ty;
+            if (y < 0 || y >= h) continue;
+#pragma unroll
+            for (int dx = 0; dx < 2; dx++) {
+                const int x = q.x0 + dx;
+                const float wx = dx ? q.tx : 1.f - q.tx;
+                if (x < 0 || x >= w) continue;
+                f(BilinTap{z, y, x, wx, wy, wz});
+            }
+        }
+    }
 }
 
 // exclusive prefix sum of n ints (graph.cu); blocksums: int[dagr_scan_blocks(n) + 2]; the grand total is left in

@@ -4,50 +4,12 @@
 #include "common.cuh"
 #include <type_traits>
 
-// grid_sample(align_corners=True) of one (x, y, batch) position: weights and corner offsets, mirroring
-// _sample_features (net.py:207-221): normalise with the event resolution, unnormalise with the map size.
-struct Bilin {
-    int x0, y0, z0;
-    float tx, ty, tz;
-};
-__device__ __forceinline__ Bilin bilin_setup(float posx, float posy, int b, float width, float height, int Bi, int h, int w)
-{
-    const float gx = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posx, width)), width - 1.f), 1.f);
-    const float gy = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, __fmul_rn(posy, height)), height - 1.f), 1.f);
-    const float bs = (float)(Bi > 1 ? Bi : 2);
-    const float gz = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, (float)b), bs - 1.f), 1.f);
-    const float ix = __fmul_rn(__fmul_rn(__fadd_rn(gx, 1.f), 0.5f), (float)(w - 1));
-    const float iy = __fmul_rn(__fmul_rn(__fadd_rn(gy, 1.f), 0.5f), (float)(h - 1));
-    const float iz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.f), 0.5f), (float)(Bi - 1));
-    Bilin r;
-    const float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
-    r.x0 = (int)x0f; r.y0 = (int)y0f; r.z0 = (int)z0f;
-    r.tx = ix - x0f; r.ty = iy - y0f; r.tz = iz - z0f;
-    return r;
-}
+// channel c of the map sampled at q, read through the read-only path
 template <typename MT>
 __device__ __forceinline__ float bilin_sample(const MT *__restrict__ img, int Bi, int C, int h, int w, int c, const Bilin &q)
 {
     float acc = 0.f;
-#pragma unroll
-    for (int dz = 0; dz < 2; dz++) {
-        const int z = q.z0 + dz;
-        const float wz = dz ? q.tz : 1.f - q.tz;
-        if (z < 0 || z >= Bi) continue;
-#pragma unroll
-        for (int dy = 0; dy < 2; dy++) {
-            const int y = q.y0 + dy;
-            const float wy = dy ? q.ty : 1.f - q.ty;
-            if (y < 0 || y >= h) continue;
-#pragma unroll
-            for (int dx = 0; dx < 2; dx++) {
-                const int x = q.x0 + dx;
-                const float wx = dx ? q.tx : 1.f - q.tx;
-                if (x < 0 || x >= w) continue;
-                acc += map_ldg(img, C, h, w, z, c, y, x) * (wx * wy * wz);
-            }
-        }
-    }
+    bilin_taps(q, Bi, h, w, [&](const BilinTap &t) { acc += map_ldg(img, C, h, w, t.z, c, t.y, t.x) * t.w(); });
     return acc;
 }
 
@@ -60,7 +22,7 @@ __device__ __forceinline__ float bilin_sample(const MT *__restrict__ img, int Bi
 // [start[cell], start[cell+1]) ranges, which lie below the total), so they are simply skipped.  live == NULL: the bound is N.
 // PLANES: img0 is a plane array [pl.n][16][h][w] and the event of sample b samples plane img_plane(pl, b) as a batch of one.
 // MT: the map format (common.cuh: float = NCHW, __nv_bfloat16 = NHWC).
-template <bool PLANES, typename MT = float>
+template <bool PLANES, typename MT>
 __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__restrict__ live, const uint32_t *__restrict__ xyb,
                               const MT *__restrict__ img0, int h, int w, float *__restrict__ x0, const ImgPlanes pl)
 {
@@ -82,136 +44,84 @@ __global__ void k_l1_x0_image(const dagr_geom_t g, int64_t N, const int32_t *__r
     dst[(q & 1) ^ XA_SWZ(p)] = make_float4(f[0], f[1], f[2], f[3]);
 }
 
-extern "C" int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s, const float *img0,
+// The checks and the launch of every x0 form.  live: the form bounds x0 by the live total start[g.NK] (ring and plane forms),
+// so start must not be NULL; the unbounded forms pass start = NULL.  The fp32 forms pass C = 16 (their NCHW tap has 16 channels
+// by definition), the bf16 forms the caller's C.  feat_s is not an input of any form.
+template <bool PLANES, typename MT>
+static int x0_image(const char *who, const dagr_geom_t *g, int64_t N, bool live, const int32_t *start, const uint32_t *xyb,
+                    const void *img0, int C, int h, int w, const ImgPlanes pl, float *x0, void *stream)
+{
+    DAGR_CHECK_ARG_AS(who, g && (start || !live) && xyb && img0 && (pl.plane || !PLANES) && x0, "null argument (only feat_s may be NULL)");
+    if (PLANES) {
+        DAGR_CHECK_ARG_AS(who, pl.n >= 1, "nplanes must be >= 1");
+        DAGR_CHECK_ARG_AS(who, pl.stride >= 1, "plane_stride must be >= 1");
+    }
+    DAGR_CHECK_ARG_AS(who, N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG_AS(who, C == 16 && h >= 1 && w >= 1, "the conv1 tap must have 16 channels and h, w >= 1");
+    if (N == 0) return DAGR_OK;
+    k_l1_x0_image<PLANES, MT><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(
+        *g, N, start, xyb, static_cast<const MT *>(img0), h, w, x0, pl);
+    DAGR_CHECK_LAUNCH_AS(who);
+    return DAGR_OK;
+}
+
+extern "C" int dagr_l1_x0_image(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float * /*feat_s*/, const float *img0,
                                 int h, int w, float *x0, void *stream)
 {
-    (void)feat_s;
-    DAGR_CHECK_ARG(g && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the conv1 tap is [B, 16, h, w] with h, w >= 1");
-    if (N == 0) return DAGR_OK;
-    k_l1_x0_image<false><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, nullptr, xyb, img0, h, w, x0, ImgPlanes{});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return x0_image<false, float>(__func__, g, N, false, nullptr, xyb, img0, 16, h, w, ImgPlanes{}, x0, stream);
 }
 
-extern "C" int dagr_l1_x0_image_live(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+extern "C" int dagr_l1_x0_image_live(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float * /*feat_s*/,
                                      const float *img0, int h, int w, float *x0, void *stream)
 {
-    (void)feat_s;
-    DAGR_CHECK_ARG(g && start && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the conv1 tap is [B, 16, h, w] with h, w >= 1");
-    if (N == 0) return DAGR_OK;
-    k_l1_x0_image<false><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0, ImgPlanes{});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return x0_image<false, float>(__func__, g, N, true, start, xyb, img0, 16, h, w, ImgPlanes{}, x0, stream);
 }
 
-extern "C" int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
+extern "C" int dagr_l1_x0_image_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float * /*feat_s*/,
                                        const float *img0, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *x0,
                                        void *stream)
 {
-    (void)feat_s;
-    DAGR_CHECK_ARG(g && start && xyb && img0 && plane && x0, "null argument (only feat_s may be NULL)");
-    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
-    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the conv1 tap is [nplanes, 16, h, w] with h, w >= 1");
-    if (N == 0) return DAGR_OK;
-    k_l1_x0_image<true><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(*g, N, start, xyb, img0, h, w, x0,
-                                                                                 ImgPlanes{plane, plane_stride, nplanes});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return x0_image<true, float>(__func__, g, N, true, start, xyb, img0, 16, h, w, ImgPlanes{plane, plane_stride, nplanes}, x0, stream);
 }
 
-// bf16 NHWC forms (include/dagr_b200.h): the same kernel with the map loader of MT = __nv_bfloat16.  live == NULL selects the
-// unbounded form, nplanes == 0 the non-plane one.
-static int x0_image_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const void *img0, int h, int w,
-                         int nplanes, const int32_t *plane, int plane_stride, float *x0, void *stream)
-{
-    const __nv_bfloat16 *img = static_cast<const __nv_bfloat16 *>(img0);
-    if (nplanes)
-        k_l1_x0_image<true, __nv_bfloat16><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(
-            *g, N, start, xyb, img, h, w, x0, ImgPlanes{plane, plane_stride, nplanes});
-    else
-        k_l1_x0_image<false, __nv_bfloat16><<<dagr_div_up(4 * N, 256), 256, 0, (cudaStream_t)stream>>>(
-            *g, N, start, xyb, img, h, w, x0, ImgPlanes{});
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
-extern "C" int dagr_l1_x0_image_bf16(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float *feat_s, const void *img0,
+// bf16 NHWC forms (include/dagr_b200.h): the same kernel with the map loader of MT = __nv_bfloat16
+extern "C" int dagr_l1_x0_image_bf16(const dagr_geom_t *g, int64_t N, const uint32_t *xyb, const float * /*feat_s*/, const void *img0,
                                      int C, int h, int w, float *x0, void *stream)
 {
-    (void)feat_s;
-    DAGR_CHECK_ARG(g && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(C == 16 && h >= 1 && w >= 1, "the conv1 tap is [B, h, w, 16] with h, w >= 1");
-    if (N == 0) return DAGR_OK;
-    return x0_image_bf16(g, N, nullptr, xyb, img0, h, w, 0, nullptr, 0, x0, stream);
+    return x0_image<false, __nv_bfloat16>(__func__, g, N, false, nullptr, xyb, img0, C, h, w, ImgPlanes{}, x0, stream);
 }
 
-extern "C" int dagr_l1_x0_image_live_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *feat_s,
-                                          const void *img0, int C, int h, int w, float *x0, void *stream)
+extern "C" int dagr_l1_x0_image_live_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
+                                          const float * /*feat_s*/, const void *img0, int C, int h, int w, float *x0, void *stream)
 {
-    (void)feat_s;
-    DAGR_CHECK_ARG(g && start && xyb && img0 && x0, "null argument (only feat_s may be NULL)");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(C == 16 && h >= 1 && w >= 1, "the conv1 tap is [B, h, w, 16] with h, w >= 1");
-    if (N == 0) return DAGR_OK;
-    return x0_image_bf16(g, N, start, xyb, img0, h, w, 0, nullptr, 0, x0, stream);
+    return x0_image<false, __nv_bfloat16>(__func__, g, N, true, start, xyb, img0, C, h, w, ImgPlanes{}, x0, stream);
 }
 
 extern "C" int dagr_l1_x0_image_planes_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb,
-                                            const float *feat_s, const void *img0, int C, int h, int w, int nplanes, const int32_t *plane,
+                                            const float * /*feat_s*/, const void *img0, int C, int h, int w, int nplanes, const int32_t *plane,
                                             int plane_stride, float *x0, void *stream)
 {
-    (void)feat_s;
-    DAGR_CHECK_ARG(g && start && xyb && img0 && plane && x0, "null argument (only feat_s may be NULL)");
-    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
-    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(C == 16 && h >= 1 && w >= 1, "the conv1 tap is [nplanes, h, w, 16] with h, w >= 1");
-    if (N == 0) return DAGR_OK;
-    return x0_image_bf16(g, N, start, xyb, img0, h, w, nplanes, plane, plane_stride, x0, stream);
+    return x0_image<true, __nv_bfloat16>(__func__, g, N, true, start, xyb, img0, C, h, w, ImgPlanes{plane, plane_stride, nplanes}, x0,
+                                         stream);
 }
 
 // ------------------------------------------------------------------------------------------------
 // per-voxel max of image features sampled at the voxel's events (net.py:128-131 before pool1): one CTA per voxel.
 // All events of a voxel sample a small window of the feature map (voxel extent x map/sensor scale, + 1), so the window
 // of both batch planes the trilinear sample can touch is staged in shared memory once ([z][y][x][C], channels
-// innermost -> conflict-free), and every (event, channel) sample reads shared memory only.  The tap order and the
-// fp32 arithmetic are those of bilin_sample, i.e. of the oracle.  Windows that do not fit fall back to global taps.
+// innermost -> conflict-free), and every (event, channel) sample reads shared memory only.  The taps are bilin_taps'
+// (common.cuh), i.e. the oracle's.  Windows that do not fit fall back to global taps (bilin_sample).
 // ------------------------------------------------------------------------------------------------
 #define VS_THREADS 128
 
-template <bool STAGED, typename MT>
-__device__ __forceinline__ float vs_sample(const MT *__restrict__ img, const float *s_patch, int Bi, int C, int h, int w,
-                                           int c, const Bilin &q, int zb, int yb, int xb, int ph, int pw)
+// channel c sampled at q from the staged window [z - zb][y - yb][x - xb][C]
+__device__ __forceinline__ float vs_sample(const float *s_patch, int Bi, int C, int h, int w, int c, const Bilin &q, int zb, int yb,
+                                           int xb, int ph, int pw)
 {
     float acc = 0.f;
-#pragma unroll
-    for (int dz = 0; dz < 2; dz++) {
-        const int z = q.z0 + dz;
-        const float wz = dz ? q.tz : 1.f - q.tz;
-        if (z < 0 || z >= Bi) continue;
-#pragma unroll
-        for (int dy = 0; dy < 2; dy++) {
-            const int y = q.y0 + dy;
-            const float wy = dy ? q.ty : 1.f - q.ty;
-            if (y < 0 || y >= h) continue;
-#pragma unroll
-            for (int dx = 0; dx < 2; dx++) {
-                const int x = q.x0 + dx;
-                const float wx = dx ? q.tx : 1.f - q.tx;
-                if (x < 0 || x >= w) continue;
-                const float v = STAGED ? s_patch[(((z - zb) * ph + (y - yb)) * pw + (x - xb)) * C + c]
-                                       : map_ldg(img, C, h, w, z, c, y, x);
-                acc += v * (wx * wy * wz);
-            }
-        }
-    }
+    bilin_taps(q, Bi, h, w, [&](const BilinTap &t) {
+        acc += s_patch[(((t.z - zb) * ph + (t.y - yb)) * pw + (t.x - xb)) * C + c] * t.w();
+    });
     return acc;
 }
 
@@ -226,11 +136,11 @@ template <bool MEAN> __device__ __forceinline__ float vs_comb(float a, float b) 
 // window is staged from that one plane (pz = 1).
 // MT: the map format (common.cuh: float = NCHW, __nv_bfloat16 = NHWC).  The window is staged as fp32 in either, so the sampling
 // below reads the same shared memory in both.
-template <bool MEAN, bool INC, bool PLANES = false, typename MT = float>
+template <bool MEAN, bool INC, bool PLANES, typename MT>
 __global__ void __launch_bounds__(VS_THREADS)
 k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const uint32_t *__restrict__ xyb,
                    const int2 *__restrict__ ti, const MT *__restrict__ img_in, int C, int h, int w, const int min_idx,
-                   float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0, const ImgPlanes pl = ImgPlanes{})
+                   float *__restrict__ persist, float *__restrict__ xg, int ldx, int c0, const ImgPlanes pl)
 {
     __shared__ float s_m[VS_THREADS / 32][128];
     __shared__ __align__(16) float s_patch[DAGR_VS_SMEM_FLOATS];
@@ -310,29 +220,13 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
                 float acc[8];
 #pragma unroll
                 for (int k = 0; k < 8; k++) acc[k] = 0.f;
-#pragma unroll
-                for (int dz = 0; dz < 2; dz++) {
-                    const int z = q.z0 + dz;
-                    const float wz = dz ? q.tz : 1.f - q.tz;
-                    if (z < 0 || z >= (PLANES ? 1 : g.B)) continue;
-#pragma unroll
-                    for (int dy = 0; dy < 2; dy++) {
-                        const int yy = q.y0 + dy;
-                        const float wy = dy ? q.ty : 1.f - q.ty;
-                        if (yy < 0 || yy >= h) continue;
-#pragma unroll
-                        for (int dx = 0; dx < 2; dx++) {
-                            const int xx = q.x0 + dx;
-                            const float wx = dx ? q.tx : 1.f - q.tx;
-                            if (xx < 0 || xx >= w) continue;
-                            const float wgt = wx * wy * wz;                 // same association as bilin_sample
-                            const float4 *src = reinterpret_cast<const float4 *>(s_patch + (((z - zb) * ph + (yy - yb)) * pw + (xx - xb)) * C + cl);
-                            const float4 v0 = src[0], v1 = src[1];
-                            acc[0] += v0.x * wgt; acc[1] += v0.y * wgt; acc[2] += v0.z * wgt; acc[3] += v0.w * wgt;
-                            acc[4] += v1.x * wgt; acc[5] += v1.y * wgt; acc[6] += v1.z * wgt; acc[7] += v1.w * wgt;
-                        }
-                    }
-                }
+                bilin_taps(q, PLANES ? 1 : g.B, h, w, [&](const BilinTap &t) {
+                    const float wgt = t.w();
+                    const float4 *src = reinterpret_cast<const float4 *>(s_patch + (((t.z - zb) * ph + (t.y - yb)) * pw + (t.x - xb)) * C + cl);
+                    const float4 v0 = src[0], v1 = src[1];
+                    acc[0] += v0.x * wgt; acc[1] += v0.y * wgt; acc[2] += v0.z * wgt; acc[3] += v0.w * wgt;
+                    acc[4] += v1.x * wgt; acc[5] += v1.y * wgt; acc[6] += v1.z * wgt; acc[7] += v1.w * wgt;
+                });
 #pragma unroll
                 for (int k = 0; k < 8; k++) m[k] = vs_comb<MEAN>(m[k], acc[k]);
             }
@@ -366,8 +260,8 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
             for (int k = 0; k < 4; k++) {
                 const int c = cb + lane + 32 * k;
                 if (c < C)
-                    m[k] = vs_comb<MEAN>(m[k], staged ? vs_sample<true>(img, s_patch, PLANES ? 1 : g.B, C, h, w, c, bl, zb, yb, xb, ph, pw)
-                                                      : vs_sample<false>(img, s_patch, PLANES ? 1 : g.B, C, h, w, c, bl, zb, yb, xb, ph, pw));
+                    m[k] = vs_comb<MEAN>(m[k], staged ? vs_sample(s_patch, PLANES ? 1 : g.B, C, h, w, c, bl, zb, yb, xb, ph, pw)
+                                                      : bilin_sample(img, PLANES ? 1 : g.B, C, h, w, c, bl));
             }
         }
 #pragma unroll
@@ -383,117 +277,78 @@ k_voxel_sample_max(const dagr_geom_t g, const int32_t *__restrict__ start, const
     }
 }
 
+// The checks and the launch of every voxel form; pool_mean selects MEAN.  The INC forms pass ti, min_idx and persist, the others
+// NULL, 0 and NULL.  Every form launches at N == 0 too: the kernel writes the zeros of the empty voxels.
+template <bool INC, bool PLANES, typename MT>
+static int voxel_sample(const char *who, const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
+                        const void *img_in, int C, int h, int w, int min_idx, float *persist, const ImgPlanes pl, float *xg, int ldx,
+                        int c0, int pool_mean, void *stream)
+{
+    DAGR_CHECK_ARG_AS(who, g && start && xyb && (ti || !INC) && img_in && (persist || !INC) && (pl.plane || !PLANES) && xg, "null argument");
+    if (INC) DAGR_CHECK_ARG_AS(who, min_idx >= 0, "min_idx must be >= 0");
+    if (PLANES) {
+        DAGR_CHECK_ARG_AS(who, pl.n >= 1, "nplanes must be >= 1");
+        DAGR_CHECK_ARG_AS(who, pl.stride >= 1, "plane_stride must be >= 1");
+    }
+    DAGR_CHECK_ARG_AS(who, N >= 0 && N < (1ll << 31), "N out of range");
+    DAGR_CHECK_ARG_AS(who, h >= 1 && w >= 1, "the map must have h, w >= 1");
+    DAGR_CHECK_ARG_AS(who, C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
+    if (INC) DAGR_CHECK_ARG_AS(who, !pool_mean, "pool_mean: the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
+    const int cells = g->B * g->ny1 * g->nx1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const MT *img = static_cast<const MT *>(img_in);
+    // MEAN never meets INC (refused above), and naming that pair would compile an instance that no form launches
+    if (!INC && pool_mean) k_voxel_sample_max<true, false, PLANES, MT><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, (const int2 *)ti, img, C,
+                                                                                                   h, w, min_idx, persist, xg, ldx, c0, pl);
+    else                   k_voxel_sample_max<false, INC, PLANES, MT><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, (const int2 *)ti, img, C,
+                                                                                                  h, w, min_idx, persist, xg, ldx, c0, pl);
+    DAGR_CHECK_LAUNCH_AS(who);
+    return DAGR_OK;
+}
+
 extern "C" int dagr_voxel_sample_max(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *img,
                                      int C, int h, int w, float *xg, int ldx, int c0, int pool_mean, void *stream)
 {
-    DAGR_CHECK_ARG(g && start && xyb && img && xg, "null argument");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
-    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
-    const int cells = g->B * g->ny1 * g->nx1;
-    if (pool_mean) k_voxel_sample_max<true, false><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
-                                                                                                 nullptr, xg, ldx, c0);
-    else           k_voxel_sample_max<false, false><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
-                                                                                                  nullptr, xg, ldx, c0);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return voxel_sample<false, false, float>(__func__, g, N, start, xyb, nullptr, img, C, h, w, 0, nullptr, ImgPlanes{}, xg, ldx, c0,
+                                             pool_mean, stream);
 }
 
 extern "C" int dagr_voxel_sample_max_inc(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
                                          const float *img, int C, int h, int w, int min_idx, float *persist, float *xg, int ldx, int c0,
                                          int pool_mean, void *stream)
 {
-    DAGR_CHECK_ARG(g && start && xyb && ti && img && persist && xg, "null argument");
-    DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
-    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
-    DAGR_CHECK_ARG(!pool_mean, "pool_mean: the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
-    const int cells = g->B * g->ny1 * g->nx1;
-    k_voxel_sample_max<false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, (const int2 *)ti, img, C, h, w, min_idx,
-                                                                                   persist, xg, ldx, c0);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return voxel_sample<true, false, float>(__func__, g, N, start, xyb, ti, img, C, h, w, min_idx, persist, ImgPlanes{}, xg, ldx, c0,
+                                            pool_mean, stream);
 }
 
 extern "C" int dagr_voxel_sample_max_planes(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const float *img,
                                             int C, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *xg, int ldx,
                                             int c0, int pool_mean, void *stream)
 {
-    DAGR_CHECK_ARG(g && start && xyb && img && plane && xg, "null argument");
-    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
-    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
-    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
-    const int cells = g->B * g->ny1 * g->nx1;
-    const ImgPlanes pl{plane, plane_stride, nplanes};
-    if (pool_mean) k_voxel_sample_max<true, false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h, w,
-                                                                                                      0, nullptr, xg, ldx, c0, pl);
-    else           k_voxel_sample_max<false, false, true><<<cells, VS_THREADS, 0, (cudaStream_t)stream>>>(*g, start, xyb, nullptr, img, C, h,
-                                                                                                       w, 0, nullptr, xg, ldx, c0, pl);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
+    return voxel_sample<false, true, float>(__func__, g, N, start, xyb, nullptr, img, C, h, w, 0, nullptr,
+                                            ImgPlanes{plane, plane_stride, nplanes}, xg, ldx, c0, pool_mean, stream);
 }
 
-// bf16 NHWC forms (include/dagr_b200.h): the same kernel with MT = __nv_bfloat16.  ti == NULL selects the non-incremental
-// instances, nplanes == 0 the non-plane ones.
-static int voxel_sample_bf16(const dagr_geom_t *g, const int32_t *start, const uint32_t *xyb, const int32_t *ti, const void *img_in,
-                             int C, int h, int w, int min_idx, float *persist, int nplanes, const int32_t *plane, int plane_stride,
-                             float *xg, int ldx, int c0, int pool_mean, void *stream)
-{
-    typedef __nv_bfloat16 bf;
-    const bf *img = static_cast<const bf *>(img_in);
-    const int cells = g->B * g->ny1 * g->nx1;
-    const cudaStream_t st = (cudaStream_t)stream;
-    const ImgPlanes pl{plane, plane_stride, nplanes};
-    if (ti)             k_voxel_sample_max<false, true, false, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, (const int2 *)ti, img, C, h, w,
-                                                                                               min_idx, persist, xg, ldx, c0);
-    else if (nplanes && pool_mean) k_voxel_sample_max<true, false, true, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h,
-                                                                                                          w, 0, nullptr, xg, ldx, c0, pl);
-    else if (nplanes)   k_voxel_sample_max<false, false, true, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
-                                                                                                nullptr, xg, ldx, c0, pl);
-    else if (pool_mean) k_voxel_sample_max<true, false, false, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
-                                                                                                nullptr, xg, ldx, c0);
-    else                k_voxel_sample_max<false, false, false, bf><<<cells, VS_THREADS, 0, st>>>(*g, start, xyb, nullptr, img, C, h, w, 0,
-                                                                                                 nullptr, xg, ldx, c0);
-    DAGR_CHECK_LAUNCH();
-    return DAGR_OK;
-}
-
+// bf16 NHWC forms (include/dagr_b200.h): the same kernel with MT = __nv_bfloat16
 extern "C" int dagr_voxel_sample_max_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const void *img,
                                           int C, int h, int w, float *xg, int ldx, int c0, int pool_mean, void *stream)
 {
-    DAGR_CHECK_ARG(g && start && xyb && img && xg, "null argument");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
-    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
-    return voxel_sample_bf16(g, start, xyb, nullptr, img, C, h, w, 0, nullptr, 0, nullptr, 0, xg, ldx, c0, pool_mean, stream);
+    return voxel_sample<false, false, __nv_bfloat16>(__func__, g, N, start, xyb, nullptr, img, C, h, w, 0, nullptr, ImgPlanes{}, xg, ldx,
+                                                     c0, pool_mean, stream);
 }
 
 extern "C" int dagr_voxel_sample_max_inc_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const int32_t *ti,
                                               const void *img, int C, int h, int w, int min_idx, float *persist, float *xg, int ldx, int c0,
                                               int pool_mean, void *stream)
 {
-    DAGR_CHECK_ARG(g && start && xyb && ti && img && persist && xg, "null argument");
-    DAGR_CHECK_ARG(min_idx >= 0, "min_idx must be >= 0");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
-    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
-    DAGR_CHECK_ARG(!pool_mean, "pool_mean: the running per-voxel aggregate of the event stream is a max (max_pool.py:59-62)");
-    return voxel_sample_bf16(g, start, xyb, ti, img, C, h, w, min_idx, persist, 0, nullptr, 0, xg, ldx, c0, 0, stream);
+    return voxel_sample<true, false, __nv_bfloat16>(__func__, g, N, start, xyb, ti, img, C, h, w, min_idx, persist, ImgPlanes{}, xg, ldx,
+                                                    c0, pool_mean, stream);
 }
 
 extern "C" int dagr_voxel_sample_max_planes_bf16(const dagr_geom_t *g, int64_t N, const int32_t *start, const uint32_t *xyb, const void *img,
                                                  int C, int h, int w, int nplanes, const int32_t *plane, int plane_stride, float *xg,
                                                  int ldx, int c0, int pool_mean, void *stream)
 {
-    DAGR_CHECK_ARG(g && start && xyb && img && plane && xg, "null argument");
-    DAGR_CHECK_ARG(nplanes >= 1, "nplanes must be >= 1");
-    DAGR_CHECK_ARG(plane_stride >= 1, "plane_stride must be >= 1");
-    DAGR_CHECK_ARG(N >= 0 && N < (1ll << 31), "N out of range");
-    DAGR_CHECK_ARG(h >= 1 && w >= 1, "the map must have h, w >= 1");
-    DAGR_CHECK_ARG(C >= 1 && c0 >= 0 && c0 + C <= ldx, "the channels [c0, c0 + C) must lie within the row stride ldx");
-    return voxel_sample_bf16(g, start, xyb, nullptr, img, C, h, w, 0, nullptr, nplanes, plane, plane_stride, xg, ldx, c0, pool_mean,
-                             stream);
+    return voxel_sample<false, true, __nv_bfloat16>(__func__, g, N, start, xyb, nullptr, img, C, h, w, 0, nullptr,
+                                                    ImgPlanes{plane, plane_stride, nplanes}, xg, ldx, c0, pool_mean, stream);
 }
