@@ -152,8 +152,10 @@ class Engine:
         self.prof = None                     # dict name -> [(start_evt, end_evt)] when per-op timing is on
         # overlap=True: the coarse stack + NMS of step i run on a side stream (double-buffered hand-off) while the
         # caller's stream already executes the event-level kernels of step i+1.  Results of a step are then valid only
-        # after join() (or on result_stream()); they stay valid until the second next forward.  Events-only model,
-        # reset=True forwards; everything else silently takes the serial path.
+        # after join() (or on result_stream()); they stay valid until the second next forward.  Plain reset=True
+        # batches, events-only or with image taps (whose last reader is then the side stream: a caller that rewrites
+        # them waits for _done[slot], see next_slot()); streaming, incremental and per-sample-frame forwards silently
+        # take the serial path.
         self.overlap = False
         self._cstream = None
         self._fstream = None                 # forked branch of the coarse stack (first head scale)
@@ -380,6 +382,13 @@ class Engine:
             slots[slot] = sw
         return _WsView(ws, sw)
 
+    def next_slot(self):
+        """-> (slot, event) of the next plain forward when it overlaps (overlap on, no per-op timing, graphs on), else
+        None: the hand-off slot it will use and the event of the last step that read that slot (None if none did)."""
+        if not (self.overlap and self.prof is None and self.use_graphs):
+            return None
+        return self._slot, self._done[self._slot]
+
     def join(self):
         """make the current stream wait for every coarse stack / NMS still running on the side stream."""
         cur = torch.cuda.current_stream()
@@ -567,7 +576,8 @@ class Engine:
         geom = self.geometry(W, H, B, dev)
         pk = self.pack(geom, dev)
         ws = self.workspace(geom, N, dev)
-        ov = bool(self.overlap and stream_state is None and image_feats is None and self.prof is None and self.use_graphs and ring is None)
+        ov = bool(self.overlap and stream_state is None and image_planes is None and self.prof is None and self.use_graphs
+                  and ring is None)
         slot = 0
         if ov:
             slot, self._slot = self._slot, self._slot ^ 1
@@ -704,7 +714,7 @@ class Engine:
         if kto:
             self._run("temporal_filter", lib.dagr_grid_temporal_filter, C.byref(geom.levels[0].grid), _lib.ptr(g1.cnt), _lib.ptr(g1.tmax),
                                                      _lib.ptr(g1.mask), st)
-        def coarse(st):
+        def coarse(st, image_wait=True):
             # ---- coarse levels -------------------------------------------------------------------
             aggr_cfg = 0 if getattr(model.args, "pooling_aggr", "max") == "max" else 1
             lay = pk["layers"]
@@ -713,7 +723,7 @@ class Engine:
                 return self._append_image(geom, lv, gs, o, image_feats[k], ws, st, dev, image_planes) if use_image else o
 
             _, _, o2 = self._layer(geom, 0, g1, lay[0], ws, "layer2", st, dev)
-            if use_image and image_event is not None:         # layer2..4 taps + CNN head maps (stage 2 of the image branch)
+            if use_image and image_event is not None and image_wait:   # layer2..4 taps + CNN head maps (image branch stage 2)
                 torch.cuda.current_stream().wait_event(image_event[1])
             g2 = self._pool(geom, 0, g1, cat_img(0, g1, o2, 2), aggr_cfg, ws, st, dev, kto)
             _, _, o3 = self._layer(geom, 1, g2, lay[1], ws, "layer3", st, dev)
@@ -787,18 +797,26 @@ class Engine:
             return out, [g1, g2, g3, g4], inter, dense_all
 
         # The coarse stack is ~55 small, fixed-shape launches: replay it as ONE CUDA graph (captured on the second
-        # call with identical buffers; the event-level kernels stay eager because their grids depend on N).
+        # call with identical buffers; the event-level kernels stay eager because their grids depend on N).  With image
+        # fusion only the overlapped step is captured (the serial hybrid forward stays eager); its graph reads the taps and
+        # head maps at fixed addresses, so they and their format are part of the key.
         gkey = (id(ws.base), slot, self._pack_gen, B, kto, cellmask.data_ptr(), bool(self.keep_node_features))
+        if use_image:
+            gkey += (sfx, tuple(t.data_ptr() for t in image_feats),
+                     tuple((k, tuple(t.data_ptr() for t in v)) for k, v in sorted((image_outs or {}).items())))
 
         def run_coarse():
-            if self.use_graphs and self.prof is None and not use_image and ring is None:
+            if self.use_graphs and self.prof is None and (ov or not use_image) and ring is None:
+                if use_image and image_event is not None:
+                    # a captured graph cannot wait for an event recorded outside it: the whole stack waits for stage 2
+                    torch.cuda.current_stream().wait_event(image_event[1])
                 cached = ws.get("graph")
                 if cached is not None and cached[0] == gkey:
                     cached[1].replay()
                     self.launches += cached[3]
                     return cached[2]
                 l0 = self.launches
-                res = coarse(_lib.stream_ptr())                          # eager: also allocates every pool buffer
+                res = coarse(_lib.stream_ptr(), image_wait=False)        # eager: also allocates every pool buffer
                 nk = self.launches - l0
                 ws["graph_warm"] = ws.get("graph_warm", 0) + 1
                 if ws["graph_warm"] >= 2 and ws.get("graph_key") == gkey:
@@ -807,7 +825,7 @@ class Engine:
                     # kernel nodes inherit the priority of the CAPTURE stream: capture on the high-priority side stream in
                     # overlap mode so the small coarse kernels get SM slots while a big event-level kernel is resident
                     with torch.cuda.graph(gr, stream=self._cstream if ov else None):
-                        res_c = coarse(_lib.stream_ptr())
+                        res_c = coarse(_lib.stream_ptr(), image_wait=False)
                     self.launches -= nk                                  # capture enqueues nothing
                     ws["graph"] = (gkey, gr, res_c, nk)
                 ws["graph_key"] = gkey
@@ -815,6 +833,9 @@ class Engine:
             return coarse(st)
 
         if ov:
+            if use_image:                                 # the caching allocator must not hand them out while the stack reads
+                for t in (*image_feats, *(t for v in (image_outs or {}).values() for t in v)):
+                    t.record_stream(self._cstream)
             fine_done = torch.cuda.Event()
             fine_done.record()
             with torch.cuda.stream(self._cstream):

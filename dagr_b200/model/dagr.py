@@ -224,8 +224,12 @@ class DAGR(YOLOX):
         feat = x.x.float().reshape(N, -1)[:, 0].contiguous() if N > 0 else torch.zeros(0, device=dev)
         return batch_i, pos_i, feat, W, H
 
-    def forward_decoded(self, x, reset=True):
-        """backbone + head up to decode_outputs: [B, n_anchors, 5 + num_classes]."""
+    def forward_decoded(self, x, reset=True, frame_ready=None, inputs_read=None):
+        """backbone + head up to decode_outputs: [B, n_anchors, 5 + num_classes].
+
+        For a caller that runs the forward on a stream of its own (PipelinedDetector): `frame_ready` is the event on which
+        x.image is valid, which the image branch of an overlapped step waits for instead of the current stream, and
+        `inputs_read` a list that receives the events after which x's tensors are no longer read."""
         if not reset:
             # incremental call sequence of the reference (evaluate_flops.py:115-116: forward(reset=True) then
             # forward(new events, reset=False)): append to the stream started by the last reset=True forward
@@ -239,12 +243,22 @@ class DAGR(YOLOX):
             return self._async.step_decoded(x, batch_size=int(getattr(x, "num_graphs", 1) or 1))
         batch_i, pos_i, feat, W, H = self._prepare_events(x)
         B = int(getattr(x, "num_graphs", 0) or (int(x.batch.max()) + 1 if len(x.batch) else 1))
+        if inputs_read is not None:
+            ev = torch.cuda.Event()
+            ev.record()
+            inputs_read.append(ev)
         image_feats = image_outs = image_event = None
         if self.backbone.use_image:
             # dense image trunk + CNN head stay torch/cuDNN (tensor cores allowed here only), net.py:110, dagr.py:205-206;
-            # they run on a side stream, concurrently with the sort + radius-graph kernels below
+            # they run on a side stream, concurrently with the sort + radius-graph kernels below.  An overlapped step
+            # (Engine.overlap) gets the outputs of its hand-off slot, which the coarse stack of the step before it does not read
+            nxt = None if self.head.no_events else self.engine.next_slot()
+            slot, after = nxt if nxt is not None else (None, None)
             image_feats, image_outs, image_event = branch_of(self).run(x.image, use_graph=self.image_graph,
-                                                                       precision=self.image_precision)
+                                                                       precision=self.image_precision, slot=slot, after=after,
+                                                                       ready=frame_ready if slot is not None else None)
+            if inputs_read is not None:
+                inputs_read.append(image_event[0])           # stage 1 has read the frame
             self.last_image_outs, self.last_image_feats = image_outs, image_feats
             if self.head.no_events:
                 # --no_events (dagr.py:284): detections from the image branch alone -- collect_outputs + decode_outputs on

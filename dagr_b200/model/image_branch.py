@@ -87,21 +87,35 @@ class ImageBranch:
         return feats, cnn_head(cnn_in)
 
     @torch.no_grad()
-    def run(self, image: torch.Tensor, use_graph: bool = True, precision: str = "tf32"):
+    def run(self, image: torch.Tensor, use_graph: bool = True, precision: str = "tf32", slot=None, after=None, ready=None):
         """-> (image_feats, image_outs, (event1, event2)): the first two feature maps are valid on any stream that waited
         for event1, everything else after event2; all of them are overwritten by the next call (static graph buffers).
-        precision "tf32": fp32 NCHW feature maps; "bf16": bf16 channels_last ones (the module docstring)."""
+        precision "tf32": fp32 NCHW feature maps; "bf16": bf16 channels_last ones (the module docstring).
+
+        slot = k selects a set of graphs and outputs of its own, which only calls with the same slot overwrite (the two
+        hand-off slots of Engine.overlap); `after` is then the event of the last reader of that slot's outputs, and
+        `ready`, when given, the event on which the image is valid: the branch then waits for these two alone, not for
+        the current stream (PipelinedDetector, whose current stream holds the previous batch's event-level kernels).
+        Without a slot every reader of the outputs is on the current stream, which the branch waits for."""
         if precision not in PRECISIONS:
             raise ValueError(f"image precision {precision!r}: expected one of {PRECISIONS}")
+        if ready is not None and slot is None:
+            raise ValueError("ready= replaces the wait for the current stream: only a slot's outputs have their last reader in `after`")
         dev = image.device
         cur = torch.cuda.current_stream(dev)
         if self.stream is None:
             self.stream = torch.cuda.Stream(device=dev)
         s = self.stream
-        s.wait_stream(cur)                                   # the image is ready and every consumer of the previous outputs is done
+        if ready is None:
+            s.wait_stream(cur)                               # the image is ready and every consumer of the previous outputs is done
+        else:
+            s.wait_event(ready)
+            image.record_stream(s)                           # read on the branch stream, which no later caller work waits for
+        if after is not None:
+            s.wait_event(after)
         if precision == "bf16":
             self._refresh_bf16()                             # before its graphs are looked up
-        key = (tuple(image.shape), str(dev), precision)
+        key = (tuple(image.shape), str(dev), precision) + (() if slot is None else (int(slot),))
         st = self._graphs.get(key)
         with torch.cuda.stream(s):
             ev1, ev2 = torch.cuda.Event(), torch.cuda.Event()

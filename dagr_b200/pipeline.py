@@ -51,6 +51,14 @@ class PipelinedDetector:
     host never waits inside `submit`.  `result()` blocks on that step's event and returns the same list of dicts
     (`boxes`, `scores`, `labels`) as `DAGR.forward(...)[0]` (src/dagr/model/utils.py:104-108), as host tensors.
     At most two steps may be in flight (results live in two alternating pinned buffers).
+
+    Image-fusion models (--use_image) take `data.image` as `model(data)` does (the loader's u8 frames or formatted
+    floats, in the model's image_precision).  Their forwards run on a stream of the detector that waits for the caller's
+    stream as of `submit`, and the image branch of step i+1 waits only for that point and for step i-1, the last reader
+    of the branch outputs of its hand-off slot (ImageBranch.run(slot=...)): it runs next to the event-level kernels, the
+    coarse stack and the NMS of step i.  The coarse stack with its image sampling replays as one CUDA graph per slot.
+    The caller's stream waits for the points where the batch has been read.  The detections are those of `model(data)`
+    on the same batch, bit for bit.  --no_events models have no event path to pipeline and are refused.
     """
 
     class Handle:
@@ -70,15 +78,59 @@ class PipelinedDetector:
         self.engine = model.engine
         self._host = {}
         self._k = 0
+        self._stream = None                  # image fusion: the stream the forwards run on
+
+    def _check(self, data):
+        """the argument checks of submit(), before any device work."""
+        m = self.model
+        if not m.backbone.use_image:
+            return
+        if m.head.no_events:
+            raise ValueError("PipelinedDetector pipelines the event path; a --no_events model has none (use model(data))")
+        img = getattr(data, "image", None)
+        if not torch.is_tensor(img):
+            raise ValueError("an image-fusion model needs data.image: u8 or float frames [B, 3, H, W]")
+        if img.dim() != 4 or img.shape[1] != 3 or not (img.dtype == torch.uint8 or img.dtype.is_floating_point):
+            raise ValueError(f"data.image {tuple(img.shape)} {img.dtype}: expected u8 or float frames [B, 3, H, W]")
+        B = int(getattr(data, "num_graphs", 0) or 0)
+        if B and int(img.shape[0]) != B:
+            raise ValueError(f"data.image holds {int(img.shape[0])} frames for a batch of {B} samples")
+        if img.device != data.pos.device:
+            raise ValueError(f"data.image is on {img.device}, the events on {data.pos.device}")
+        if m.keep_stream:
+            raise ValueError("PipelinedDetector runs reset=True forwards of independent batches; keep_stream=True starts an "
+                             "incremental stream (use model(data) or AsyncDAGR)")
 
     def submit(self, data, filtering=True) -> "PipelinedDetector.Handle":
+        self._check(data)
+        if not self.model.backbone.use_image:
+            return self._step(data, filtering)
+        # image fusion: the forward runs on a stream of the detector, so that the caller's stream holds nothing of it.  The
+        # image branch then waits for the caller's stream as of this call (where the batch is valid) and for the last reader
+        # of its slot, not for the event-level kernels of the batch before; the caller's stream waits for the points where
+        # the batch has been read, so it may write the batch's tensors again, as after a synchronous call
+        cur = torch.cuda.current_stream(data.pos.device)
+        if self._stream is None:
+            self._stream = torch.cuda.Stream(device=data.pos.device)
+        ready = torch.cuda.Event()
+        ready.record(cur)
+        self._stream.wait_event(ready)
+        read = []
+        with torch.cuda.stream(self._stream):
+            h = self._step(data, filtering, frame_ready=ready, inputs_read=read)
+        for v in data.__dict__.values():                    # read on the detector's stream, which the caller never waits for
+            if torch.is_tensor(v) and v.is_cuda:
+                v.record_stream(self._stream)
+        for ev in read:
+            cur.wait_event(ev)
+        return h
+
+    def _step(self, data, filtering, **kw) -> "PipelinedDetector.Handle":
         m, eng = self.model, self.engine
-        if m.backbone.use_image:
-            raise NotImplementedError("PipelinedDetector drives the events-only model; use model(data) with images")
         prev = eng.overlap
         eng.overlap = True
         try:
-            dec = m.forward_decoded(data, reset=True)
+            dec = m.forward_decoded(data, reset=True, **kw)
             det, ndet = eng.postprocess(dec, m.conf_threshold, m.nms_threshold, m.width, m.height, filtering=filtering)
             k = self._k & 1
             self._k += 1
