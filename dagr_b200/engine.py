@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+from dataclasses import dataclass
 from typing import Dict, List, Optional
 
 import torch
@@ -55,6 +56,123 @@ def _image_format(image_feats) -> torch.dtype:
     if dt == torch.bfloat16 and not all(f.dim() == 4 and f.is_contiguous(memory_format=torch.channels_last) for f in image_feats):
         raise ValueError("bfloat16 image_feats must be [B, C, h, w] tensors in channels_last memory format (NHWC)")
     return dt
+
+
+@dataclass(frozen=True, eq=False)
+class _Taps:
+    """the image taps of one forward_events call and the entry points that sample them.  Each image kernel's entry point is
+    chosen here: first the format (fp32 NCHW, or bf16 channels_last: the _bf16 forms), then the mode: a plane per sample
+    (the _planes forms), x0 bounded by the live total (_live), the running voxel max of an incremental call (_inc), or
+    plain.  Call sites pass the arguments every form takes."""
+    feats: list                        # the five taps [B or P, C, h, w]: conv1 (x0), layer1 (voxel max), layer2..4 (coarse)
+    outs: Optional[dict]               # CNN head maps: "{cls,reg,obj}_output" -> one fp32 [B or P, C, ny, nx] per scale
+    fmt: torch.dtype                   # _image_format(feats)
+    planes: Optional[tuple] = None     # (plane table int32 on the device, stride): sample b reads plane table[b * stride]
+    live: bool = False                 # ring sorts: N is the capacity, x0 is bounded by the live total start[NK]
+    state: object = None               # the StreamState of an incremental call (voxel max into state.imgmax)
+    min_idx: int = 0
+
+    @property
+    def sfx(self):
+        return "_bf16" if self.fmt == torch.bfloat16 else ""
+
+    def _plane_args(self, t):
+        return (int(t.shape[0]), _lib.ptr(self.planes[0]), int(self.planes[1])) if self.planes is not None else ()
+
+    def x0(self, eng, g, N, start, xyb, feat_s, x0, st):
+        """the conv1 tap at every node; incremental steps resample every node too: a new node's conv reads the x0 rows of
+        its older neighbours."""
+        f = self.feats[0]
+        img = (_lib.ptr(f),) + ((int(f.shape[1]),) if self.sfx else ()) + (int(f.shape[2]), int(f.shape[3]))  # bf16 takes C
+        if self.planes is not None:
+            form, args = "_planes", (start, xyb, feat_s, *img, *self._plane_args(f))
+        elif self.live:
+            # N = ring capacity: positions behind the live total hold stale xyb words, so the launch is bounded by the
+            # total the sort wrote (start[NK]); the synchronous path keeps the unbounded form (N is the live count there)
+            form, args = "_live", (start, xyb, feat_s, *img)
+        else:
+            form, args = "", (xyb, feat_s, *img)
+        eng._run("l1_x0_image", getattr(eng.lib, "dagr_l1_x0_image" + form + self.sfx), g, N, *args, x0, st)
+
+    def voxel_max(self, eng, g, N, start, xyb, ti, xg, ldx, c0, pool_mean, st):
+        """the per-voxel max of the layer1 tap's samples into xg[:, c0:] (sampling_skip before pool1, net.py:128-131)."""
+        f = self.feats[1]
+        img = (_lib.ptr(f), int(f.shape[1]), int(f.shape[2]), int(f.shape[3]))
+        if self.state is not None:            # running per-voxel max of the samples, new events only
+            label, form, args = "voxel_sample_max_inc", "_inc", (ti, *img, self.min_idx, _lib.ptr(self.state.imgmax))
+        else:
+            label, form, args = "voxel_sample_max", "_planes" if self.planes is not None else "", (*img, *self._plane_args(f))
+        eng._run(label, getattr(eng.lib, "dagr_voxel_sample_max" + form + self.sfx), g, N, start, xyb, *args, xg, ldx, c0,
+                 pool_mean, st)
+
+    def sample_features(self, eng, k, posx, posy, bidx, n, width, height, out, ldo, c0, st):
+        """tap k sampled at n grid nodes into out[:, c0:]."""
+        f = self.feats[k]
+        form = "_planes" if self.planes is not None else ""
+        eng._run("sample_features", getattr(eng.lib, "dagr_sample_features" + form + self.sfx), _lib.ptr(f),
+                 *(self._plane_args(f) or (int(f.shape[0]),)), int(f.shape[1]), int(f.shape[2]), int(f.shape[3]), posx, posy,
+                 bidx, n, width, height, out, ldo, c0, st)
+
+    def head_maps(self, k):
+        """-> (form, maps, plane arguments) of dagr_head_finish[form] at scale k: the CNN head maps added to the graph
+        head's cls / reg / obj outputs (fp32 in every format; None without maps)."""
+        adds = {n: None if self.outs is None else self.outs[n + "_output"][k].float().contiguous() for n in ("cls", "reg", "obj")}
+        return ("_planes" if self.planes is not None else ""), adds, self._plane_args(adds["cls"])
+
+
+def _overlaps(overlap: bool, profiling: bool, use_graphs: bool) -> bool:
+    """whether a plain forward runs its coarse stack + NMS on the side stream (Engine.overlap): only with graphs on and
+    per-op timing off."""
+    return bool(overlap and not profiling and use_graphs)
+
+
+@dataclass(frozen=True, eq=False)
+class _Mode:
+    """how one forward_events call runs (resolve_mode)."""
+    sort: str                          # "batch" (dagr_graph_sort), "ring" (one ring) or "rings" (S rings of N / S slots)
+    ring: Optional[torch.Tensor]       # the ring control block: int32[8], or int32[S+1][8] for S rings
+    streams: int                       # S of "rings", else 1
+    state: object                      # the StreamState of an incremental call, else None
+    min_idx: int                       # incremental: the arrival indices below it were processed by earlier steps
+    taps: Optional[_Taps]              # image fusion
+    overlap: bool                      # coarse stack + NMS on the side stream, double-buffered hand-off
+    capture: bool                      # coarse stack replayed as one captured CUDA graph
+    fixed: bool                        # rings or incremental: "auto" queues no voxels for the dense kernels (_dense_policy)
+
+
+def resolve_mode(B: int, N: int, image_feats=None, image_outs=None, stream_state=None, n_old: int = 0, ring=None,
+                 ring_streams=None, image_planes=None, *, overlap=False, profiling=False, use_graphs=True,
+                 keep_node_features=False) -> _Mode:
+    """the mode of one Engine.forward_events call, from its arguments and the engine's switches.  Host only, no CUDA: every
+    refusal comes before any device work."""
+    if ring_streams is not None and (ring is None or int(ring_streams) != int(B) or N % int(ring_streams)):
+        raise ValueError(f"ring_streams={ring_streams} needs a ring control block, B == ring_streams and N a multiple of it "
+                         f"(B={B}, N={N})")
+    if stream_state is not None and ring is not None:
+        raise ValueError("stream_state with a ring: an incremental call appends to one event history, whose arrival indices "
+                         "a ring shifts with every eviction")
+    if image_planes is not None:
+        if image_feats is None or image_outs is None:
+            raise ValueError("image_planes selects a frame per sample: it needs image_feats and image_outs")
+        if keep_node_features:
+            raise ValueError("keep_node_features: the dense head maps (dagr_grid_to_dense) have no plane mode")
+        if stream_state is not None:
+            raise ValueError("stream_state with image_planes: the running voxel max (dagr_voxel_sample_max_inc) has no plane "
+                             "mode")
+    min_idx = int(n_old) if stream_state is not None else 0
+    taps = None
+    if image_feats is not None:
+        # the taps' format picks the fp32 or the bf16 sampling entry points
+        taps = _Taps(image_feats, image_outs, _image_format(image_feats),
+                     None if image_planes is None else (image_planes[0], int(image_planes[1])), ring is not None,
+                     stream_state, min_idx)
+    ov = _overlaps(overlap, profiling, use_graphs) and ring is None and stream_state is None and image_planes is None
+    return _Mode(sort="batch" if ring is None else "ring" if ring_streams is None else "rings", ring=ring,
+                 streams=1 if ring_streams is None else int(ring_streams), state=stream_state, min_idx=min_idx, taps=taps,
+                 overlap=ov,
+                 # with image fusion only the overlapped step is captured (the serial hybrid forward stays eager)
+                 capture=bool(use_graphs and not profiling and ring is None and (ov or taps is None)),
+                 fixed=ring is not None or stream_state is not None)
 
 
 class _ConvPack:
@@ -385,7 +503,7 @@ class Engine:
     def next_slot(self):
         """-> (slot, event) of the next plain forward when it overlaps (overlap on, no per-op timing, graphs on), else
         None: the hand-off slot it will use and the event of the last step that read that slot (None if none did)."""
-        if not (self.overlap and self.prof is None and self.use_graphs):
+        if not _overlaps(self.overlap, self.prof is not None, self.use_graphs):
             return None
         return self._slot, self._done[self._slot]
 
@@ -518,10 +636,12 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def _append_image(self, geom, lv, gs, o, feat, ws, st, dev, planes=None):
-        """sampling_skip on a voxel grid (net.py:141-142 etc.): [o | bilinear samples of `feat` at the nodes].
-        planes = (plane table, stride): `feat` is a plane array and sample b samples its plane alone (forward_events)."""
-        cells, Cc, Cf = gs.cells, o.shape[1], int(feat.shape[1])
+    def _append_image(self, geom, lv, gs, o, taps: _Taps, k, ws, st, dev):
+        """sampling_skip on a voxel grid (net.py:141-142 etc.): [o | bilinear samples of tap k at the nodes]; o alone for an
+        events-only forward."""
+        if taps is None:
+            return o
+        cells, Cc, Cf = gs.cells, o.shape[1], int(taps.feats[k].shape[1])
         xcat = self._buf(ws, f"xcat{lv}", (cells, Cc + Cf), torch.float32, dev)
         xcat[:, :Cc] = o
         pxy = gs.pxy[:cells].long()
@@ -531,15 +651,8 @@ class Engine:
         if key not in ws:
             per = geom.levels[lv].nx * geom.levels[lv].ny
             ws[key] = (torch.arange(cells, device=dev) // per).int()
-        sfx = "_bf16" if feat.dtype == torch.bfloat16 else ""           # the map's format (_image_format)
-        if planes is not None:
-            self._run("sample_features", getattr(self.lib, "dagr_sample_features_planes" + sfx), _lib.ptr(feat), int(feat.shape[0]), _lib.ptr(planes[0]),
-                      int(planes[1]), Cf, int(feat.shape[2]), int(feat.shape[3]), _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells,
-                      geom.W, geom.H, _lib.ptr(xcat), Cc + Cf, Cc, st)
-            return xcat
-        self._run("sample_features", getattr(self.lib, "dagr_sample_features" + sfx), _lib.ptr(feat), int(feat.shape[0]), Cf, int(feat.shape[2]),
-                  int(feat.shape[3]), _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells, geom.W, geom.H, _lib.ptr(xcat),
-                  Cc + Cf, Cc, st)
+        taps.sample_features(self, k, _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells, geom.W, geom.H, _lib.ptr(xcat),
+                             Cc + Cf, Cc, st)
         return xcat
 
     @torch.no_grad()
@@ -557,155 +670,113 @@ class Engine:
         [P, C, h, w] and sample b reads plane table[b * stride] alone, sampled as a batch of one (the *_planes kernels), so
         each sample gets the bits of a B = 1 forward with its own frame.  The table may be device data written inside the
         step (the stage header, dagr_b200.streaming.FusionMultiStreamDetector).  A plain batch (ring None) takes it too: the
-        windows of one recording, each with its own frame (dagr_b200.sequence)."""
+        windows of one recording, each with its own frame (dagr_b200.sequence).
+        stream_state, n_old: incremental step (dagr_b200.asynchronous); neither a ring nor image_planes takes it."""
         for n, t in (("batch", batch_i32), ("pos", pos_i32), ("x", feat)):
             _lib.require_cuda(t, n)
         dev = pos_i32.device
         N = int(batch_i32.shape[0])
-        if ring_streams is not None and (ring is None or int(ring_streams) != int(B) or N % int(ring_streams)):
-            raise ValueError(f"ring_streams={ring_streams} needs a ring control block, B == ring_streams and N a multiple of it "
-                             f"(B={B}, N={N})")
-        if image_planes is not None:
-            if image_feats is None or image_outs is None:
-                raise ValueError("image_planes selects a frame per sample: it needs image_feats and image_outs")
-            if self.keep_node_features:
-                raise ValueError("keep_node_features: the dense head maps (dagr_grid_to_dense) have no plane mode")
-            plane_tab, plane_stride = image_planes
-        # the taps' format picks the fp32 or the bf16 sampling entry points (checked before any device work)
-        sfx = "_bf16" if image_feats is not None and _image_format(image_feats) == torch.bfloat16 else ""
+        mode = resolve_mode(B, N, image_feats, image_outs, stream_state, n_old, ring, ring_streams, image_planes,
+                            overlap=self.overlap, profiling=self.prof is not None, use_graphs=self.use_graphs,
+                            keep_node_features=self.keep_node_features)
         geom = self.geometry(W, H, B, dev)
         pk = self.pack(geom, dev)
-        ws = self.workspace(geom, N, dev)
-        ov = bool(self.overlap and stream_state is None and image_planes is None and self.prof is None and self.use_graphs
-                  and ring is None)
-        slot = 0
-        if ov:
-            slot, self._slot = self._slot, self._slot ^ 1
-            if self._cstream is None:
-                # high priority: the small coarse kernels take SM slots as soon as CTAs of the big event-level kernels retire
-                self._cstream = torch.cuda.Stream(device=dev, priority=-1)
-            if self._done[slot] is not None:                 # the coarse stack that last read this slot's hand-off buffers
-                torch.cuda.current_stream().wait_event(self._done[slot])
-        else:
-            self.join()
-        ws = self._slot_view(ws, slot, geom, dev)
-        st = _lib.stream_ptr()
-        lib = self.lib
-        g = C.byref(geom.c_geom)
-        model = self.model
-        kto = bool(getattr(model.args, "keep_temporal_ordering", False))
-
-        ws["zero_buf"].zero_()
-        nbr, off = ws["nbr"], ws["off"]
-        cellmask = self._zs(ws, "cellmask", torch.int32)
-        min_idx, persist = 0, None
+        base = self.workspace(geom, N, dev)
+        slot = self._take_slot(mode, dev)
+        ws = self._slot_view(base, slot, geom, dev)
         if stream_state is not None:
-            # incremental step: the first n_old arrival indices were processed before; only newer events get
-            # their edges / activations computed (the causal graph never changes an old node's inputs).  With image fusion
-            # the frame is the same for every step between two re-seeds (dagr_b200.asynchronous)
             stream_state.ensure(geom, N, dev, img_channels=int(image_feats[1].shape[1]) if image_feats is not None else 0)
-            cellmask, persist, min_idx = stream_state.cellmask, stream_state.voxmax, int(n_old)
+        kto = bool(getattr(self.model.args, "keep_temporal_ordering", False))
+        g1, x1 = self._event_level(mode, geom, pk, ws, N, batch_i32, pos_i32, feat, image_event, kto)
+        out, grids, inter, dense_all = self._coarse_stack(mode, slot, geom, pk, ws, g1, B, kto, image_event)
+        self.last = dict(geom=geom, ws=ws, N=N, grids=list(grids), inter=inter, dense=dense_all, x1=x1)
+        return out
+
+    def _take_slot(self, mode: _Mode, dev) -> int:
+        """the hand-off slot of this forward.  An overlapped forward alternates between two and first waits for the last
+        coarse stack that read its slot's buffers; a serial one takes slot 0 after every coarse stack in flight."""
+        if not mode.overlap:
+            self.join()
+            return 0
+        slot, self._slot = self._slot, self._slot ^ 1
+        if self._cstream is None:
+            # high priority: the small coarse kernels take SM slots as soon as CTAs of the big event-level kernels retire
+            self._cstream = torch.cuda.Stream(device=dev, priority=-1)
+        if self._done[slot] is not None:
+            torch.cuda.current_stream().wait_event(self._done[slot])
+        return slot
+
+    def _cellmask(self, mode: _Mode, ws):
+        """the in-edge mask of the pool1 voxels: an incremental call's running mask, else this forward's zeroed one."""
+        return mode.state.cellmask if mode.state is not None else self._zs(ws, "cellmask", torch.int32)
+
+    def _event_level(self, mode: _Mode, geom, pk, ws, N, batch_i32, pos_i32, feat, image_event, kto):
+        """graph sort -> adjacency + conv_a -> conv_b + pool1 into grid level 0, with the image samples of a hybrid model.
+        -> (level-0 grid, the per-event conv_b activations when keep_node_features, else None)"""
+        lib, g, st, dev = self.lib, C.byref(geom.c_geom), _lib.stream_ptr(), pos_i32.device
+        taps, state, min_idx = mode.taps, mode.state, mode.min_idx
+        ws["zero_buf"].zero_()
+        start, perm, ti, xyb, feat_s, nbr, off, xa = (_lib.ptr(ws[k])
+                                                      for k in ("start", "perm", "ti", "xyb", "feat_s", "nbr", "off", "xa"))
+        cellmask = self._cellmask(mode, ws)
         flags = self._zs(ws, "flags", torch.int32)
         wl_hdr = self._zs(ws, "wl_hdr", torch.int32)
-        defer = self._dense_policy(ws, wl_hdr, ring is not None or stream_state is not None)
-        # ---- event level ---------------------------------------------------------------------
-        if ring is not None and ring_streams is not None:
-            self._run("graph_sort", lib.dagr_graph_sort_rings, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), N // ring_streams,
-                      int(ring_streams), _lib.ptr(ring), _lib.ptr(ws["key"]), _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]),
-                      _lib.ptr(ws["blocksums"]), _lib.ptr(ws["start"]), _lib.ptr(ws["perm"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), _lib.ptr(flags), st)
-        elif ring is not None:
-            self._run("graph_sort", lib.dagr_graph_sort_ring, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), N, _lib.ptr(ring),
-                      _lib.ptr(ws["key"]), _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]), _lib.ptr(ws["blocksums"]), _lib.ptr(ws["start"]),
-                      _lib.ptr(ws["perm"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]), _lib.ptr(flags), st)
+        defer = self._dense_policy(ws, wl_hdr, mode.fixed)
+        if mode.sort == "rings":
+            fn, size = lib.dagr_graph_sort_rings, (N // mode.streams, mode.streams, _lib.ptr(mode.ring))
+        elif mode.sort == "ring":
+            fn, size = lib.dagr_graph_sort_ring, (N, _lib.ptr(mode.ring))
         else:
-            self._run("graph_sort", lib.dagr_graph_sort, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), N, _lib.ptr(ws["key"]),
-                      _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]), _lib.ptr(ws["blocksums"]),
-                      _lib.ptr(ws["start"]), _lib.ptr(ws["perm"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), _lib.ptr(flags), st)
-        use_image = image_feats is not None
-        if use_image:
-            if stream_state is not None and min_idx > 0:
-                self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
-                          _lib.ptr(stream_state.xa_arr), 0, st)
-            # adjacency + the (polarity, x, y) part of conv_block1.conv_block1, which runs on [polarity, 16 image samples, x, y]
-            # (net.py:117-126); the image channels follow in dagr_l1_conv_a_image_tc
-            self._run("l1_build", lib.dagr_l1_build_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), C.byref(pk["l1a_img"]), _lib.ptr(pk["l1a_img_wfrag"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr), _lib.ptr(off),
-                      _lib.ptr(cellmask), _lib.ptr(ws["xa"]), _lib.ptr(wl_hdr), _lib.ptr(self._zs(ws, "wl_build", torch.int32)), defer[0], st)
+            fn, size = lib.dagr_graph_sort, (N,)
+        self._run("graph_sort", fn, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), *size, _lib.ptr(ws["key"]),
+                  _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]), _lib.ptr(ws["blocksums"]), start, perm, ti, xyb, feat_s,
+                  _lib.ptr(flags), st)
+        if min_idx > 0:
+            # incremental step: the first n_old arrival indices were processed before; only newer events get their edges /
+            # activations computed (the causal graph never changes an old node's inputs), the older xa rows are gathered.
+            # With image fusion the frame is the same for every step between two re-seeds (dagr_b200.asynchronous)
+            self._run("xa_gather", lib.dagr_xa_permute, N, perm, min_idx, xa, _lib.ptr(state.xa_arr), 0, st)
+        # adjacency + conv_block1.conv_block1.  With image fusion the layer runs on [polarity, 16 image samples, x, y]
+        # (net.py:117-126): this is its (polarity, x, y) part, the image channels follow in the conv_a image kernel
+        l1a = "l1a" if taps is None else "l1a_img"
+        self._run("l1_build", lib.dagr_l1_build_tc, g, N, start, ti, xyb, feat_s, C.byref(pk[l1a]), _lib.ptr(pk[l1a + "_wfrag"]),
+                  _lib.ptr(flags), min_idx, nbr, off, _lib.ptr(cellmask), xa, _lib.ptr(wl_hdr),
+                  _lib.ptr(self._zs(ws, "wl_build", torch.int32)), defer[0], st)
+        skipv = None
+        if taps is not None:
             if image_event is not None:                       # stage 1 of the image branch ran on a side stream next to sort + probe
                 torch.cuda.current_stream().wait_event(image_event[0])
-            f0 = image_feats[0]
-            c0w = (int(f0.shape[1]),) if sfx else ()                  # the bf16 forms take the tap's channel count
             x0 = self._buf(ws, "x0img", (2 * max(N, 1) * 8,), torch.float32, dev)
             skipv = self._buf(ws, "skipv", (max(N, 1), 16), torch.float32, dev)
-            if image_planes is not None:
-                self._run("l1_x0_image", getattr(lib, "dagr_l1_x0_image_planes" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                          _lib.ptr(ws["feat_s"]), _lib.ptr(f0), *c0w, int(f0.shape[2]), int(f0.shape[3]), int(f0.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
-                          _lib.ptr(x0), st)
-            elif ring is not None:
-                # N = ring capacity: positions behind the live total hold stale xyb words, so the launch is bounded by the
-                # total the sort wrote (start[NK]); the synchronous path keeps the unbounded form (N is the live count there)
-                self._run("l1_x0_image", getattr(lib, "dagr_l1_x0_image_live" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                          _lib.ptr(ws["feat_s"]), _lib.ptr(f0), *c0w, int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
-            else:
-                # incremental steps resample every node too: a new node's conv reads the x0 rows of its older neighbours
-                self._run("l1_x0_image", getattr(lib, "dagr_l1_x0_image" + sfx), g, N, _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
-                          _lib.ptr(f0), *c0w, int(f0.shape[2]), int(f0.shape[3]), _lib.ptr(x0), st)
-            if stream_state is not None:
+            taps.x0(self, g, N, start, xyb, feat_s, _lib.ptr(x0), st)
+            wl = (_lib.ptr(wl_hdr[2:]), _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
+            if state is not None:
                 # only the new nodes are convolved; the xa rows of the older ones are final and stay as gathered
-                self._run("l1_conv_a_image_inc", lib.dagr_l1_conv_a_image_inc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                          _lib.ptr(ws["ti"]), _lib.ptr(ws["feat_s"]), _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off), C.byref(pk["l1img"]),
-                          _lib.ptr(pk["l1img_wfrag"]), min_idx, _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
-                          _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
-                self._run("xa_scatter", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
-                          _lib.ptr(stream_state.xa_arr), 1, st)
+                self._run("l1_conv_a_image_inc", lib.dagr_l1_conv_a_image_inc, g, N, start, xyb, ti, feat_s, _lib.ptr(x0), nbr, off,
+                          C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), min_idx, xa, _lib.ptr(skipv), *wl)
             else:
-                self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(ws["feat_s"]),
-                          _lib.ptr(x0), _lib.ptr(nbr), _lib.ptr(off),
-                          C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), _lib.ptr(ws["xa"]), _lib.ptr(skipv), _lib.ptr(wl_hdr[2:]),
-                          _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
-        else:
-            if min_idx > 0:
-                self._run("xa_gather", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
-                          _lib.ptr(stream_state.xa_arr), 0, st)
-            self._run("l1_build", lib.dagr_l1_build_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["ti"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["feat_s"]), C.byref(pk["l1a"]), _lib.ptr(pk["l1a_wfrag"]), _lib.ptr(flags), min_idx, _lib.ptr(nbr),
-                      _lib.ptr(off), _lib.ptr(cellmask), _lib.ptr(ws["xa"]), _lib.ptr(wl_hdr), _lib.ptr(self._zs(ws, "wl_build", torch.int32)),
-                      defer[0], st)
-            if stream_state is not None:
-                self._run("xa_scatter", lib.dagr_xa_permute, N, _lib.ptr(ws["perm"]), min_idx, _lib.ptr(ws["xa"]),
-                          _lib.ptr(stream_state.xa_arr), 1, st)
+                self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, start, xyb, feat_s, _lib.ptr(x0), nbr, off,
+                          C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), xa, _lib.ptr(skipv), *wl)
+        if state is not None:
+            self._run("xa_scatter", lib.dagr_xa_permute, N, perm, min_idx, xa, _lib.ptr(state.xa_arr), 1, st)
         x1 = None
         if self.keep_node_features:
             if ws["x1"] is None or ws["x1"].shape[0] < ws["cap"]:
                 ws["x1"] = torch.empty((ws["cap"], 16), dtype=torch.float32, device=dev)
             x1 = ws["x1"]
         g1: GridState = ws["grids"][0]
-        c1 = 16 + (int(image_feats[1].shape[1]) if use_image else 0)
+        c1 = 16 + (int(taps.feats[1].shape[1]) if taps is not None else 0)
         g1.x = self._buf(ws, "gx0", (g1.cells, c1), torch.float32, dev)
-        self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel_tc, g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                  _lib.ptr(ws["ti"]), _lib.ptr(ws["feat_s"]), _lib.ptr(ws["xa"]), _lib.ptr(nbr), _lib.ptr(off),
-                  C.byref(pk["l1b"]), _lib.ptr(pk["l1b_wfrag"]), _lib.ptr(skipv) if use_image else None, min_idx, _lib.ptr(persist),
-                  _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy), _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1,
-                  _lib.ptr(wl_hdr[4:]), _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
+        self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel_tc, g, N, start, xyb, ti, feat_s, xa, nbr, off,
+                  C.byref(pk["l1b"]), _lib.ptr(pk["l1b_wfrag"]), _lib.ptr(skipv), min_idx,
+                  _lib.ptr(state.voxmax if state is not None else None), _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy),
+                  _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1, _lib.ptr(wl_hdr[4:]),
+                  _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
         self._dense_report(ws, wl_hdr)
-        if use_image and stream_state is not None:        # running per-voxel max of the samples, new events only
-            f1 = image_feats[1]
-            self._run("voxel_sample_max_inc", getattr(lib, "dagr_voxel_sample_max_inc" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]),
-                      _lib.ptr(ws["ti"]), _lib.ptr(f1), int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), min_idx,
-                      _lib.ptr(stream_state.imgmax), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
-        elif image_planes is not None:
-            f1 = image_feats[1]
-            self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max_planes" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
-                      int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), int(f1.shape[0]), _lib.ptr(plane_tab), int(plane_stride),
-                      _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
-        elif use_image:                                   # sampling_skip before pool1 (net.py:128-131)
-            f1 = image_feats[1]
-            self._run("voxel_sample_max", getattr(lib, "dagr_voxel_sample_max" + sfx), g, N, _lib.ptr(ws["start"]), _lib.ptr(ws["xyb"]), _lib.ptr(f1),
-                      int(f1.shape[1]), int(f1.shape[2]), int(f1.shape[3]), _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
+        if taps is not None:
+            taps.voxel_max(self, g, N, start, xyb, ti, _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
         g1.mask = cellmask[:g1.cells]
-        if kto and stream_state is not None:
+        if kto and state is not None:
             # the persistent stream mask only ever gains edges; the temporal filter (pooling.py:69-72) depends on the CURRENT
             # t_max of both voxels, so it must work on a per-step copy or edges dropped once could never come back
             step_mask = self._zs(ws, "cellmask", torch.int32)
@@ -714,143 +785,140 @@ class Engine:
         if kto:
             self._run("temporal_filter", lib.dagr_grid_temporal_filter, C.byref(geom.levels[0].grid), _lib.ptr(g1.cnt), _lib.ptr(g1.tmax),
                                                      _lib.ptr(g1.mask), st)
-        def coarse(st, image_wait=True):
-            # ---- coarse levels -------------------------------------------------------------------
-            aggr_cfg = 0 if getattr(model.args, "pooling_aggr", "max") == "max" else 1
-            lay = pk["layers"]
-            inter = {}
-            def cat_img(lv, gs, o, k):
-                return self._append_image(geom, lv, gs, o, image_feats[k], ws, st, dev, image_planes) if use_image else o
+        return g1, x1
 
-            _, _, o2 = self._layer(geom, 0, g1, lay[0], ws, "layer2", st, dev)
-            if use_image and image_event is not None and image_wait:   # layer2..4 taps + CNN head maps (image branch stage 2)
-                torch.cuda.current_stream().wait_event(image_event[1])
-            g2 = self._pool(geom, 0, g1, cat_img(0, g1, o2, 2), aggr_cfg, ws, st, dev, kto)
-            _, _, o3 = self._layer(geom, 1, g2, lay[1], ws, "layer3", st, dev)
-            g3 = self._pool(geom, 1, g2, cat_img(1, g2, o3, 3), aggr_cfg, ws, st, dev, kto)
-            _, _, o4 = self._layer(geom, 2, g3, lay[2], ws, "layer4", st, dev)           # out3
-            nc = model.backbone.num_classes
-            nscale = model.head.num_scales
-            A = sum(geom.levels[lv].nx * geom.levels[lv].ny for lv in ((2, 3) if nscale == 2 else (3,)))
-            out = self._buf(ws, "decoded", (B, A, 5 + nc), torch.float32, dev)
-            dense_all = [None] * nscale
-
-            def head_scale(k, lv, gs, xo, a0, st):
-                """GNNHead.process_feature + collect_outputs + decode_outputs of one scale (dagr.py:179-312)."""
-                hp = pk["heads"][k]
-                level = geom.levels[lv]
-                cells = gs.cells
-                nm = f"head{k}"
-                stem = self._buf(ws, nm + "_stem", (cells, hp["stem"].cout), torch.float32, dev)
-                self._grid_conv(geom, lv, gs, xo, hp["stem"], None, stem, st)
-                Cf = hp["cls_conv"].cout
-                cr = self._buf(ws, nm + "_cr", (cells, 2 * Cf), torch.float32, dev)          # [cls_feat | reg_feat]
-                self._grid_conv(geom, lv, gs, stem, hp["clsreg_conv"], None, cr, st)
-                ocls = self._buf(ws, nm + "_cls", (cells, nc), torch.float32, dev)
-                self._grid_conv(geom, lv, gs, cr, hp["cls_pred"], None, ocls, st, ldin=2 * Cf)
-                oro = self._buf(ws, nm + "_regobj", (cells, 5), torch.float32, dev)         # [reg(4) | obj(1)]
-                self._grid_conv(geom, lv, gs, cr[:, Cf:], hp["regobj_pred"], None, oro, st, ldin=2 * Cf)
-                adds = {}
-                for name in ("cls", "reg", "obj"):
-                    adds[name] = image_outs[name + "_output"][k].float().contiguous() if image_outs is not None else None
-                stride = model.backbone.strides[k]
-                if image_planes is not None:
-                    self._run("head_finish", lib.dagr_head_finish_planes, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(ocls), nc,
-                              _lib.ptr(oro), 5, _lib.ptr(adds["cls"]), _lib.ptr(adds["reg"]), _lib.ptr(adds["obj"]), nc, int(stride), a0, A,
-                              int(adds["cls"].shape[0]), _lib.ptr(plane_tab), int(plane_stride), _lib.ptr(out), st)
-                    dense_all[k] = {}
-                    return
-                self._run("head_finish", lib.dagr_head_finish, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(ocls), nc, _lib.ptr(oro), 5,
-                          _lib.ptr(adds["cls"]), _lib.ptr(adds["reg"]), _lib.ptr(adds["obj"]), nc, int(stride), a0, A, _lib.ptr(out), st)
-                dense = {}
-                if self.keep_node_features:
-                    # parity / debugging: the dense [B,C,ny,nx] head maps of SplineConvToDense (spline_conv.py:80-107)
-                    for name, src, c0, cw, ld in (("cls", ocls, 0, nc, nc), ("reg", oro, 0, 4, 5), ("obj", oro, 4, 1, 5)):
-                        d = self._buf(ws, nm + "_d" + name, (B, cw, level.ny, level.nx), torch.float32, dev)
-                        self._run("to_dense", lib.dagr_grid_to_dense, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(src[:, c0:]), cw, ld,
-                                  _lib.ptr(adds[name]), _lib.ptr(d), st)
-                        dense[name] = d
-                dense_all[k] = dense
-
-            # The first head scale only needs layer4's output: it runs on a forked stream next to pool4 + layer5 + the second
-            # scale (all of them are single-wave kernels on <= B*140 voxels, so they share the GPU instead of queueing);
-            # fork / join through events is captured like any other dependency when this stack is replayed as a graph.
-            join_ev = None
-            if nscale == 2:
-                cur = torch.cuda.current_stream()
-                if self._fstream is None:
-                    self._fstream = torch.cuda.Stream(device=dev, priority=-1)
-                fork_ev = torch.cuda.Event()
-                fork_ev.record(cur)
-                with torch.cuda.stream(self._fstream):
-                    self._fstream.wait_event(fork_ev)
-                    head_scale(0, 2, g3, o4, 0, _lib.stream_ptr())
-                    join_ev = torch.cuda.Event()
-                    join_ev.record(self._fstream)
-            g4 = self._pool(geom, 2, g3, cat_img(2, g3, o4, 4), 1, ws, st, dev, kto)     # pool4 is always mean (net.py:96-97)
-            _, _, o5 = self._layer(geom, 3, g4, lay[3], ws, "layer5", st, dev)           # out4
-            inter.update(o2=o2, o3=o3, o4=o4, o5=o5)
-            a0 = geom.levels[2].nx * geom.levels[2].ny if nscale == 2 else 0
-            head_scale(nscale - 1, 3, g4, o5, a0, st)
-            if join_ev is not None:
-                torch.cuda.current_stream().wait_event(join_ev)
-            return out, [g1, g2, g3, g4], inter, dense_all
-
-        # The coarse stack is ~55 small, fixed-shape launches: replay it as ONE CUDA graph (captured on the second
-        # call with identical buffers; the event-level kernels stay eager because their grids depend on N).  With image
-        # fusion only the overlapped step is captured (the serial hybrid forward stays eager); its graph reads the taps and
-        # head maps at fixed addresses, so they and their format are part of the key.
-        gkey = (id(ws.base), slot, self._pack_gen, B, kto, cellmask.data_ptr(), bool(self.keep_node_features))
-        if use_image:
-            gkey += (sfx, tuple(t.data_ptr() for t in image_feats),
-                     tuple((k, tuple(t.data_ptr() for t in v)) for k, v in sorted((image_outs or {}).items())))
-
-        def run_coarse():
-            if self.use_graphs and self.prof is None and (ov or not use_image) and ring is None:
-                if use_image and image_event is not None:
-                    # a captured graph cannot wait for an event recorded outside it: the whole stack waits for stage 2
-                    torch.cuda.current_stream().wait_event(image_event[1])
-                cached = ws.get("graph")
-                if cached is not None and cached[0] == gkey:
-                    cached[1].replay()
-                    self.launches += cached[3]
-                    return cached[2]
-                l0 = self.launches
-                res = coarse(_lib.stream_ptr(), image_wait=False)        # eager: also allocates every pool buffer
-                nk = self.launches - l0
-                ws["graph_warm"] = ws.get("graph_warm", 0) + 1
-                if ws["graph_warm"] >= 2 and ws.get("graph_key") == gkey:
-                    torch.cuda.synchronize()
-                    gr = torch.cuda.CUDAGraph()
-                    # kernel nodes inherit the priority of the CAPTURE stream: capture on the high-priority side stream in
-                    # overlap mode so the small coarse kernels get SM slots while a big event-level kernel is resident
-                    with torch.cuda.graph(gr, stream=self._cstream if ov else None):
-                        res_c = coarse(_lib.stream_ptr(), image_wait=False)
-                    self.launches -= nk                                  # capture enqueues nothing
-                    ws["graph"] = (gkey, gr, res_c, nk)
-                ws["graph_key"] = gkey
-                return res
-            return coarse(st)
-
-        if ov:
-            if use_image:                                 # the caching allocator must not hand them out while the stack reads
-                for t in (*image_feats, *(t for v in (image_outs or {}).values() for t in v)):
-                    t.record_stream(self._cstream)
-            fine_done = torch.cuda.Event()
-            fine_done.record()
-            with torch.cuda.stream(self._cstream):
-                self._cstream.wait_event(fine_done)
-                out, grids, inter, dense_all = run_coarse()
-                ev = torch.cuda.Event()
-                ev.record()
-            self._done[slot] = ev
-            self._out_slot = {out.data_ptr(): slot}
-        else:
-            out, grids, inter, dense_all = run_coarse()
+    def _coarse_stack(self, mode: _Mode, slot, geom, pk, ws, g1, B, kto, image_event):
+        """the coarse levels and the head after the event level -> (decoded, grids, layer outputs, dense head maps).  Serial:
+        on the caller's stream.  Overlapped: on the side stream once the event level is done; the slot's done-event marks
+        the end of its reads, and the results are valid on result_stream()."""
+        args = (mode, slot, geom, pk, ws, g1, B, kto, image_event)
+        if not mode.overlap:
+            res = self._coarse_graph(*args)
             self._out_slot = {}
-        g1, g2, g3, g4 = grids
-        self.last = dict(geom=geom, ws=ws, N=N, grids=[g1, g2, g3, g4], inter=inter, dense=dense_all, x1=x1)
-        return out
+            return res
+        taps = mode.taps
+        if taps is not None:                              # the caching allocator must not hand them out while the stack reads
+            for t in (*taps.feats, *(t for v in (taps.outs or {}).values() for t in v)):
+                t.record_stream(self._cstream)
+        fine_done = torch.cuda.Event()
+        fine_done.record()
+        with torch.cuda.stream(self._cstream):
+            self._cstream.wait_event(fine_done)
+            res = self._coarse_graph(*args)
+            ev = torch.cuda.Event()
+            ev.record()
+        self._done[slot] = ev
+        self._out_slot = {res[0].data_ptr(): slot}
+        return res
+
+    def _coarse_graph(self, mode: _Mode, slot, geom, pk, ws, g1, B, kto, image_event):
+        """the coarse stack, eager or replayed.  It is ~55 small, fixed-shape launches: replay it as ONE CUDA graph (captured
+        on the second call with identical buffers; the event-level kernels stay eager because their grids depend on N).
+        With image fusion only the overlapped step is captured (the serial hybrid forward stays eager); its graph reads the
+        taps and head maps at fixed addresses, so they and their format are part of the key."""
+        args = (mode, geom, pk, ws, g1, B, kto)
+        taps = mode.taps
+        if not mode.capture:
+            return self._coarse(*args, _lib.stream_ptr(), None if image_event is None else image_event[1])
+        if image_event is not None:
+            # a captured graph cannot wait for an event recorded outside it: the whole stack waits for stage 2
+            torch.cuda.current_stream().wait_event(image_event[1])
+        gkey = (id(ws.base), slot, self._pack_gen, B, kto, self._cellmask(mode, ws).data_ptr(), bool(self.keep_node_features))
+        if taps is not None:
+            gkey += (taps.sfx, tuple(t.data_ptr() for t in taps.feats),
+                     tuple((k, tuple(t.data_ptr() for t in v)) for k, v in sorted((taps.outs or {}).items())))
+        cached = ws.get("graph")
+        if cached is not None and cached[0] == gkey:
+            cached[1].replay()
+            self.launches += cached[3]
+            return cached[2]
+        l0 = self.launches
+        res = self._coarse(*args, _lib.stream_ptr())                 # eager: also allocates every pool buffer
+        nk = self.launches - l0
+        ws["graph_warm"] = ws.get("graph_warm", 0) + 1
+        if ws["graph_warm"] >= 2 and ws.get("graph_key") == gkey:
+            torch.cuda.synchronize()
+            gr = torch.cuda.CUDAGraph()
+            # kernel nodes inherit the priority of the CAPTURE stream: capture on the high-priority side stream in
+            # overlap mode so the small coarse kernels get SM slots while a big event-level kernel is resident
+            with torch.cuda.graph(gr, stream=self._cstream if mode.overlap else None):
+                res_c = self._coarse(*args, _lib.stream_ptr())
+            self.launches -= nk                                      # capture enqueues nothing
+            ws["graph"] = (gkey, gr, res_c, nk)
+        ws["graph_key"] = gkey
+        return res
+
+    def _coarse(self, mode: _Mode, geom, pk, ws, g1, B, kto, st, stage2=None):
+        """layers 2..5 with their pooling and the head's scales.  stage2: the event on which the image branch's layer2..4
+        taps and CNN head maps are ready, waited for after layer2 (eager hybrid forwards)."""
+        taps, dev = mode.taps, g1.cnt.device
+        aggr = 0 if getattr(self.model.args, "pooling_aggr", "max") == "max" else 1
+        lay = pk["layers"]
+        _, _, o2 = self._layer(geom, 0, g1, lay[0], ws, "layer2", st, dev)
+        if stage2 is not None:
+            torch.cuda.current_stream().wait_event(stage2)
+        g2 = self._pool(geom, 0, g1, self._append_image(geom, 0, g1, o2, taps, 2, ws, st, dev), aggr, ws, st, dev, kto)
+        _, _, o3 = self._layer(geom, 1, g2, lay[1], ws, "layer3", st, dev)
+        g3 = self._pool(geom, 1, g2, self._append_image(geom, 1, g2, o3, taps, 3, ws, st, dev), aggr, ws, st, dev, kto)
+        _, _, o4 = self._layer(geom, 2, g3, lay[2], ws, "layer4", st, dev)           # out3
+        nscale = self.model.head.num_scales
+        A = sum(geom.levels[lv].nx * geom.levels[lv].ny for lv in ((2, 3) if nscale == 2 else (3,)))
+        out = self._buf(ws, "decoded", (B, A, 5 + self.model.backbone.num_classes), torch.float32, dev)
+        dense_all = [None] * nscale
+        # The first head scale only needs layer4's output: it runs on a forked stream next to pool4 + layer5 + the second
+        # scale (all of them are single-wave kernels on <= B*140 voxels, so they share the GPU instead of queueing);
+        # fork / join through events is captured like any other dependency when this stack is replayed as a graph.
+        join_ev = None
+        if nscale == 2:
+            cur = torch.cuda.current_stream()
+            if self._fstream is None:
+                self._fstream = torch.cuda.Stream(device=dev, priority=-1)
+            fork_ev = torch.cuda.Event()
+            fork_ev.record(cur)
+            with torch.cuda.stream(self._fstream):
+                self._fstream.wait_event(fork_ev)
+                dense_all[0] = self._head_scale(taps, geom, pk, ws, 0, 2, g3, o4, 0, A, B, out, _lib.stream_ptr())
+                join_ev = torch.cuda.Event()
+                join_ev.record(self._fstream)
+        # pool4 is always mean (net.py:96-97)
+        g4 = self._pool(geom, 2, g3, self._append_image(geom, 2, g3, o4, taps, 4, ws, st, dev), 1, ws, st, dev, kto)
+        _, _, o5 = self._layer(geom, 3, g4, lay[3], ws, "layer5", st, dev)           # out4
+        a0 = geom.levels[2].nx * geom.levels[2].ny if nscale == 2 else 0
+        dense_all[nscale - 1] = self._head_scale(taps, geom, pk, ws, nscale - 1, 3, g4, o5, a0, A, B, out, st)
+        if join_ev is not None:
+            torch.cuda.current_stream().wait_event(join_ev)
+        return out, [g1, g2, g3, g4], dict(o2=o2, o3=o3, o4=o4, o5=o5), dense_all
+
+    def _head_scale(self, taps: Optional[_Taps], geom, pk, ws, k, lv, gs: GridState, xo, a0, A, B, out, st):
+        """GNNHead.process_feature + collect_outputs + decode_outputs of one scale (dagr.py:179-312) into out[:, a0:].
+        -> the dense head maps {cls, reg, obj} of the scale when keep_node_features, else {}"""
+        lib, dev, nc = self.lib, gs.cnt.device, self.model.backbone.num_classes
+        hp = pk["heads"][k]
+        level = geom.levels[lv]
+        cells = gs.cells
+        nm = f"head{k}"
+        stem = self._buf(ws, nm + "_stem", (cells, hp["stem"].cout), torch.float32, dev)
+        self._grid_conv(geom, lv, gs, xo, hp["stem"], None, stem, st)
+        Cf = hp["cls_conv"].cout
+        cr = self._buf(ws, nm + "_cr", (cells, 2 * Cf), torch.float32, dev)          # [cls_feat | reg_feat]
+        self._grid_conv(geom, lv, gs, stem, hp["clsreg_conv"], None, cr, st)
+        ocls = self._buf(ws, nm + "_cls", (cells, nc), torch.float32, dev)
+        self._grid_conv(geom, lv, gs, cr, hp["cls_pred"], None, ocls, st, ldin=2 * Cf)
+        oro = self._buf(ws, nm + "_regobj", (cells, 5), torch.float32, dev)         # [reg(4) | obj(1)]
+        self._grid_conv(geom, lv, gs, cr[:, Cf:], hp["regobj_pred"], None, oro, st, ldin=2 * Cf)
+        form, adds, planes = taps.head_maps(k) if taps is not None else ("", dict.fromkeys(("cls", "reg", "obj")), ())
+        self._run("head_finish", getattr(lib, "dagr_head_finish" + form), C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(ocls), nc,
+                  _lib.ptr(oro), 5, _lib.ptr(adds["cls"]), _lib.ptr(adds["reg"]), _lib.ptr(adds["obj"]), nc,
+                  int(self.model.backbone.strides[k]), a0, A, *planes, _lib.ptr(out), st)
+        dense = {}
+        if self.keep_node_features:
+            # parity / debugging: the dense [B,C,ny,nx] head maps of SplineConvToDense (spline_conv.py:80-107)
+            for name, src, c0, cw, ld in (("cls", ocls, 0, nc, nc), ("reg", oro, 0, 4, 5), ("obj", oro, 4, 1, 5)):
+                d = self._buf(ws, nm + "_d" + name, (B, cw, level.ny, level.nx), torch.float32, dev)
+                self._run("to_dense", lib.dagr_grid_to_dense, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(src[:, c0:]), cw, ld,
+                          _lib.ptr(adds[name]), _lib.ptr(d), st)
+                dense[name] = d
+        return dense
 
     def xa_rows(self):
         """conv_block1.conv_block1 activations of the last forward as [N,16] rows in sorted order
