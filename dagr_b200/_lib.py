@@ -27,6 +27,32 @@ p = C.c_void_p
 i32 = C.c_int32
 i64 = C.c_int64
 f32 = C.c_float
+_Tensor = torch.Tensor
+_void_p = C.c_void_p.from_param
+
+
+class Dev:
+    """argument type of a device pointer (the header's convention: every pointer not named *_host).  A CUDA tensor passes
+    its data_ptr() and stays alive through the call; None passes NULL; raw addresses (int, c_void_p) pass unchanged.  A
+    tensor in host memory, pinned or not, is refused before the call: a kernel would fault on it or read it over PCIe."""
+
+    @staticmethod
+    def from_param(obj):
+        if isinstance(obj, _Tensor):
+            if not obj.is_cuda:
+                raise RuntimeError(f"a {obj.device} tensor where the library takes a device pointer")
+            return _void_p(obj.data_ptr())
+        return _void_p(obj)
+
+
+class Host:
+    """argument type of a *_host pointer: host memory (ctypes arrays and buffers), never a CUDA tensor."""
+
+    @staticmethod
+    def from_param(obj):
+        if getattr(obj, "is_cuda", False):
+            raise RuntimeError("a CUDA tensor where the library takes a host pointer")
+        return _void_p(obj)
 
 
 class Geom(C.Structure):
@@ -80,78 +106,91 @@ _SIGS = {
     "dagr_check_config": (C.c_int, [C.POINTER(Geom), i64, C.c_int, C.c_int, C.c_char_p]),
     "dagr_event_workspace_bytes": (C.c_int, [C.POINTER(Geom), i64, C.POINTER(EventWs)]),
     "dagr_pool_workspace_bytes": (C.c_int, [i64, C.c_int, C.POINTER(PoolWs)]),
-    "dagr_downsample_events": (C.c_int, [p, p, p, i64, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, p, p, p, p, p, p]),
-    "dagr_compact_events": (C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, p, p, p, p, p, p, p, p, p]),
-    "dagr_ingest_events": (C.c_int, [p, p, p, p, i64, C.c_int, C.c_int, C.c_int, C.c_int, i64, C.c_int, p, p, p, p, p, p, p, p, p]),
-    "dagr_window_bounds": (C.c_int, [p, i64, p, p, i64, p, p, p]),
-    "dagr_window_gather": (C.c_int, [p, p, p, p, i64, p, p, C.c_int, i64, C.c_int, i64, p, p, p, p, p]),
-    "dagr_stream_ingest": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int, p]),
-    "dagr_frame_preprocess": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, p]),
-    "dagr_denormalize_pos": (C.c_int, [p, i64, C.c_int, C.c_int, C.c_int, p, p]),
-    "dagr_prepare_events": (C.c_int, [p, p, p, C.c_int, i64, C.c_int, C.c_int, C.c_int, p, p, p, p]),
-    "dagr_graph_sort": (C.c_int, [C.POINTER(Geom), p, p, p, i64, p, p, p, p, p, p, p, p, p, p, p]),
-    "dagr_graph_sort_ring": (C.c_int, [C.POINTER(Geom), p, p, p, i64, p, p, p, p, p, p, p, p, p, p, p, p]),
-    "dagr_stream_push": (C.c_int, [p, p, p, p, p, i64, C.c_int, C.c_int, p]),
-    "dagr_stream_push_multi": (C.c_int, [p, p, p, p, p, i64, C.c_int, C.c_int, p]),
-    "dagr_graph_sort_rings": (C.c_int, [C.POINTER(Geom), p, p, p, i64, C.c_int, p, p, p, p, p, p, p, p, p, p, p, p]),
-    "dagr_l1_build": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.POINTER(L1AParams), p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
-    "dagr_l1a_tc_weights": (C.c_int, [C.POINTER(L1AParams), p]),
-    "dagr_l1_build_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.POINTER(L1AParams), p, p, C.c_int, p, p, p, p, p, p, C.c_int, p]),
-    "dagr_xa_permute": (C.c_int, [i64, p, C.c_int, p, p, C.c_int, p]),
-    "dagr_l1_x0_image": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, p, p]),
-    "dagr_l1_x0_image_live": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, p, p]),
-    "dagr_l1_x0_image_planes": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, p, p]),
-    "dagr_voxel_sample_max": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, C.c_int, C.c_int, p]),
-    "dagr_voxel_sample_max_planes": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p, C.c_int,
-                                               C.c_int, C.c_int, p]),
-    "dagr_graph_export": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, p, i64, p]),
-    "dagr_l1_tc_weights": (C.c_int, [p, p, C.c_int, p]),
-    "dagr_l1_conv_b_pool_voxel_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, C.POINTER(L1BParams), p, p, C.c_int, p, p, p, p, p, p, p, C.c_int, p, p, C.c_int, p]),
-    "dagr_l1_conv_a_image_tc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, C.POINTER(L1ImgParams), p, p, p, p, p, C.c_int, p]),
-    "dagr_l1_conv_a_image_inc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, p, p, p, C.POINTER(L1ImgParams), p, C.c_int, p, p, p, p,
-                                           C.c_int, p]),
-    "dagr_voxel_sample_max_inc": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int, C.c_int,
-                                            C.c_int, p]),
-    "dagr_grid_cat_pos": (C.c_int, [C.POINTER(Grid), p, p, p, C.c_int, p, p]),
-    "dagr_grid_conv": (C.c_int, [C.POINTER(Grid), p, p, p, p, C.c_int, C.c_int, C.c_int, p, p, p, p, p, p, C.c_int, f32, f32, p, p]),
+    "dagr_downsample_events": (C.c_int, [Dev, Dev, Dev, i64, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, Dev, Dev, Dev,
+                                         Dev, Dev, p]),
+    "dagr_compact_events": (C.c_int, [Dev, i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, p]),
+    "dagr_ingest_events": (C.c_int, [Dev, Dev, Dev, Dev, i64, C.c_int, C.c_int, C.c_int, C.c_int, i64, C.c_int, Dev, Dev, Dev, Dev, Dev,
+                                     Dev, Dev, Dev, p]),
+    "dagr_window_bounds": (C.c_int, [Dev, i64, Dev, Dev, i64, Dev, Dev, p]),
+    "dagr_window_gather": (C.c_int, [Dev, Dev, Dev, Dev, i64, Dev, Dev, C.c_int, i64, C.c_int, i64, Dev, Dev, Dev, Dev, p]),
+    "dagr_stream_ingest": (C.c_int, [Dev, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, C.c_int, p]),
+    "dagr_frame_preprocess": (C.c_int, [Dev, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, p]),
+    "dagr_denormalize_pos": (C.c_int, [Dev, i64, C.c_int, C.c_int, C.c_int, Dev, p]),
+    "dagr_prepare_events": (C.c_int, [Dev, Dev, Dev, C.c_int, i64, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, p]),
+    "dagr_graph_sort": (C.c_int, [C.POINTER(Geom), Dev, Dev, Dev, i64, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, p]),
+    "dagr_graph_sort_ring": (C.c_int, [C.POINTER(Geom), Dev, Dev, Dev, i64, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, p]),
+    "dagr_stream_push": (C.c_int, [Dev, Dev, Dev, Dev, Dev, i64, C.c_int, C.c_int, p]),
+    "dagr_stream_push_multi": (C.c_int, [Dev, Dev, Dev, Dev, Dev, i64, C.c_int, C.c_int, p]),
+    "dagr_graph_sort_rings": (C.c_int, [C.POINTER(Geom), Dev, Dev, Dev, i64, C.c_int, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev,
+                                        Dev, Dev, p]),
+    "dagr_l1_build": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.POINTER(L1AParams), Dev, C.c_int, Dev, Dev, Dev, Dev, Dev,
+                                Dev, C.c_int, p]),
+    "dagr_l1a_tc_weights": (C.c_int, [C.POINTER(L1AParams), Host]),
+    "dagr_l1_build_tc": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.POINTER(L1AParams), Dev, Dev, C.c_int, Dev, Dev, Dev,
+                                   Dev, Dev, Dev, C.c_int, p]),
+    "dagr_xa_permute": (C.c_int, [i64, Dev, C.c_int, Dev, Dev, C.c_int, p]),
+    "dagr_l1_x0_image": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, C.c_int, C.c_int, Dev, p]),
+    "dagr_l1_x0_image_live": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, Dev, p]),
+    "dagr_l1_x0_image_planes": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, Dev, C.c_int, Dev, p]),
+    "dagr_voxel_sample_max": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, Dev, C.c_int,
+                                        C.c_int, C.c_int, p]),
+    "dagr_voxel_sample_max_planes": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, C.c_int,
+                                               Dev, C.c_int, C.c_int, C.c_int, p]),
+    "dagr_graph_export": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, i64, p]),
+    "dagr_l1_tc_weights": (C.c_int, [Host, Host, C.c_int, Host]),
+    "dagr_l1_conv_b_pool_voxel_tc": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, Dev, Dev, Dev, C.POINTER(L1BParams), Dev, Dev,
+                                               C.c_int, Dev, Dev, Dev, Dev, Dev, Dev, Dev, C.c_int, Dev, Dev, C.c_int, p]),
+    "dagr_l1_conv_a_image_tc": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, Dev, Dev, C.POINTER(L1ImgParams), Dev, Dev, Dev,
+                                          Dev, Dev, C.c_int, p]),
+    "dagr_l1_conv_a_image_inc": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, Dev, Dev, Dev, C.POINTER(L1ImgParams), Dev,
+                                           C.c_int, Dev, Dev, Dev, Dev, C.c_int, p]),
+    "dagr_voxel_sample_max_inc": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev,
+                                            C.c_int, C.c_int, C.c_int, p]),
+    "dagr_grid_cat_pos": (C.c_int, [C.POINTER(Grid), Dev, Dev, Dev, C.c_int, Dev, p]),
+    "dagr_grid_conv": (C.c_int, [C.POINTER(Grid), Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, Dev, Dev, Dev, C.c_int,
+                                 f32, f32, Dev, p]),
     "dagr_grid_conv_last_instance": (C.c_int, []),
-    "dagr_grid_linear_bn": (C.c_int, [i64, p, p, C.c_int, C.c_int, p, p, p, p, p]),
-    "dagr_grid_pool": (C.c_int, [C.POINTER(Grid), C.POINTER(Grid), p, p, p, p, p, p, p, p, C.c_int, C.c_int,
-                                 p, p, p, p, p, p, p, p]),
-    "dagr_grid_pool_finalize": (C.c_int, [C.POINTER(Grid), C.c_int, C.c_int, p, p, p, p, p, p, p, p, p, p]),
-    "dagr_grid_temporal_filter": (C.c_int, [C.POINTER(Grid), p, p, p, p]),
-    "dagr_grid_to_dense": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, C.c_int, p, p, p]),
-    "dagr_head_finish": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, p, C.c_int, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p]),
-    "dagr_head_finish_planes": (C.c_int, [C.POINTER(Grid), p, p, C.c_int, p, C.c_int, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int,
-                                          C.c_int, p, C.c_int, p, p]),
-    "dagr_postprocess_nms": (C.c_int, [p, C.c_int, C.c_int, C.c_int, f32, f32, C.c_int, C.c_int, C.c_int, p, p, p]),
-    "dagr_sample_features": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p,
+    "dagr_grid_linear_bn": (C.c_int, [i64, Dev, Dev, C.c_int, C.c_int, Dev, Dev, Dev, Dev, p]),
+    "dagr_grid_pool": (C.c_int, [C.POINTER(Grid), C.POINTER(Grid), Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, C.c_int, C.c_int, Dev, Dev,
+                                 Dev, Dev, Dev, Dev, Dev, p]),
+    "dagr_grid_pool_finalize": (C.c_int, [C.POINTER(Grid), C.c_int, C.c_int, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, Dev, p]),
+    "dagr_grid_temporal_filter": (C.c_int, [C.POINTER(Grid), Dev, Dev, Dev, p]),
+    "dagr_grid_to_dense": (C.c_int, [C.POINTER(Grid), Dev, Dev, C.c_int, C.c_int, Dev, Dev, p]),
+    "dagr_head_finish": (C.c_int, [C.POINTER(Grid), Dev, Dev, C.c_int, Dev, C.c_int, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int,
+                                   C.c_int, Dev, p]),
+    "dagr_head_finish_planes": (C.c_int, [C.POINTER(Grid), Dev, Dev, C.c_int, Dev, C.c_int, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int,
+                                          C.c_int, C.c_int, Dev, C.c_int, Dev, p]),
+    "dagr_postprocess_nms": (C.c_int, [Dev, C.c_int, C.c_int, C.c_int, f32, f32, C.c_int, C.c_int, C.c_int, Dev, Dev, p]),
+    "dagr_sample_features": (C.c_int, [Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, i64, C.c_int, C.c_int, Dev,
                                        C.c_int, C.c_int, p]),
-    "dagr_sample_features_planes": (C.c_int, [p, C.c_int, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p,
-                                              C.c_int, C.c_int, p]),
+    "dagr_sample_features_planes": (C.c_int, [Dev, C.c_int, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, i64, C.c_int,
+                                              C.c_int, Dev, C.c_int, C.c_int, p]),
     # bf16 NHWC forms of the image-sampling calls (map as const void *, with its C)
-    "dagr_l1_x0_image_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, p]),
-    "dagr_l1_x0_image_live_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p, p]),
-    "dagr_l1_x0_image_planes_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p, p]),
-    "dagr_voxel_sample_max_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, p, C.c_int, C.c_int, C.c_int, p]),
-    "dagr_voxel_sample_max_inc_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, C.c_int,
-                                                 C.c_int, C.c_int, p]),
-    "dagr_voxel_sample_max_planes_bf16": (C.c_int, [C.POINTER(Geom), i64, p, p, p, C.c_int, C.c_int, C.c_int, C.c_int, p, C.c_int, p,
-                                                    C.c_int, C.c_int, C.c_int, p]),
-    "dagr_sample_features_bf16": (C.c_int, [p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int, p, C.c_int, C.c_int,
-                                            p]),
-    "dagr_sample_features_planes_bf16": (C.c_int, [p, C.c_int, p, C.c_int, C.c_int, C.c_int, C.c_int, p, p, p, i64, C.c_int, C.c_int,
-                                                   p, C.c_int, C.c_int, p]),
-    "dagr_masked_lin":(C.c_int, [p, i64, p, p, p, p, C.c_int, C.c_int, C.c_int, p]),
-    "dagr_masked_inplace_bn": (C.c_int, [p, i64, p, p, p, p, p, p, C.c_int, f32, p]),
-    "dagr_masked_isdiff": (C.c_int, [p, i64, p, p, C.c_int, f32, f32, p]),
+    "dagr_l1_x0_image_bf16": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, Dev, p]),
+    "dagr_l1_x0_image_live_bf16": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, Dev, p]),
+    "dagr_l1_x0_image_planes_bf16": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev,
+                                               C.c_int, Dev, p]),
+    "dagr_voxel_sample_max_bf16": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, Dev, C.c_int,
+                                             C.c_int, C.c_int, p]),
+    "dagr_voxel_sample_max_inc_bf16": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev,
+                                                 C.c_int, C.c_int, C.c_int, p]),
+    "dagr_voxel_sample_max_planes_bf16": (C.c_int, [C.POINTER(Geom), i64, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev,
+                                                    C.c_int, Dev, C.c_int, C.c_int, C.c_int, p]),
+    "dagr_sample_features_bf16": (C.c_int, [Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, i64, C.c_int, C.c_int, Dev,
+                                            C.c_int, C.c_int, p]),
+    "dagr_sample_features_planes_bf16": (C.c_int, [Dev, C.c_int, Dev, C.c_int, C.c_int, C.c_int, C.c_int, Dev, Dev, Dev, i64, C.c_int,
+                                                   C.c_int, Dev, C.c_int, C.c_int, p]),
+    "dagr_masked_lin": (C.c_int, [Dev, i64, Dev, Dev, Dev, Dev, C.c_int, C.c_int, C.c_int, p]),
+    "dagr_masked_inplace_bn": (C.c_int, [Dev, i64, Dev, Dev, Dev, Dev, Dev, Dev, C.c_int, f32, p]),
+    "dagr_masked_isdiff": (C.c_int, [Dev, i64, Dev, Dev, C.c_int, f32, f32, p]),
     "dagr_eval_workspace_bytes": (C.c_int, [i64, C.c_int, i64, i64, C.POINTER(i64)]),
-    "dagr_evaluate_bbox": (C.c_int, [p, p, p, p, p, p, p, i64, C.c_int, i64, i64, C.POINTER(EvalParams), p, i64, p, p, p]),
+    "dagr_evaluate_bbox": (C.c_int, [Dev, Dev, Dev, Dev, Dev, Dev, Dev, i64, C.c_int, i64, i64, C.POINTER(EvalParams), Dev, i64,
+                                     Dev, Dev, p]),
     "dagr_interframe_targets_workspace_bytes": (C.c_int, [i64, i64, C.POINTER(i64)]),
-    "dagr_interframe_targets": (C.c_int, [p, p, p, p, p, i64, i64, p, p, p, i64, C.c_int, C.c_int, C.c_int, f32, f32, i64, p, i64,
-                                          p, p, p, p]),
+    "dagr_interframe_targets": (C.c_int, [Dev, Dev, Dev, Dev, Dev, i64, i64, Dev, Dev, Dev, i64, C.c_int, C.c_int, C.c_int, f32, f32,
+                                          i64, Dev, i64, Dev, Dev, Dev, p]),
     "dagr_eval_pack_workspace_bytes": (C.c_int, [i64, C.POINTER(i64)]),
-    "dagr_eval_pack_detections": (C.c_int, [p, p, i64, C.c_int, p, p, C.c_int, p, i64, p, p, p, p, p]),
+    "dagr_eval_pack_detections": (C.c_int, [Dev, Dev, i64, C.c_int, Dev, Dev, C.c_int, Dev, i64, Dev, Dev, Dev, Dev, p]),
 }
 
 EXPORTS = tuple(_SIGS.keys())
@@ -159,6 +198,18 @@ EXPORTS = tuple(_SIGS.keys())
 
 def lib_path() -> Path:
     return _LIB_PATH
+
+
+def _entry(name, fn):
+    """fn, with an argument its type refuses raised as RuntimeError naming the entry point and the argument (ctypes
+    reports it as ArgumentError); nothing is launched."""
+    def call(*args):
+        try:
+            return fn(*args)
+        except C.ArgumentError as e:
+            raise RuntimeError(f"dagr_b200: {name} {e}") from None
+    call.__name__ = name
+    return call
 
 
 def load():
@@ -184,6 +235,7 @@ def load():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
+        setattr(lib, name, _entry(name, fn))
     if lib.dagr_abi_version() != 3:
         raise RuntimeError("dagr_b200: ABI version mismatch between python host and libdagr_b200.so")
     _lib = lib
@@ -197,7 +249,8 @@ def check(code: int, what: str = ""):
 
 
 def ptr(t):
-    """device pointer of a tensor (None -> NULL)."""
+    """raw address of a tensor (None -> NULL), for tests and tools that work with addresses; product code passes the
+    tensor itself (Dev)."""
     if t is None:
         return None
     return C.c_void_p(t.data_ptr())

@@ -28,8 +28,7 @@ def _fold_bn(bn):
 def _tc_weights(lib, params, cin: int, device) -> torch.Tensor:
     """params.w / params.root (input channels 0..15) in the mma fragment order of the tensor-core conv kernels (dagr_l1_tc_weights)."""
     out = (C.c_float * _lib.L1_TC_WFRAG_FLOATS)()
-    _lib.check(lib.dagr_l1_tc_weights(C.cast(params.w, C.c_void_p), C.cast(params.root, C.c_void_p), cin, C.cast(out, C.c_void_p)),
-               "dagr_l1_tc_weights")
+    _lib.check(lib.dagr_l1_tc_weights(params.w, params.root, cin, out), "dagr_l1_tc_weights")
     return torch.frombuffer(out, dtype=torch.float32).clone().to(device)
 
 
@@ -37,7 +36,7 @@ def _l1a_tc_weights(lib, params, device) -> torch.Tensor:
     """params.w / params.root of conv_block1.conv_block1's event channels in the mma fragment order of the tensor-core build
     kernel (dagr_l1a_tc_weights)."""
     out = (C.c_float * _lib.L1A_TC_WFRAG_FLOATS)()
-    _lib.check(lib.dagr_l1a_tc_weights(C.byref(params), C.cast(out, C.c_void_p)), "dagr_l1a_tc_weights")
+    _lib.check(lib.dagr_l1a_tc_weights(params, out), "dagr_l1a_tc_weights")
     return torch.frombuffer(out, dtype=torch.float32).clone().to(device)
 
 
@@ -77,13 +76,13 @@ class _Taps:
         return "_bf16" if self.fmt == torch.bfloat16 else ""
 
     def _plane_args(self, t):
-        return (int(t.shape[0]), _lib.ptr(self.planes[0]), int(self.planes[1])) if self.planes is not None else ()
+        return (int(t.shape[0]), self.planes[0], int(self.planes[1])) if self.planes is not None else ()
 
     def x0(self, eng, g, N, start, xyb, feat_s, x0, st):
         """the conv1 tap at every node; incremental steps resample every node too: a new node's conv reads the x0 rows of
         its older neighbours."""
         f = self.feats[0]
-        img = (_lib.ptr(f),) + ((int(f.shape[1]),) if self.sfx else ()) + (int(f.shape[2]), int(f.shape[3]))  # bf16 takes C
+        img = (f,) + ((int(f.shape[1]),) if self.sfx else ()) + (int(f.shape[2]), int(f.shape[3]))  # bf16 takes C
         if self.planes is not None:
             form, args = "_planes", (start, xyb, feat_s, *img, *self._plane_args(f))
         elif self.live:
@@ -97,9 +96,9 @@ class _Taps:
     def voxel_max(self, eng, g, N, start, xyb, ti, xg, ldx, c0, pool_mean, st):
         """the per-voxel max of the layer1 tap's samples into xg[:, c0:] (sampling_skip before pool1, net.py:128-131)."""
         f = self.feats[1]
-        img = (_lib.ptr(f), int(f.shape[1]), int(f.shape[2]), int(f.shape[3]))
+        img = (f, int(f.shape[1]), int(f.shape[2]), int(f.shape[3]))
         if self.state is not None:            # running per-voxel max of the samples, new events only
-            label, form, args = "voxel_sample_max_inc", "_inc", (ti, *img, self.min_idx, _lib.ptr(self.state.imgmax))
+            label, form, args = "voxel_sample_max_inc", "_inc", (ti, *img, self.min_idx, self.state.imgmax)
         else:
             label, form, args = "voxel_sample_max", "_planes" if self.planes is not None else "", (*img, *self._plane_args(f))
         eng._run(label, getattr(eng.lib, "dagr_voxel_sample_max" + form + self.sfx), g, N, start, xyb, *args, xg, ldx, c0,
@@ -109,7 +108,7 @@ class _Taps:
         """tap k sampled at n grid nodes into out[:, c0:]."""
         f = self.feats[k]
         form = "_planes" if self.planes is not None else ""
-        eng._run("sample_features", getattr(eng.lib, "dagr_sample_features" + form + self.sfx), _lib.ptr(f),
+        eng._run("sample_features", getattr(eng.lib, "dagr_sample_features" + form + self.sfx), f,
                  *(self._plane_args(f) or (int(f.shape[0]),)), int(f.shape[1]), int(f.shape[2]), int(f.shape[3]), posx, posy,
                  bidx, n, width, height, out, ldo, c0, st)
 
@@ -359,7 +358,7 @@ class Engine:
         slots = torch.tensor(geom.slots1, dtype=torch.long)
         cin0 = ca.conv.in_channels
         # every shape restriction of the kernels lives in ONE C-ABI call (include/dagr_b200.h: dagr_check_config)
-        if self.lib.dagr_check_config(C.byref(geom.c_geom), 0, int(cin0), int(ca.conv.out_channels), str(act).encode()) != 0:
+        if self.lib.dagr_check_config(geom.c_geom, 0, int(cin0), int(ca.conv.out_channels), str(act).encode()) != 0:
             raise NotImplementedError("dagr_b200: " + (self.lib.dagr_last_error() or b"").decode())
         pb = _lib.L1BParams()
         _fill(pb.w, cb.conv.weight.detach().cpu()[slots])                    # [15,16,16]
@@ -441,7 +440,7 @@ class Engine:
             nscan = max(geom.NK + 1, cap + 1)
             ws = dict(cap=cap)
             sz = _lib.EventWs()                                   # the library states its own workspace sizes (bytes)
-            _lib.check(self.lib.dagr_event_workspace_bytes(C.byref(geom.c_geom), cap, C.byref(sz)), "event_workspace_bytes")
+            _lib.check(self.lib.dagr_event_workspace_bytes(geom.c_geom, cap, sz), "event_workspace_bytes")
             for name, dt in (("key", torch.int32), ("tmp", torch.int32), ("blocksums", torch.int32), ("start", torch.int32),
                              ("perm", torch.int32), ("ti", torch.int32), ("xyb", torch.int32), ("feat_s", torch.float32),
                              ("nbr", torch.int32), ("off", torch.int16), ("xa", torch.float32)):
@@ -467,7 +466,7 @@ class Engine:
                 cells = geom.cells(lv)
                 Cc = C_lv[lv] + (fc[lv + 1] if bb.use_image else 0)      # channels pooled into this level (net.py:141-171)
                 psz = _lib.PoolWs()
-                _lib.check(self.lib.dagr_pool_workspace_bytes(cells, int(Cc), C.byref(psz)), "pool_workspace_bytes")
+                _lib.check(self.lib.dagr_pool_workspace_bytes(cells, int(Cc), psz), "pool_workspace_bytes")
                 take(f"acc{lv}", int(psz.acc))
                 take(f"possum{lv}", int(psz.possum))
                 take(f"ptmax{lv}", int(psz.ptmax))
@@ -578,25 +577,21 @@ class Engine:
     # ------------------------------------------------------------------------------------------
     def _grid_conv(self, geom, lv, gs: GridState, xin, pack: _ConvPack, skip, out, st, ldin=0):
         level = geom.levels[lv]
-        self._run(f"grid_conv_L{lv + 1}_{pack.cin}x{pack.cout}", self.lib.dagr_grid_conv, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(gs.pxy), _lib.ptr(gs.mask),
-                                           _lib.ptr(xin), int(ldin), pack.cin, pack.cout, _lib.ptr(pack.weight), _lib.ptr(pack.rootT),
-                                           _lib.ptr(pack.bias), _lib.ptr(pack.scale), _lib.ptr(pack.shift),
-                                           _lib.ptr(skip), 1 if pack.relu else 0, level.den_x, level.den_y,
-                                           _lib.ptr(out), st)
+        self._run(f"grid_conv_L{lv + 1}_{pack.cin}x{pack.cout}", self.lib.dagr_grid_conv, level.grid, gs.cnt, gs.pxy, gs.mask,
+                  xin, int(ldin), pack.cin, pack.cout, pack.weight, pack.rootT, pack.bias, pack.scale, pack.shift, skip,
+                  1 if pack.relu else 0, level.den_x, level.den_y, out, st)
 
     def _layer(self, geom, lv, gs: GridState, lp: _LayerPack, ws, name, st, dev):
         level = geom.levels[lv]
         cells = gs.cells
         cx = gs.x.shape[1]
         xin = self._buf(ws, name + "_in", (cells, cx + 2), torch.float32, dev)
-        self._run("cat_pos", self.lib.dagr_grid_cat_pos, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(gs.pxy), _lib.ptr(gs.x), cx,
-                                              _lib.ptr(xin), st)
+        self._run("cat_pos", self.lib.dagr_grid_cat_pos, level.grid, gs.cnt, gs.pxy, gs.x, cx, xin, st)
         a = self._buf(ws, name + "_a", (cells, lp.a.cout), torch.float32, dev)
         self._grid_conv(geom, lv, gs, xin, lp.a, None, a, st)
         sk = self._buf(ws, name + "_s", (cells, lp.b.cout), torch.float32, dev)
-        self._run("linear_bn", self.lib.dagr_grid_linear_bn, cells, _lib.ptr(gs.cnt), _lib.ptr(xin), cx + 2, lp.b.cout,
-                                                _lib.ptr(lp.skipT), _lib.ptr(lp.sscale), _lib.ptr(lp.sshift),
-                                                _lib.ptr(sk), st)
+        self._run("linear_bn", self.lib.dagr_grid_linear_bn, cells, gs.cnt, xin, cx + 2, lp.b.cout, lp.skipT, lp.sscale,
+                  lp.sshift, sk, st)
         out = self._buf(ws, name + "_o", (cells, lp.b.cout), torch.float32, dev)
         self._grid_conv(geom, lv, gs, a, lp.b, sk, out, st)
         return xin, a, out
@@ -618,20 +613,15 @@ class Engine:
         pcnt = self._zs(ws, f"pcnt{lp}", torch.int32)
         pmask = self._zs(ws, f"pmask{lp}", torch.int32)
         err = self._zs(ws, "err", torch.int32)
-        self._run("grid_pool", self.lib.dagr_grid_pool, C.byref(child.grid), C.byref(parent.grid), _lib.ptr(parent.cellx_dev),
-                                           _lib.ptr(parent.celly_dev), _lib.ptr(gc.cnt), _lib.ptr(gc.pxy),
-                                           _lib.ptr(gc.tmean), _lib.ptr(gc.tmax), _lib.ptr(gc.mask), _lib.ptr(x), Cc, aggr,
-                                           _lib.ptr(accmax), _lib.ptr(accsum), _lib.ptr(possum), _lib.ptr(ptmax),
-                                           _lib.ptr(pcnt), _lib.ptr(pmask), _lib.ptr(err), st)
+        self._run("grid_pool", self.lib.dagr_grid_pool, child.grid, parent.grid, parent.cellx_dev, parent.celly_dev, gc.cnt,
+                  gc.pxy, gc.tmean, gc.tmax, gc.mask, x, Cc, aggr, accmax, accsum, possum, ptmax, pcnt, pmask, err, st)
         gp.x = self._buf(ws, f"gx{lp}", (gp.cells, Cc), torch.float32, dev)
-        self._run("grid_pool_finalize", self.lib.dagr_grid_pool_finalize, C.byref(parent.grid), Cc, aggr, _lib.ptr(accmax), _lib.ptr(accsum),
-                                                    _lib.ptr(possum), _lib.ptr(ptmax), _lib.ptr(pcnt), _lib.ptr(gp.pxy),
-                                                    _lib.ptr(gp.tmean), _lib.ptr(gp.tmax), _lib.ptr(gp.x), st)
+        self._run("grid_pool_finalize", self.lib.dagr_grid_pool_finalize, parent.grid, Cc, aggr, accmax, accsum, possum, ptmax,
+                  pcnt, gp.pxy, gp.tmean, gp.tmax, gp.x, st)
         gp.cnt = pcnt[:gp.cells]
         gp.mask = pmask[:gp.cells]
         if keep_temporal:
-            self._run("temporal_filter", self.lib.dagr_grid_temporal_filter, C.byref(parent.grid), _lib.ptr(gp.cnt), _lib.ptr(gp.tmax),
-                                                          _lib.ptr(gp.mask), st)
+            self._run("temporal_filter", self.lib.dagr_grid_temporal_filter, parent.grid, gp.cnt, gp.tmax, gp.mask, st)
         return gp
 
     # ------------------------------------------------------------------------------------------
@@ -651,8 +641,7 @@ class Engine:
         if key not in ws:
             per = geom.levels[lv].nx * geom.levels[lv].ny
             ws[key] = (torch.arange(cells, device=dev) // per).int()
-        taps.sample_features(self, k, _lib.ptr(posx), _lib.ptr(posy), _lib.ptr(ws[key]), cells, geom.W, geom.H, _lib.ptr(xcat),
-                             Cc + Cf, Cc, st)
+        taps.sample_features(self, k, posx, posy, ws[key], cells, geom.W, geom.H, xcat, Cc + Cf, Cc, st)
         return xcat
 
     @torch.no_grad()
@@ -713,52 +702,49 @@ class Engine:
     def _event_level(self, mode: _Mode, geom, pk, ws, N, batch_i32, pos_i32, feat, image_event, kto):
         """graph sort -> adjacency + conv_a -> conv_b + pool1 into grid level 0, with the image samples of a hybrid model.
         -> (level-0 grid, the per-event conv_b activations when keep_node_features, else None)"""
-        lib, g, st, dev = self.lib, C.byref(geom.c_geom), _lib.stream_ptr(), pos_i32.device
+        lib, g, st, dev = self.lib, geom.c_geom, _lib.stream_ptr(), pos_i32.device
         taps, state, min_idx = mode.taps, mode.state, mode.min_idx
         ws["zero_buf"].zero_()
-        start, perm, ti, xyb, feat_s, nbr, off, xa = (_lib.ptr(ws[k])
-                                                      for k in ("start", "perm", "ti", "xyb", "feat_s", "nbr", "off", "xa"))
+        start, perm, ti, xyb, feat_s, nbr, off, xa = (ws[k] for k in ("start", "perm", "ti", "xyb", "feat_s", "nbr", "off", "xa"))
         cellmask = self._cellmask(mode, ws)
         flags = self._zs(ws, "flags", torch.int32)
         wl_hdr = self._zs(ws, "wl_hdr", torch.int32)
         defer = self._dense_policy(ws, wl_hdr, mode.fixed)
         if mode.sort == "rings":
-            fn, size = lib.dagr_graph_sort_rings, (N // mode.streams, mode.streams, _lib.ptr(mode.ring))
+            fn, size = lib.dagr_graph_sort_rings, (N // mode.streams, mode.streams, mode.ring)
         elif mode.sort == "ring":
-            fn, size = lib.dagr_graph_sort_ring, (N, _lib.ptr(mode.ring))
+            fn, size = lib.dagr_graph_sort_ring, (N, mode.ring)
         else:
             fn, size = lib.dagr_graph_sort, (N,)
-        self._run("graph_sort", fn, g, _lib.ptr(batch_i32), _lib.ptr(pos_i32), _lib.ptr(feat), *size, _lib.ptr(ws["key"]),
-                  _lib.ptr(ws["tmp"]), _lib.ptr(ws["count"]), _lib.ptr(ws["blocksums"]), start, perm, ti, xyb, feat_s,
-                  _lib.ptr(flags), st)
+        self._run("graph_sort", fn, g, batch_i32, pos_i32, feat, *size, ws["key"], ws["tmp"], ws["count"], ws["blocksums"], start,
+                  perm, ti, xyb, feat_s, flags, st)
         if min_idx > 0:
             # incremental step: the first n_old arrival indices were processed before; only newer events get their edges /
             # activations computed (the causal graph never changes an old node's inputs), the older xa rows are gathered.
             # With image fusion the frame is the same for every step between two re-seeds (dagr_b200.asynchronous)
-            self._run("xa_gather", lib.dagr_xa_permute, N, perm, min_idx, xa, _lib.ptr(state.xa_arr), 0, st)
+            self._run("xa_gather", lib.dagr_xa_permute, N, perm, min_idx, xa, state.xa_arr, 0, st)
         # adjacency + conv_block1.conv_block1.  With image fusion the layer runs on [polarity, 16 image samples, x, y]
         # (net.py:117-126): this is its (polarity, x, y) part, the image channels follow in the conv_a image kernel
         l1a = "l1a" if taps is None else "l1a_img"
-        self._run("l1_build", lib.dagr_l1_build_tc, g, N, start, ti, xyb, feat_s, C.byref(pk[l1a]), _lib.ptr(pk[l1a + "_wfrag"]),
-                  _lib.ptr(flags), min_idx, nbr, off, _lib.ptr(cellmask), xa, _lib.ptr(wl_hdr),
-                  _lib.ptr(self._zs(ws, "wl_build", torch.int32)), defer[0], st)
+        self._run("l1_build", lib.dagr_l1_build_tc, g, N, start, ti, xyb, feat_s, pk[l1a], pk[l1a + "_wfrag"], flags, min_idx,
+                  nbr, off, cellmask, xa, wl_hdr, self._zs(ws, "wl_build", torch.int32), defer[0], st)
         skipv = None
         if taps is not None:
             if image_event is not None:                       # stage 1 of the image branch ran on a side stream next to sort + probe
                 torch.cuda.current_stream().wait_event(image_event[0])
             x0 = self._buf(ws, "x0img", (2 * max(N, 1) * 8,), torch.float32, dev)
             skipv = self._buf(ws, "skipv", (max(N, 1), 16), torch.float32, dev)
-            taps.x0(self, g, N, start, xyb, feat_s, _lib.ptr(x0), st)
-            wl = (_lib.ptr(wl_hdr[2:]), _lib.ptr(self._zs(ws, "wl_conv_a", torch.int32)), defer[1], st)
+            taps.x0(self, g, N, start, xyb, feat_s, x0, st)
+            wl = (wl_hdr[2:], self._zs(ws, "wl_conv_a", torch.int32), defer[1], st)
             if state is not None:
                 # only the new nodes are convolved; the xa rows of the older ones are final and stay as gathered
-                self._run("l1_conv_a_image_inc", lib.dagr_l1_conv_a_image_inc, g, N, start, xyb, ti, feat_s, _lib.ptr(x0), nbr, off,
-                          C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), min_idx, xa, _lib.ptr(skipv), *wl)
+                self._run("l1_conv_a_image_inc", lib.dagr_l1_conv_a_image_inc, g, N, start, xyb, ti, feat_s, x0, nbr, off,
+                          pk["l1img"], pk["l1img_wfrag"], min_idx, xa, skipv, *wl)
             else:
-                self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, start, xyb, feat_s, _lib.ptr(x0), nbr, off,
-                          C.byref(pk["l1img"]), _lib.ptr(pk["l1img_wfrag"]), xa, _lib.ptr(skipv), *wl)
+                self._run("l1_conv_a_image", lib.dagr_l1_conv_a_image_tc, g, N, start, xyb, feat_s, x0, nbr, off,
+                          pk["l1img"], pk["l1img_wfrag"], xa, skipv, *wl)
         if state is not None:
-            self._run("xa_scatter", lib.dagr_xa_permute, N, perm, min_idx, xa, _lib.ptr(state.xa_arr), 1, st)
+            self._run("xa_scatter", lib.dagr_xa_permute, N, perm, min_idx, xa, state.xa_arr, 1, st)
         x1 = None
         if self.keep_node_features:
             if ws["x1"] is None or ws["x1"].shape[0] < ws["cap"]:
@@ -768,13 +754,11 @@ class Engine:
         c1 = 16 + (int(taps.feats[1].shape[1]) if taps is not None else 0)
         g1.x = self._buf(ws, "gx0", (g1.cells, c1), torch.float32, dev)
         self._run("l1_conv_b_pool_voxel", lib.dagr_l1_conv_b_pool_voxel_tc, g, N, start, xyb, ti, feat_s, xa, nbr, off,
-                  C.byref(pk["l1b"]), _lib.ptr(pk["l1b_wfrag"]), _lib.ptr(skipv), min_idx,
-                  _lib.ptr(state.voxmax if state is not None else None), _lib.ptr(x1), _lib.ptr(g1.cnt), _lib.ptr(g1.pxy),
-                  _lib.ptr(g1.tmean), _lib.ptr(g1.tmax), _lib.ptr(g1.x), c1, _lib.ptr(wl_hdr[4:]),
-                  _lib.ptr(self._zs(ws, "wl_conv_b", torch.int32)), defer[2], st)
+                  pk["l1b"], pk["l1b_wfrag"], skipv, min_idx, state.voxmax if state is not None else None, x1, g1.cnt, g1.pxy,
+                  g1.tmean, g1.tmax, g1.x, c1, wl_hdr[4:], self._zs(ws, "wl_conv_b", torch.int32), defer[2], st)
         self._dense_report(ws, wl_hdr)
         if taps is not None:
-            taps.voxel_max(self, g, N, start, xyb, ti, _lib.ptr(g1.x), c1, 16, int(pk["l1b"].pool_mean), st)
+            taps.voxel_max(self, g, N, start, xyb, ti, g1.x, c1, 16, int(pk["l1b"].pool_mean), st)
         g1.mask = cellmask[:g1.cells]
         if kto and state is not None:
             # the persistent stream mask only ever gains edges; the temporal filter (pooling.py:69-72) depends on the CURRENT
@@ -783,8 +767,7 @@ class Engine:
             step_mask[:g1.cells].copy_(cellmask[:g1.cells])
             g1.mask = step_mask[:g1.cells]
         if kto:
-            self._run("temporal_filter", lib.dagr_grid_temporal_filter, C.byref(geom.levels[0].grid), _lib.ptr(g1.cnt), _lib.ptr(g1.tmax),
-                                                     _lib.ptr(g1.mask), st)
+            self._run("temporal_filter", lib.dagr_grid_temporal_filter, geom.levels[0].grid, g1.cnt, g1.tmax, g1.mask, st)
         return g1, x1
 
     def _coarse_stack(self, mode: _Mode, slot, geom, pk, ws, g1, B, kto, image_event):
@@ -907,16 +890,14 @@ class Engine:
         oro = self._buf(ws, nm + "_regobj", (cells, 5), torch.float32, dev)         # [reg(4) | obj(1)]
         self._grid_conv(geom, lv, gs, cr[:, Cf:], hp["regobj_pred"], None, oro, st, ldin=2 * Cf)
         form, adds, planes = taps.head_maps(k) if taps is not None else ("", dict.fromkeys(("cls", "reg", "obj")), ())
-        self._run("head_finish", getattr(lib, "dagr_head_finish" + form), C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(ocls), nc,
-                  _lib.ptr(oro), 5, _lib.ptr(adds["cls"]), _lib.ptr(adds["reg"]), _lib.ptr(adds["obj"]), nc,
-                  int(self.model.backbone.strides[k]), a0, A, *planes, _lib.ptr(out), st)
+        self._run("head_finish", getattr(lib, "dagr_head_finish" + form), level.grid, gs.cnt, ocls, nc, oro, 5, adds["cls"],
+                  adds["reg"], adds["obj"], nc, int(self.model.backbone.strides[k]), a0, A, *planes, out, st)
         dense = {}
         if self.keep_node_features:
             # parity / debugging: the dense [B,C,ny,nx] head maps of SplineConvToDense (spline_conv.py:80-107)
             for name, src, c0, cw, ld in (("cls", ocls, 0, nc, nc), ("reg", oro, 0, 4, 5), ("obj", oro, 4, 1, 5)):
                 d = self._buf(ws, nm + "_d" + name, (B, cw, level.ny, level.nx), torch.float32, dev)
-                self._run("to_dense", lib.dagr_grid_to_dense, C.byref(level.grid), _lib.ptr(gs.cnt), _lib.ptr(src[:, c0:]), cw, ld,
-                          _lib.ptr(adds[name]), _lib.ptr(d), st)
+                self._run("to_dense", lib.dagr_grid_to_dense, level.grid, gs.cnt, src[:, c0:], cw, ld, adds[name], d, st)
                 dense[name] = d
         return dense
 
@@ -941,16 +922,16 @@ class Engine:
         if slot is None:
             det = torch.empty((B, A, 6), dtype=torch.float32, device=dev)
             ndet = torch.empty(B, dtype=torch.int32, device=dev)
-            self._run("postprocess_nms", self.lib.dagr_postprocess_nms, _lib.ptr(decoded), B, A, nc, float(conf_thre), float(nms_thre),
-                      int(width), int(height), 1 if filtering else 0, _lib.ptr(det), _lib.ptr(ndet), _lib.stream_ptr())
+            self._run("postprocess_nms", self.lib.dagr_postprocess_nms, decoded, B, A, nc, float(conf_thre), float(nms_thre),
+                      int(width), int(height), 1 if filtering else 0, det, ndet, _lib.stream_ptr())
             return det, ndet
         # overlapped forward: NMS follows the coarse stack on the side stream, into per-slot result buffers
         sw = self.last["ws"]
         det = self._buf(sw, "post_det", (B, A, 6), torch.float32, dev)
         ndet = self._buf(sw, "post_ndet", (B,), torch.int32, dev)
         with torch.cuda.stream(self._cstream):
-            self._run("postprocess_nms", self.lib.dagr_postprocess_nms, _lib.ptr(decoded), B, A, nc, float(conf_thre), float(nms_thre),
-                      int(width), int(height), 1 if filtering else 0, _lib.ptr(det), _lib.ptr(ndet), _lib.stream_ptr())
+            self._run("postprocess_nms", self.lib.dagr_postprocess_nms, decoded, B, A, nc, float(conf_thre), float(nms_thre),
+                      int(width), int(height), 1 if filtering else 0, det, ndet, _lib.stream_ptr())
             ev = torch.cuda.Event()
             ev.record()
         self._done[slot] = ev
@@ -970,8 +951,7 @@ class Engine:
         rowptr = torch.empty(N + 1, dtype=torch.int32, device=dev)
         es = torch.empty(cap, dtype=torch.int64, device=dev)
         ed = torch.empty(cap, dtype=torch.int64, device=dev)
-        self._run("graph_export", self.lib.dagr_graph_export, C.byref(geom.c_geom), N, _lib.ptr(ws["perm"]), _lib.ptr(ws["ti"]),
-                                              _lib.ptr(ws["nbr"]), _lib.ptr(inv), _lib.ptr(rowptr), _lib.ptr(ws["blocksums"]),
-                                              _lib.ptr(es), _lib.ptr(ed), cap, _lib.stream_ptr())
+        self._run("graph_export", self.lib.dagr_graph_export, geom.c_geom, N, ws["perm"], ws["ti"], ws["nbr"], inv, rowptr,
+                  ws["blocksums"], es, ed, cap, _lib.stream_ptr())
         E = int(rowptr[N].item())
         return torch.stack([es[:E], ed[:E]])

@@ -39,7 +39,7 @@ def _params() -> _lib.EvalParams:
 
 def workspace_bytes(n_images: int, num_classes: int, n_gt: int, n_det: int) -> int:
     out = C.c_int64(0)
-    _lib.check(_lib.load().dagr_eval_workspace_bytes(n_images, num_classes, n_gt, n_det, C.byref(out)), "dagr_eval_workspace_bytes")
+    _lib.check(_lib.load().dagr_eval_workspace_bytes(n_images, num_classes, n_gt, n_det, out), "dagr_eval_workspace_bytes")
     return out.value
 
 
@@ -83,10 +83,8 @@ def accumulate(gt_boxes_list: Sequence[Dict[str, torch.Tensor]], dt_boxes_list: 
             ws = workspace
         precision = torch.empty((len(IOU_THRS), len(REC_THRS), K, len(AREA_RNG)), dtype=torch.float64, device=dev)
         recall = torch.empty((len(IOU_THRS), K, len(AREA_RNG)), dtype=torch.float64, device=dev)
-        _lib.check(lib.dagr_evaluate_bbox(_lib.ptr(gt_box), _lib.ptr(gt_lab), _lib.ptr(gt_off), _lib.ptr(dt_box), _lib.ptr(dt_score),
-                                          _lib.ptr(dt_lab), _lib.ptr(dt_off), n, K, len(gt_box), len(dt_box), C.byref(_params()),
-                                          _lib.ptr(ws), ws.numel(), _lib.ptr(precision), _lib.ptr(recall), _lib.stream_ptr()),
-                   "dagr_evaluate_bbox")
+        _lib.check(lib.dagr_evaluate_bbox(gt_box, gt_lab, gt_off, dt_box, dt_score, dt_lab, dt_off, n, K, len(gt_box), len(dt_box),
+                                          _params(), ws, ws.numel(), precision, recall, _lib.stream_ptr()), "dagr_evaluate_bbox")
     return precision, recall
 
 

@@ -66,18 +66,16 @@ def downsample_events(events: Dict[str, torch.Tensor], input_height: int, input_
     start, blocksums = _i32(cells + 2, dev), _i32(nb, dev)
     mask = torch.zeros(max(N, 1), dtype=torch.uint8, device=dev)
     st = _lib.stream_ptr()
-    _lib.check(lib.dagr_downsample_events(_lib.ptr(x), _lib.ptr(y), _lib.ptr(p), N, fx, fy, output_width, output_height,
-                                          _lib.ptr(change_map), _lib.ptr(cell), _lib.ptr(tmp), _lib.ptr(srt), _lib.ptr(count),
-                                          _lib.ptr(start), _lib.ptr(blocksums), _lib.ptr(mask), st), "downsample_events")
+    _lib.check(lib.dagr_downsample_events(x, y, p, N, fx, fy, output_width, output_height, change_map, cell, tmp, srt, count,
+                                          start, blocksums, mask, st), "downsample_events")
     flag, pos = _i32(N, dev), _i32(N + 1, dev)
     xo = torch.empty(max(N, 1), dtype=torch.int16, device=dev)
     yo = torch.empty(max(N, 1), dtype=torch.int16, device=dev)
     to = torch.empty(max(N, 1), dtype=torch.int64, device=dev)
     po = torch.empty(max(N, 1), dtype=torch.int8, device=dev)
     n_out = torch.zeros(1, dtype=torch.int32, device=dev)
-    _lib.check(lib.dagr_compact_events(_lib.ptr(mask), N, _lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), fx, fy,
-                                       _lib.ptr(flag), _lib.ptr(pos), _lib.ptr(blocksums), _lib.ptr(xo), _lib.ptr(yo),
-                                       _lib.ptr(to), _lib.ptr(po), _lib.ptr(n_out), st), "compact_events")
+    _lib.check(lib.dagr_compact_events(mask, N, x, y, t, p, fx, fy, flag, pos, blocksums, xo, yo, to, po, n_out, st),
+               "compact_events")
     M = int(n_out.item())                                       # the one host sync: output length
     return dict(x=xo[:M], y=yo[:M], t=to[:M], p=po[:M]), change_map
 
@@ -100,10 +98,9 @@ def ingest_window(events: Dict[str, torch.Tensor], width: int, height: int, time
     feat_o = torch.empty(max(N, 1), dtype=torch.float32, device=dev)
     n_out = torch.zeros(1, dtype=torch.int32, device=dev)
     cut = (1 << 62) if t_cut is None else int(t_cut)
-    _lib.check(lib.dagr_ingest_events(_lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), N, 1 if p_is_01 else 0, int(width),
-                                      int(height), int(time_window), cut, int(sample), _lib.ptr(flag), _lib.ptr(pos),
-                                      _lib.ptr(blocksums), _lib.ptr(tlast), _lib.ptr(batch_o), _lib.ptr(pos_o), _lib.ptr(feat_o),
-                                      _lib.ptr(n_out), _lib.stream_ptr()), "ingest_events")
+    _lib.check(lib.dagr_ingest_events(x, y, t, p, N, 1 if p_is_01 else 0, int(width), int(height), int(time_window), cut,
+                                      int(sample), flag, pos, blocksums, tlast, batch_o, pos_o, feat_o, n_out,
+                                      _lib.stream_ptr()), "ingest_events")
     M = int(n_out.item())
     return batch_o[:M], pos_o[:M], feat_o[:M]
 
@@ -123,9 +120,8 @@ def preprocess_frames(frames: torch.Tensor, height: int, width: int, scale: int,
         raise ValueError(f"frames {tuple(frames.shape)} {frames.dtype}: expected u8 [F, sh, sw, 3]")
     F, sh, sw = (int(v) for v in frames.shape[:3])
     out = torch.empty((F, 3, height, width), dtype=torch.uint8 if lut is None else torch.float32, device=frames.device)
-    _lib.check(lib.dagr_frame_preprocess(_lib.ptr(frames), F, sh, sw, int(scale), int(height), int(width),
-                                         _lib.ptr(out) if lut is None else None, None if lut is None else _lib.ptr(out),
-                                         _lib.ptr(lut), _lib.stream_ptr()), "frame_preprocess")
+    _lib.check(lib.dagr_frame_preprocess(frames, F, sh, sw, int(scale), int(height), int(width), out if lut is None else None,
+                                         None if lut is None else out, lut, _lib.stream_ptr()), "frame_preprocess")
     return out
 
 

@@ -99,17 +99,16 @@ class InterframeEvaluation:
         R = G * int(pl.off[min(kept, P)])
         with torch.cuda.device(dev):
             ws_t, ws_p = C.c_int64(0), C.c_int64(0)
-            _lib.check(lib.dagr_interframe_targets_workspace_bytes(Q, R, C.byref(ws_t)), "dagr_interframe_targets_workspace_bytes")
-            _lib.check(lib.dagr_eval_pack_workspace_bytes(Q, C.byref(ws_p)), "dagr_eval_pack_workspace_bytes")
+            _lib.check(lib.dagr_interframe_targets_workspace_bytes(Q, R, ws_t), "dagr_interframe_targets_workspace_bytes")
+            _lib.check(lib.dagr_eval_pack_workspace_bytes(Q, ws_p), "dagr_eval_pack_workspace_bytes")
             ws = torch.empty(max(ws_t.value, ws_p.value), dtype=torch.uint8, device=dev)
             gt_box = torch.empty((R, 4), dtype=torch.float32, device=dev)
             gt_label = torch.empty(R, dtype=torch.int64, device=dev)
             gt_off = torch.empty(Q + 1, dtype=torch.int64, device=dev)
             _lib.check(lib.dagr_interframe_targets(
-                _lib.ptr(rec["box0"]), _lib.ptr(rec["box1"]), _lib.ptr(rec["cls"]), _lib.ptr(rec["pair_off"]), _lib.ptr(rec["pair_t"]),
-                P + 1, L, _lib.ptr(win_pair), _lib.ptr(rec["win_t"]), _lib.ptr(rec["win_group"]), Q, self.K, self.W, self.H,
-                float(self.min_bbox_height), float(self.min_bbox_diag), R, _lib.ptr(ws), ws.numel(), _lib.ptr(gt_box),
-                _lib.ptr(gt_label), _lib.ptr(gt_off), _lib.stream_ptr()), "dagr_interframe_targets")
+                rec["box0"], rec["box1"], rec["cls"], rec["pair_off"], rec["pair_t"], P + 1, L, win_pair, rec["win_t"],
+                rec["win_group"], Q, self.K, self.W, self.H, float(self.min_bbox_height), float(self.min_bbox_diag), R, ws,
+                ws.numel(), gt_box, gt_label, gt_off, _lib.stream_ptr()), "dagr_interframe_targets")
             det, ndet = rec["det"], rec["ndet"]
             A = det.shape[1]
             dt_box = torch.empty((Q * A, 4), dtype=torch.float32, device=dev)
@@ -117,9 +116,8 @@ class InterframeEvaluation:
             dt_label = torch.empty(Q * A, dtype=torch.int64, device=dev)
             dt_off = torch.empty(Q + 1, dtype=torch.int64, device=dev)
             _lib.check(lib.dagr_eval_pack_detections(
-                _lib.ptr(det), _lib.ptr(ndet), Q, A, _lib.ptr(rec["win_group"]), _lib.ptr(gt_off), self.K, _lib.ptr(ws), ws.numel(),
-                _lib.ptr(dt_box), _lib.ptr(dt_score), _lib.ptr(dt_label), _lib.ptr(dt_off), _lib.stream_ptr()),
-                "dagr_eval_pack_detections")
+                det, ndet, Q, A, rec["win_group"], gt_off, self.K, ws, ws.numel(), dt_box, dt_score, dt_label, dt_off,
+                _lib.stream_ptr()), "dagr_eval_pack_detections")
         rec.update(kept=kept, gt_box=gt_box, gt_label=gt_label, gt_off=gt_off, dt_box=dt_box, dt_score=dt_score, dt_label=dt_label,
                    dt_off=dt_off)
 
@@ -173,9 +171,8 @@ class InterframeEvaluation:
                                     dtype=torch.float64, device=dev)
             recall = torch.empty((len(evaluation.IOU_THRS), G * K, len(evaluation.AREA_RNG)), dtype=torch.float64, device=dev)
             _lib.check(_lib.load().dagr_evaluate_bbox(
-                _lib.ptr(gt_box), _lib.ptr(gt_label), _lib.ptr(gt_off), _lib.ptr(dt_box), _lib.ptr(dt_score), _lib.ptr(dt_label),
-                _lib.ptr(dt_off), n_images, G * K, len(gt_box), len(dt_box), C.byref(evaluation._params()), _lib.ptr(ws), ws.numel(),
-                _lib.ptr(precision), _lib.ptr(recall), _lib.stream_ptr()), "dagr_evaluate_bbox")
+                gt_box, gt_label, gt_off, dt_box, dt_score, dt_label, dt_off, n_images, G * K, len(gt_box), len(dt_box),
+                evaluation._params(), ws, ws.numel(), precision, recall, _lib.stream_ptr()), "dagr_evaluate_bbox")
         self.last = (precision, recall)
         prec = precision.cpu().numpy()
         out = {}

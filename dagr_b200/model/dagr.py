@@ -209,8 +209,8 @@ class DAGR(YOLOX):
             batch_i = torch.empty(N, dtype=torch.int32, device=dev)
             feat = torch.empty(N, dtype=torch.float32, device=dev)
             ldx = 1 if xf.dim() == 1 else int(xf.shape[1])
-            _lib.check(lib.dagr_prepare_events(_lib.ptr(x.pos), _lib.ptr(x.batch), _lib.ptr(xf), ldx, N, W, H, T, _lib.ptr(pos_i),
-                                               _lib.ptr(batch_i), _lib.ptr(feat), _lib.stream_ptr()), "prepare_events")
+            _lib.check(lib.dagr_prepare_events(x.pos, x.batch, xf, ldx, N, W, H, T, pos_i, batch_i, feat, _lib.stream_ptr()),
+                       "prepare_events")
             self.engine.launches += 1
             return batch_i, pos_i, feat, W, H
         if hasattr(x, "pos_denorm") and x.pos_denorm is not None:               # ev_tgn.py:12-13
@@ -218,8 +218,7 @@ class DAGR(YOLOX):
         else:
             pos_f = x.pos.float().contiguous()
             pos_i = torch.empty((N, 3), dtype=torch.int32, device=dev)
-            _lib.check(lib.dagr_denormalize_pos(_lib.ptr(pos_f), N, W, H, T, _lib.ptr(pos_i), _lib.stream_ptr()),
-                       "denormalize_pos")
+            _lib.check(lib.dagr_denormalize_pos(pos_f, N, W, H, T, pos_i, _lib.stream_ptr()), "denormalize_pos")
         batch_i = x.batch.int().contiguous()
         feat = x.x.float().reshape(N, -1)[:, 0].contiguous() if N > 0 else torch.zeros(0, device=dev)
         return batch_i, pos_i, feat, W, H

@@ -243,9 +243,8 @@ class SequenceDetector:
         feats, outs, tab = planes if planes is not None else (None, None, None)
         det_all = ndet_all = None
         for i, ((q0, q1), n) in enumerate(zip(blocks, totals)):
-            eng._run("window_gather", lib.dagr_window_gather, _lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), N, _lib.ptr(begin[q0:]),
-                     _lib.ptr(end[q0:]), q1 - q0, int(t_base), 0, n, _lib.ptr(batch), _lib.ptr(pos), _lib.ptr(feat), _lib.ptr(offs),
-                     _lib.stream_ptr())
+            eng._run("window_gather", lib.dagr_window_gather, x, y, t, p, N, begin[q0:], end[q0:], q1 - q0, int(t_base), 0, n,
+                     batch, pos, feat, offs, _lib.stream_ptr())
             dec = eng.forward_events(batch[:n], pos[:n], feat[:n], G, self.W, self.H, image_feats=feats, image_outs=outs,
                                      image_planes=None if tab is None else (tab[i], 1))
             det, ndet = eng.postprocess(dec, m.conf_threshold, m.nms_threshold, self.W, self.H)
@@ -286,9 +285,8 @@ class SequenceDetector:
         N = len(ev[2])
         begin = torch.zeros(max(Q, 1), dtype=torch.int32, device=dev)
         end = torch.zeros(max(Q, 1), dtype=torch.int32, device=dev)
-        d_tb, d_te = torch.from_numpy(tb).to(dev), torch.from_numpy(te).to(dev)       # held: the call only gets their addresses
-        _lib.check(lib.dagr_window_bounds(_lib.ptr(ev[2]), N, _lib.ptr(d_tb), _lib.ptr(d_te), Q, _lib.ptr(begin), _lib.ptr(end),
-                                          _lib.stream_ptr()), "window_bounds")
+        d_tb, d_te = torch.from_numpy(tb).to(dev), torch.from_numpy(te).to(dev)
+        _lib.check(lib.dagr_window_bounds(ev[2], N, d_tb, d_te, Q, begin, end, _lib.stream_ptr()), "window_bounds")
         be = torch.stack([begin[:Q], end[:Q]]).cpu().numpy()                  # host sync 1: the bounds
         sizes = np.maximum(be[1].astype(np.int64) - be[0], 0)
         blocks = plan_blocks(sizes, self.max_windows, self.max_events)

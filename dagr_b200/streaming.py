@@ -151,9 +151,8 @@ class _RingDetector:
         return None
 
     def _push(self):
-        _lib.check(self.lib.dagr_stream_push_multi(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
-                                                   _lib.ptr(self.feat), self.cap, self.S, self.max_chunk, _lib.stream_ptr()),
-                   "stream_push_multi")
+        _lib.check(self.lib.dagr_stream_push_multi(self.ctl, self.stage_d, self.batch, self.pos, self.feat, self.cap, self.S,
+                                                   self.max_chunk, _lib.stream_ptr()), "stream_push_multi")
 
     def _check_sensor(self, sensor, p_is_01):
         """raw sensor mode: the down-sampling factor and grid of a `sensor` = (width, height) stream for this model."""
@@ -179,8 +178,8 @@ class _RingDetector:
 
     def _ingest(self):
         ow, oh = self.grid
-        self.eng._run("stream_ingest", self.lib.dagr_stream_ingest, _lib.ptr(self.raw_d), self.S, self.max_chunk, self.scale,
-                      self.scale, ow, oh, self.H, _lib.ptr(self._cmap), _lib.ptr(self.stage_d), self.max_chunk, _lib.stream_ptr())
+        self.eng._run("stream_ingest", self.lib.dagr_stream_ingest, self.raw_d, self.S, self.max_chunk, self.scale, self.scale,
+                      ow, oh, self.H, self._cmap, self.stage_d, self.max_chunk, _lib.stream_ptr())
 
     def _enqueue(self):
         """one streaming step on the current stream (eager or under capture)."""
@@ -373,8 +372,8 @@ class StreamingDetector(_RingDetector):
         self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
 
     def _push(self):
-        _lib.check(self.lib.dagr_stream_push(_lib.ptr(self.ctl), _lib.ptr(self.stage_d), _lib.ptr(self.batch), _lib.ptr(self.pos),
-                                             _lib.ptr(self.feat), self.cap, self.max_chunk, 0, _lib.stream_ptr()), "stream_push")
+        _lib.check(self.lib.dagr_stream_push(self.ctl, self.stage_d, self.batch, self.pos, self.feat, self.cap, self.max_chunk, 0,
+                                             _lib.stream_ptr()), "stream_push")
 
     # ------------------------------------------------------------------------------------------------------------
     def reset(self):
