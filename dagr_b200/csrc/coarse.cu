@@ -111,6 +111,28 @@ k_grid_conv(const dagr_grid_t gr, const int32_t *__restrict__ cnt, const int32_t
     }
 }
 
+// The in-edge of voxel `cell` from window position `bit` (0..8, centre 4 excluded) of its 3x3 neighbourhood: false when
+// the cell is past the grid or empty, the mask bit is clear, or the neighbour is off the grid or empty; otherwise its
+// source cell and the four spline weights and slots of the edge.
+__device__ __forceinline__ bool grid_in_edge(const dagr_grid_t &gr, const int32_t *__restrict__ cnt, const int32_t *__restrict__ pxy,
+                                             const uint32_t *__restrict__ mask, int cell, int bit, float den_x, float den_y, int &src,
+                                             float w[4], int slot[4])
+{
+    const int cells = gr.B * gr.ny * gr.nx, per = gr.ny * gr.nx;
+    if (bit == 4 || cell >= cells || cnt[cell] <= 0 || !((mask[cell] >> bit) & 1u)) return false;
+    const int b = cell / per, rem = cell % per, cy = rem / gr.nx, cx = rem % gr.nx;
+    const int sx = cx + bit % 3 - 1, sy = cy + bit / 3 - 1;
+    if (sx < 0 || sy < 0 || sx >= gr.nx || sy >= gr.ny) return false;
+    src = b * per + sy * gr.nx + sx;
+    if (cnt[src] <= 0) return false;
+    const int dx = pxy[2 * src] - pxy[2 * cell], dy = pxy[2 * src + 1] - pxy[2 * cell + 1];
+    // attr = d / (2*M*size) + 0.5 exactly as init_lut evaluates it (spline_conv.py:28-29)
+    const float ax = __fadd_rn(__fdiv_rn((float)dx, den_x), 0.5f);
+    const float ay = __fadd_rn(__fdiv_rn((float)dy, den_y), 0.5f);
+    spline_basis2(ax, ay, 5, w, slot);
+    return true;
+}
+
 // ------------------------------------------------------------------------------------------------
 // v2: split-K SplineConv on a voxel grid.  One CTA handles CPB consecutive voxels with 8 warps:
 //   phase 1  A[k][c][j] = sum_{in-edges e of voxel j} b_k(e) * x[src_e][c]   (k < 25), A[25] = x[j] (root)
@@ -144,44 +166,25 @@ k_grid_conv_sk(const dagr_grid_t gr, const int32_t *__restrict__ cnt, const int3
     const int cells = gr.B * gr.ny * gr.nx;
     const int cell0 = blockIdx.x * CPB;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int per = gr.ny * gr.nx;
 
     if (tid == 0) s_used = 0;
     for (int i = tid; i < SK_SLOTS * Cin * CPB; i += blockDim.x) A[i] = 0.f;
     __syncthreads();
     // ---- edge tables: one thread per (voxel, neighbour bit) ---------------------------------------------
-    if (tid < CPB * 9) {
+    if (tid < CPB * 9 && tid % 9 != 4) {
         const int j = tid / 9, bit = tid % 9;
-        const int cell = cell0 + j;
-        if (bit == 4) {
-            // slot bookkeeping done by the other lanes; this lane counts the edges afterwards
-        } else if (cell < cells && cnt[cell] > 0 && ((mask[cell] >> bit) & 1u)) {
-            const int b = cell / per, rem = cell % per, cy = rem / gr.nx, cx = rem % gr.nx;
-            const int sx = cx + bit % 3 - 1, sy = cy + bit / 3 - 1;
-            if (sx >= 0 && sy >= 0 && sx < gr.nx && sy < gr.ny) {
-                const int src = b * per + sy * gr.nx + sx;
-                if (cnt[src] > 0) {
-                    const int dx = pxy[2 * src] - pxy[2 * cell], dy = pxy[2 * src + 1] - pxy[2 * cell + 1];
-                    const float ax = __fadd_rn(__fdiv_rn((float)dx, den_x), 0.5f);
-                    const float ay = __fadd_rn(__fdiv_rn((float)dy, den_y), 0.5f);
-                    float w[4]; int slot[4];
-                    spline_basis2(ax, ay, 5, w, slot);
-                    const int e = bit < 4 ? bit : bit - 1;              // dense edge index 0..7
-                    s_src[e][j] = src;
-                    unsigned int used = 0;
+        const int e = bit < 4 ? bit : bit - 1;                          // dense edge index 0..7
+        int src; float w[4]; int slot[4];
+        if (grid_in_edge(gr, cnt, pxy, mask, cell0 + j, bit, den_x, den_y, src, w, slot)) {
+            s_src[e][j] = src;
+            unsigned int used = 0;
 #pragma unroll
-                    for (int q = 0; q < 4; q++) { s_w[e][q][j] = w[q]; s_slot[e][q][j] = (unsigned char)slot[q]; if (w[q] != 0.f) used |= 1u << slot[q]; }
-                    atomicOr(&s_used, used);
-                    goto table_done;
-                }
-            }
-            { const int e = bit < 4 ? bit : bit - 1; s_src[e][j] = -1; }
+            for (int q = 0; q < 4; q++) { s_w[e][q][j] = w[q]; s_slot[e][q][j] = (unsigned char)slot[q]; if (w[q] != 0.f) used |= 1u << slot[q]; }
+            atomicOr(&s_used, used);
         } else {
-            const int e = bit < 4 ? bit : bit - 1;
-            if (bit != 4) s_src[e][j] = -1;
+            s_src[e][j] = -1;
         }
     }
-table_done:
     __syncthreads();
     // ---- phase 1: A[k][c][j] --------------------------------------------------------------------------------
     // the voxel index j runs fastest across the lanes: the read-modify-writes of A then touch CPB consecutive floats per
@@ -298,6 +301,249 @@ static int launch_grid_conv_sk(const dagr_grid_t *gr, const int32_t *cnt, const 
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// v3: the large-grid kernel.  A GEMM over 26 K-blocks, one per spline slot (root = slot 25), each Cin deep, on a tile of
+// M consecutive voxels x 64 output channels.  The weights of a slot are copied into shared memory (cp.async, double
+// buffered) and reused by all M voxels; the slot's A tile [M][Cin] is built in shared memory from the voxels' edge tables
+// just before it is consumed; each thread owns 4 voxels x 4 outputs in registers.
+//
+// Arithmetic contract: every output has the bits of k_grid_conv_sk<CPB> at any CPB, for finite inputs.
+//   1. edges: grid_in_edge, the same helper as k_grid_conv_sk.
+//   2. A[k][v][c] = fmaf chain from 0.f over the dense edges e = 0..7 in order, then q = 0..3, over the entries whose
+//      slot is k (zero weights included); A[25][v][c] = x[v][c].
+//   3. P_w (w = 0..7) = fmaf chain from 0.f over the slots k = w, w+8, w+16, w+24 (< 26, ascending) and inside each slot
+//      over c ascending.  The K-blocks are visited in that order (0, 8, 16, 24, 1, 9, ...), so a thread keeps one set of
+//      accumulators for the current class and the running sum.  Padding rows (c >= Cin) carry zeros on both sides.
+//   4. out = ((0.f + P_0) + P_1) ... + P_7, + bias, fmaf(., scale, shift), + skip, relu; cells with cnt <= 0 write 0.
+//   5. a slot block without any edge entry in the tile is skipped: its A tile is exactly zero, and neither an accumulator
+//      nor a partial sum that starts at +0 can become -0, so adding its products changes no bit.
+// Each of these sums is independent of M, so the tile size is free to follow the grid size.
+// ------------------------------------------------------------------------------------------------
+#define GT_NT 64                                                  // output channels per CTA (16 threads x 4)
+#define GT_CH 3                                                   // 32-channel chunks of an A row built by one lane: Cin <= 96
+
+__device__ __forceinline__ void cp_async16(void *dst, const void *src)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src));
+}
+__device__ __forceinline__ void cp_async4(void *dst, const void *src)
+{
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src));
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
+
+// shared memory of k_grid_conv_tiled: A [2][M][ldA], W [2][ldK][64], edge masks [25][M], weights [32][M], sources [8][M],
+// valid flags [M]
+__host__ __device__ inline int gt_ldk(int Cin) { return (Cin + 3) & ~3; }
+__host__ __device__ inline int gt_lda(int Cin) { return gt_ldk(Cin) % 8 ? gt_ldk(Cin) : gt_ldk(Cin) + 4; }
+static inline size_t gt_smem(int M, int Cin)
+{
+    return ((size_t)2 * M * gt_lda(Cin) + (size_t)2 * gt_ldk(Cin) * GT_NT + (size_t)(25 + 32 + 8 + 1) * M) * sizeof(float);
+}
+
+// blockDim.x = 4 M threads: thread (g, n) owns voxels g + i M/4 (i < 4) and outputs 4n .. 4n+3 of the CTA's 64 columns
+// (blockIdx.y); a warp covers 4 voxel groups x 8 column groups, so its A reads are 4 rows at a row stride of 4 mod 8 floats
+// and its W reads one contiguous 128-byte run: no bank conflicts.
+__global__ void __launch_bounds__(256)
+k_grid_conv_tiled(const dagr_grid_t gr, const int32_t *__restrict__ cnt, const int32_t *__restrict__ pxy,
+                  const uint32_t *__restrict__ mask, const float *__restrict__ xin, int ldin, int Cin, int Cout,
+                  const float *__restrict__ weight, const float *__restrict__ rootT, const float *__restrict__ bias,
+                  const float *__restrict__ scale, const float *__restrict__ shift, const float *__restrict__ skip,
+                  int relu, float den_x, float den_y, float *__restrict__ out)
+{
+    extern __shared__ __align__(16) float smem_f[];
+    const int M = blockDim.x / 4, G = M / 4, nwarps = blockDim.x / 32;
+    const int ldK = gt_ldk(Cin), ldA = gt_lda(Cin);
+    float *As = smem_f;
+    float *Ws = As + 2 * M * ldA;
+    uint32_t *s_mask = reinterpret_cast<uint32_t *>(Ws + 2 * ldK * GT_NT);
+    float *s_w = reinterpret_cast<float *>(s_mask + 25 * M);
+    int *s_src = reinterpret_cast<int *>(s_w + 32 * M);
+    int *s_ok = s_src + 8 * M;
+    __shared__ int s_list[SK_SLOTS];
+    __shared__ int s_n;
+    __shared__ unsigned int s_used;
+    const int cells = gr.B * gr.ny * gr.nx;
+    const int cell0 = blockIdx.x * M, o0 = blockIdx.y * GT_NT, ncols = min(GT_NT, Cout - o0);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    // zero both A and W buffers once: the padding (c >= Cin, columns >= Cout) is never written again
+    for (int i = tid; i < (2 * M * ldA + 2 * ldK * GT_NT) / 4; i += blockDim.x)
+        reinterpret_cast<float4 *>(smem_f)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = tid; i < 25 * M; i += blockDim.x) s_mask[i] = 0u;
+    for (int v = tid; v < M; v += blockDim.x) s_ok[v] = cell0 + v < cells && cnt[cell0 + v] > 0;
+    if (tid == 0) s_used = 1u << 25;
+    __syncthreads();
+    // ---- edge tables: bit e*4+q of s_mask[k][v] marks entry (e, q) of voxel v as one of slot k's -----------------------
+    for (int i = tid; i < 8 * M; i += blockDim.x) {
+        const int v = i % M, e = i / M;
+        int src; float w[4]; int slot[4];
+        if (grid_in_edge(gr, cnt, pxy, mask, cell0 + v, e < 4 ? e : e + 1, den_x, den_y, src, w, slot)) {
+            s_src[e * M + v] = src;
+            unsigned int used = 0;
+#pragma unroll
+            for (int q = 0; q < 4; q++) {
+                s_w[(4 * e + q) * M + v] = w[q];
+                atomicOr(&s_mask[slot[q] * M + v], 1u << (4 * e + q));
+                used |= 1u << slot[q];
+            }
+            atomicOr(&s_used, used);
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int n = 0;
+        for (int w = 0; w < 8; w++)
+            for (int k = w; k < SK_SLOTS; k += 8)
+                if ((s_used >> k) & 1u) s_list[n++] = k;
+        s_n = n;
+    }
+    __syncthreads();
+
+    const bool vec = Cout % 4 == 0 && ((reinterpret_cast<uintptr_t>(weight) | reinterpret_cast<uintptr_t>(rootT)) & 15) == 0;
+    // W_k[c][o0 + o] -> Wb[c][o] for c < Cin, o < ncols
+    auto stage_w = [&](int k, float *Wb) {
+        const float *wk = (k < 25 ? weight + (int64_t)k * Cin * Cout : rootT) + o0;
+        if (vec) {
+            const int q4 = ncols / 4;
+            for (int i = tid; i < Cin * q4; i += blockDim.x) {
+                const int c = i / q4, o = 4 * (i % q4);
+                cp_async16(Wb + c * GT_NT + o, wk + (int64_t)c * Cout + o);
+            }
+        } else {
+            for (int i = tid; i < Cin * ncols; i += blockDim.x) {
+                const int c = i / ncols, o = i % ncols;
+                cp_async4(Wb + c * GT_NT + o, wk + (int64_t)c * Cout + o);
+            }
+        }
+        cp_async_commit();
+    };
+    // A_k -> Ab[v][c]: one warp per voxel, lanes over channels (the source rows are read coalesced)
+    auto build_a = [&](int k, float *Ab) {
+        for (int v = warp; v < M; v += nwarps) {
+            float *arow = Ab + v * ldA;
+            if (k == 25) {
+                const float *xd = xin + (int64_t)(cell0 + v) * ldin;
+                const bool ok = s_ok[v];
+                for (int c = lane; c < Cin; c += 32) arow[c] = ok ? xd[c] : 0.f;
+                continue;
+            }
+            float a[GT_CH] = {};
+            for (uint32_t m = s_mask[k * M + v]; m; m &= m - 1) {
+                const int i = __ffs(m) - 1;
+                const float w = s_w[i * M + v];
+                const float *xs = xin + (int64_t)s_src[(i >> 2) * M + v] * ldin;
+                float xv[GT_CH];
+#pragma unroll
+                for (int h = 0; h < GT_CH; h++) xv[h] = lane + 32 * h < Cin ? xs[lane + 32 * h] : 0.f;
+#pragma unroll
+                for (int h = 0; h < GT_CH; h++) a[h] = fmaf(w, xv[h], a[h]);
+            }
+#pragma unroll
+            for (int h = 0; h < GT_CH; h++)
+                if (lane + 32 * h < Cin) arow[lane + 32 * h] = a[h];
+        }
+    };
+
+    const int n = (warp & 1) * 8 + (lane & 7), g = (warp >> 1) * 4 + (lane >> 3);
+    float acc[4][4], sum[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) acc[i][j] = sum[i][j] = 0.f;
+
+    const int nblk = s_n;
+    stage_w(s_list[0], Ws);
+    build_a(s_list[0], As);
+    for (int t = 0; t < nblk; t++) {
+        const int k = s_list[t];
+        cp_async_wait_all();
+        __syncthreads();                              // A / W of block t visible; every thread is done with block t - 1
+        if (t + 1 < nblk) {
+            stage_w(s_list[t + 1], Ws + ((t + 1) & 1) * ldK * GT_NT);
+            build_a(s_list[t + 1], As + ((t + 1) & 1) * M * ldA);
+        }
+        const float *Ab = As + (t & 1) * M * ldA + g * ldA;
+        const float *Wb = Ws + (t & 1) * ldK * GT_NT + 4 * n;
+#pragma unroll 2
+        for (int c = 0; c < ldK; c += 4) {
+            float4 a[4];
+#pragma unroll
+            for (int i = 0; i < 4; i++) a[i] = *reinterpret_cast<const float4 *>(Ab + i * G * ldA + c);
+#pragma unroll
+            for (int cc = 0; cc < 4; cc++) {
+                const float4 w = *reinterpret_cast<const float4 *>(Wb + (c + cc) * GT_NT);
+#pragma unroll
+                for (int i = 0; i < 4; i++) {
+                    const float av = cc == 0 ? a[i].x : cc == 1 ? a[i].y : cc == 2 ? a[i].z : a[i].w;
+                    acc[i][0] = fmaf(av, w.x, acc[i][0]);
+                    acc[i][1] = fmaf(av, w.y, acc[i][1]);
+                    acc[i][2] = fmaf(av, w.z, acc[i][2]);
+                    acc[i][3] = fmaf(av, w.w, acc[i][3]);
+                }
+            }
+        }
+        if (t + 1 == nblk || (s_list[t + 1] & 7) != (k & 7)) {          // end of chain class k % 8
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) { sum[i][j] = sum[i][j] + acc[i][j]; acc[i][j] = 0.f; }
+        }
+    }
+    // ---- epilogue ----------------------------------------------------------------------------------------------------
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const int v = g + i * G, cell = cell0 + v;
+        if (cell >= cells) continue;
+        const bool ok = s_ok[v];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int o = o0 + 4 * n + j;
+            if (o >= Cout) continue;
+            float r = 0.f;
+            if (ok) {
+                r = sum[i][j];
+                if (bias) r += bias[o];
+                if (scale) r = fmaf(r, scale[o], shift[o]);
+                if (skip) r += skip[(int64_t)cell * Cout + o];
+                if (relu) r = fmaxf(r, 0.f);
+            }
+            out[(int64_t)cell * Cout + o] = r;
+        }
+    }
+}
+
+// Tile size M (voxels per CTA, a multiple of 16 up to 64): the least voxels on the busiest SM when the CTAs are spread
+// over the SMs, the larger M (more reuse of each staged weight) on a tie.  17920 cells on 132 SMs: M = 48 (374 CTAs,
+// 144 voxels on the busiest SM against 192 at M = 64); 4480 cells: M = 48 (94 CTAs).
+static int grid_conv_tile(int cells, int n_sm)
+{
+    int best_m = 64;
+    int64_t best = INT64_MAX;
+    for (int m = 64; m >= 16; m -= 16) {
+        const int64_t ctas = (cells + m - 1) / m, load = (ctas + n_sm - 1) / n_sm * m;
+        if (load < best) { best = load; best_m = m; }
+    }
+    return best_m;
+}
+
+static int launch_grid_conv_tiled(const dagr_grid_t *gr, const int32_t *cnt, const int32_t *pxy, const uint32_t *mask,
+                                  const float *xin, int ldin, int Cin, int Cout, const float *weight, const float *rootT,
+                                  const float *bias, const float *scale, const float *shift, const float *skip, int relu,
+                                  float den_x, float den_y, float *out, int n_sm, cudaStream_t st)
+{
+    const int cells = gr->B * gr->ny * gr->nx;
+    if (Cin > 32 * GT_CH) return -1;
+    const int M = grid_conv_tile(cells, n_sm);
+    const size_t smem = gt_smem(M, Cin);
+    if (dagr_allow_smem(k_grid_conv_tiled, smem) != cudaSuccess) return -2;
+    const dim3 grid(dagr_div_up(cells, M), dagr_div_up(Cout, GT_NT));
+    k_grid_conv_tiled<<<grid, 4 * M, smem, st>>>(*gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip,
+                                                relu, den_x, den_y, out);
+    return 0;
+}
+
 // kernel of the last successful dagr_grid_conv call on this thread (see dagr_grid_conv_last_instance)
 static thread_local int grid_conv_last = -1;
 
@@ -322,7 +568,8 @@ extern "C" int dagr_grid_conv(const dagr_grid_t *gr, const int32_t *cnt, const i
     int rc = -1, cpb = 0;
     const size_t per_cell = ((size_t)SK_SLOTS * Cin + (Cout <= 64 ? 0 : (size_t)SK_WARPS * Cout)) * sizeof(float);
     if (cells >= n_sm * 16 * 2 && per_cell * 16 <= 110 * 1024)
-        rc = launch_grid_conv_sk<16>(gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out, st);
+        rc = launch_grid_conv_tiled(gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out,
+                                    n_sm, st);
     if (rc == 0 && cpb == 0) cpb = 16;
     if (rc != 0 && cells >= n_sm * 4 && per_cell * 4 <= 160 * 1024)
         rc = launch_grid_conv_sk<4>(gr, cnt, pxy, mask, xin, ldin, Cin, Cout, weight, rootT, bias, scale, shift, skip, relu, den_x, den_y, out, st);

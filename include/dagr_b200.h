@@ -395,8 +395,9 @@ int dagr_grid_conv(const dagr_grid_t *gr, const int32_t *cnt, const int32_t *pxy
                    int Cin, int Cout, const float *weight, const float *rootT,
                    const float *bias, const float *scale, const float *shift, const float *skip,
                    int relu, float den_x, float den_y, float *out, void *stream);
-/* which kernel the last successful dagr_grid_conv call on this thread launched: the voxels per CTA of the split-K kernel
- * (16, 4 or 1), 0 for the one-warp-per-voxel kernel, -1 before any such call (tests assert the instance a shape reaches) */
+/* which kernel the last successful dagr_grid_conv call on this thread launched: 16 for the large-grid tiled kernel, the
+ * voxels per CTA of the split-K kernel (4 or 1), 0 for the one-warp-per-voxel kernel, -1 before any such call (tests
+ * assert the instance a shape reaches) */
 int dagr_grid_conv_last_instance(void);
 
 /* y = BN(x @ W^T) on valid cells (Linear + BatchNormData of ConvBlockWithSkip, conv.py:41-52);
