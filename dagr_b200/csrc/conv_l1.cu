@@ -258,6 +258,52 @@ struct CB2Shared {
     __align__(16) float xt[THREADS / 32][64];   // per-warp exchange tile of the tensor-core phase 2
 };
 
+// pool1's per-thread state (channel sum or max m, integer x / y / t sums, latest t) reduced over the warp with one shuffle tree.
+// Lane 0 stores the mean instance's voxel state in the warp's row of S.red / S.sum / S.tm; a max instance's chunk state is
+// folded into what the row holds (max / sum).
+template <bool POOL_MEAN, int THREADS>
+__device__ __forceinline__ void cb2_pool_warp(CB2Shared<THREADS> &S, float m[16], long long sx, long long sy, long long st, int tm)
+{
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+#pragma unroll
+        for (int c = 0; c < 16; c++) {
+            const float o2 = __shfl_xor_sync(0xffffffffu, m[c], d);
+            m[c] = POOL_MEAN ? m[c] + o2 : fmaxf(m[c], o2);
+        }
+        sx += __shfl_xor_sync(0xffffffffu, sx, d);
+        sy += __shfl_xor_sync(0xffffffffu, sy, d);
+        st += __shfl_xor_sync(0xffffffffu, st, d);
+        tm = max(tm, __shfl_xor_sync(0xffffffffu, tm, d));
+    }
+    if (lane == 0) {
+        if constexpr (POOL_MEAN) {
+#pragma unroll
+            for (int c = 0; c < 16; c++) S.red[wid][c] = m[c];
+            S.sum[wid][0] = sx; S.sum[wid][1] = sy; S.sum[wid][2] = st; S.tm[wid] = tm;
+        } else {
+#pragma unroll
+            for (int c = 0; c < 16; c++) S.red[wid][c] = fmaxf(S.red[wid][c], m[c]);
+            S.sum[wid][0] += sx; S.sum[wid][1] += sy; S.sum[wid][2] += st; S.tm[wid] = max(S.tm[wid], tm);
+        }
+    }
+}
+
+// The max instances' pool1 state of one chunk of nodes, one node per lane (node p where `inrange`, its outputs o where `has_o`),
+// folded into the warp's row.  Warp-uniform.
+template <int THREADS>
+__device__ __forceinline__ void cb2_pool_chunk(CB2Shared<THREADS> &S, const uint32_t *__restrict__ xyb, const int2 *__restrict__ ti,
+                                               int p, bool inrange, bool has_o, const float *o)
+{
+    float mo[16];
+#pragma unroll
+    for (int c = 0; c < 16; c++) mo[c] = has_o ? o[c] : -INFINITY;
+    const uint32_t w0 = inrange ? xyb[p] : 0u;
+    const int t0 = inrange ? ti[p].x : 0;
+    cb2_pool_warp<false>(S, mo, w0 & 0xfff, (w0 >> 12) & 0xfff, t0, inrange ? t0 : -2147483647);
+}
+
 // The per-voxel routine is a template over the input rows: <dagr_l1b_params_t, 2, false> is conv_block2 (16 channels = 2
 // staged 8-channel chunks, skip + act + pool1 epilogue); <dagr_l1img_params_t, 3, true> is the image-fusion variant of
 // conv_block1.conv_block1 (the 16 sampled image channels = 2 chunks, added to the (polarity, x, y) part the probe kernel
@@ -346,11 +392,24 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
     // pool1 aggregation (pooling.py:74-77).  A template parameter: as a run-time flag (selects in the row epilogue and in the
     // reductions, one more live predicate) it slowed the max instance down (A/B on one GPU)
     constexpr bool pool_mean = POOL_MEAN && !MODE_A;
-    float m[16];
+    // The max instances fold each chunk's pool1 state (one node per thread) into the warp's row of S.red / S.sum / S.tm at the
+    // end of the chunk (cb2_pool_chunk), so that none of it is live through the next chunk's passes: held in registers across
+    // chunks, these 23 registers more than doubled the spill of the 96-register cap (four CTAs per SM) around phase 2 (stack
+    // frame 168 -> 80 bytes in the headline instance, kernel 4 % faster, measured).  A max over floats and sums over integers
+    // are exact in any order, so the outputs keep their bits.  The mean instance keeps its per-thread sums in registers: its
+    // float sums folded chunk by chunk would associate differently.
+    constexpr bool pool_fold = !MODE_A && !pool_mean;
+    const int lane_ = threadIdx.x & 31, wid_ = threadIdx.x >> 5;
+    float m[16];                                                         // the mean instance's per-thread state
 #pragma unroll
-    for (int c = 0; c < 16; c++) m[c] = pool_mean ? 0.f : -INFINITY;
+    for (int c = 0; c < 16; c++) m[c] = 0.f;
     long long sx = 0, sy = 0, st = 0;
     int tm = -2147483647;
+    if (pool_fold && lane_ == 0) {                                       // read by the same lane only, until the final barrier
+#pragma unroll
+        for (int c = 0; c < 16; c++) s_red[wid_][c] = -INFINITY;
+        s_sum[wid_][0] = 0; s_sum[wid_][1] = 0; s_sum[wid_][2] = 0; s_tm[wid_] = -2147483647;
+    }
     // Sparse voxels (at most one warp of nodes, e.g. the early windows of an inter-frame sequence): the per-thread chain of
     // six passes is the whole run time of the CTA and four of its five warps would idle.  Warps 0..2 then share the SAME
     // nodes and take one x-slot each (both channel halves), their partial sums are added through shared memory: a third of
@@ -362,7 +421,6 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
     // every instance (a gathered neighbourhood reads its rows from global memory and leaves s_rows free for the partials) --
     // otherwise its nodes would get other bits with defer = 0 than with defer = 1.
     const bool sparse = MODE_A && nown <= DAGR_L1_SPARSE_NODES;
-    const int lane_ = threadIdx.x & 31, wid_ = threadIdx.x >> 5;
     for (int pb0 = p0; pb0 < p1; pb0 += blockDim.x) {
         const int p = sparse ? p0 + lane_ : pb0 + threadIdx.x;
         const bool inrange = sparse ? (p < p1 && wid_ < 3) : (p < p1);
@@ -370,7 +428,8 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
         // incremental mode: only new nodes are convolved (the arrival index is only looked at then)
         const bool active = inrange && (min_idx <= 0 || ti[p].y >= min_idx);
         if (min_idx > 0 && !__syncthreads_or(active)) {                  // block-uniform: nothing new in this chunk
-            if (inrange) { const uint32_t w0 = xyb[p]; const int t0 = ti[p].x; sx += w0 & 0xfff; sy += (w0 >> 12) & 0xfff; st += t0; tm = max(tm, t0); }
+            if (pool_fold) cb2_pool_chunk(S, xyb, ti, p, inrange, false, nullptr);
+            else if (inrange) { const uint32_t w0 = xyb[p]; const int t0 = ti[p].x; sx += w0 & 0xfff; sy += (w0 >> 12) & 0xfff; st += t0; tm = max(tm, t0); }
             continue;
         }
         const int n = active ? nbr[(int64_t)(DAGR_ELL - 1) * N + p] : 0;
@@ -395,7 +454,11 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
         for (int k = 0; k < 8; k++) o2[k] = make_float2(0.f, 0.f);
 #pragma unroll
         for (int k = 0; k < (MODE_A ? 8 : 1); k++) sk2[k] = make_float2(0.f, 0.f);
-#pragma unroll 1
+        // Unrolled in the conv_block2 instances: a rolled loop hoists the node's 64-bit row offsets and swizzle words out of it, and
+        // they stay live through all six passes; unrolled, ptxas places them next to their use (headline instance: stack frame
+        // 80 -> 48 bytes at the 96-register cap, same code size: the halves were already separate template instances).  Rolled
+        // in the image-fusion instance, which spills when unrolled.
+#pragma unroll (MODE_A ? 1 : NCH)
         for (int half = 0; half < NCH; half++) {
             if (staged) {
                 __syncthreads();                                        // everyone is done with the previous half's rows
@@ -490,8 +553,8 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
             }
         }
         const bool owner = !sparse || wid_ == 0;                            // the thread that finishes this node
-        if (!MODE_A && inrange && owner) { const uint32_t w0 = xyb[p]; const int t0 = ti[p].x; sx += w0 & 0xfff; sy += (w0 >> 12) & 0xfff; st += t0; tm = max(tm, t0); }
-        if (!active || !owner) continue;
+        if (pool_mean && inrange) { const uint32_t w0 = xyb[p]; const int t0 = ti[p].x; sx += w0 & 0xfff; sy += (w0 >> 12) & 0xfff; st += t0; tm = max(tm, t0); }
+        if (!pool_fold && (!active || !owner)) continue;                   // (the max instances fold the chunk below, all lanes)
         float o[16];
 #pragma unroll
         for (int c = 0; c < 8; c++) { o[2 * c] = o2[c].x; o[2 * c + 1] = o2[c].y; }
@@ -538,60 +601,48 @@ __device__ __forceinline__ void cb2_voxel(const dagr_geom_t &g, int64_t N, const
             sd[3] = make_float4(sk[12], sk[13], sk[14], sk[15]);
             continue;
         }
-        const uint32_t wxy = xyb[p];
-        const int x = wxy & 0xfff, y = (wxy >> 12) & 0xfff;
-        float skv[16];
-        if (skip_pre != nullptr) {
-            const float4 *sp = reinterpret_cast<const float4 *>(skip_pre + (int64_t)p * 16);
-            const float4 a = sp[0], b4 = sp[1], c4 = sp[2], d4 = sp[3];
-            skv[0] = a.x; skv[1] = a.y; skv[2] = a.z; skv[3] = a.w; skv[4] = b4.x; skv[5] = b4.y; skv[6] = b4.z; skv[7] = b4.w;
-            skv[8] = c4.x; skv[9] = c4.y; skv[10] = c4.z; skv[11] = c4.w; skv[12] = d4.x; skv[13] = d4.y; skv[14] = d4.z; skv[15] = d4.w;
-        } else {
-            const float f0 = feat_s[p], f1 = __ldg(g.posx0 + x), f2 = __ldg(g.posy0 + y);
+        if (active) {
+            const uint32_t wxy = xyb[p];
+            const int x = wxy & 0xfff, y = (wxy >> 12) & 0xfff;
+            float skv[16];
+            if (skip_pre != nullptr) {
+                const float4 *sp = reinterpret_cast<const float4 *>(skip_pre + (int64_t)p * 16);
+                const float4 a = sp[0], b4 = sp[1], c4 = sp[2], d4 = sp[3];
+                skv[0] = a.x; skv[1] = a.y; skv[2] = a.z; skv[3] = a.w; skv[4] = b4.x; skv[5] = b4.y; skv[6] = b4.z; skv[7] = b4.w;
+                skv[8] = c4.x; skv[9] = c4.y; skv[10] = c4.z; skv[11] = c4.w; skv[12] = d4.x; skv[13] = d4.y; skv[14] = d4.z; skv[15] = d4.w;
+            } else {
+                const float f0 = feat_s[p], f1 = __ldg(g.posx0 + x), f2 = __ldg(g.posy0 + y);
+#pragma unroll
+                for (int c = 0; c < 16; c++) {
+                    float sk = f0 * P.skip[0][c];
+                    sk = fmaf(f1, P.skip[1][c], sk);
+                    sk = fmaf(f2, P.skip[2][c], sk);
+                    skv[c] = fmaf(sk, P.sscale[c], P.sshift[c]);
+                }
+            }
 #pragma unroll
             for (int c = 0; c < 16; c++) {
-                float sk = f0 * P.skip[0][c];
-                sk = fmaf(f1, P.skip[1][c], sk);
-                sk = fmaf(f2, P.skip[2][c], sk);
-                skv[c] = fmaf(sk, P.sscale[c], P.sshift[c]);
+                float r = fmaf(o[c], P.scale[c], P.shift[c]) + skv[c];
+                r = relu ? fmaxf(r, 0.f) : r;
+                o[c] = r;
+            }
+            if constexpr (pool_mean) {
+#pragma unroll
+                for (int c = 0; c < 16; c++) m[c] += o[c];
+            }
+            if (x1 != nullptr) {
+                float4 *dst = reinterpret_cast<float4 *>(x1 + (int64_t)p * 16);
+                dst[0] = make_float4(o[0], o[1], o[2], o[3]);
+                dst[1] = make_float4(o[4], o[5], o[6], o[7]);
+                dst[2] = make_float4(o[8], o[9], o[10], o[11]);
+                dst[3] = make_float4(o[12], o[13], o[14], o[15]);
             }
         }
-#pragma unroll
-        for (int c = 0; c < 16; c++) {
-            float r = fmaf(o[c], P.scale[c], P.shift[c]) + skv[c];
-            r = relu ? fmaxf(r, 0.f) : r;
-            o[c] = r;
-        }
-#pragma unroll
-        for (int c = 0; c < 16; c++) m[c] = pool_mean ? m[c] + o[c] : fmaxf(m[c], o[c]);
-        if (x1 != nullptr) {
-            float4 *dst = reinterpret_cast<float4 *>(x1 + (int64_t)p * 16);
-            dst[0] = make_float4(o[0], o[1], o[2], o[3]);
-            dst[1] = make_float4(o[4], o[5], o[6], o[7]);
-            dst[2] = make_float4(o[8], o[9], o[10], o[11]);
-            dst[3] = make_float4(o[12], o[13], o[14], o[15]);
-        }
+        if constexpr (pool_fold) cb2_pool_chunk(S, xyb, ti, p, inrange, active, o);
     }
     if (MODE_A) return;
     // ---- pool1: per-voxel max / mean position (pooling.py:66-86) -------------------------------------
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-#pragma unroll
-        for (int c = 0; c < 16; c++) {
-            const float o2 = __shfl_xor_sync(0xffffffffu, m[c], d);
-            m[c] = pool_mean ? m[c] + o2 : fmaxf(m[c], o2);
-        }
-        sx += __shfl_xor_sync(0xffffffffu, sx, d);
-        sy += __shfl_xor_sync(0xffffffffu, sy, d);
-        st += __shfl_xor_sync(0xffffffffu, st, d);
-        tm = max(tm, __shfl_xor_sync(0xffffffffu, tm, d));
-    }
-    if (lane == 0) {
-#pragma unroll
-        for (int c = 0; c < 16; c++) s_red[wid][c] = m[c];
-        s_sum[wid][0] = sx; s_sum[wid][1] = sy; s_sum[wid][2] = st; s_tm[wid] = tm;
-    }
+    if constexpr (pool_mean) cb2_pool_warp<true>(S, m, sx, sy, st, tm);
     __syncthreads();
     const int nw = blockDim.x >> 5;
     if (threadIdx.x < 16) {
