@@ -22,7 +22,9 @@ works on a batch.  The step is still one CUDA graph replay.
 FusionStreamingDetector streams the hybrid (image + events) model: a camera frame runs through the image trunk once, into one
 of two frame slots, and every chunk's step (one replay of that slot's graph) reads the newest frame whose trunk has finished.
 FusionMultiStreamDetector does the same for S hybrid cameras in one step: the frame slots of all cameras are planes of one
-array, and each camera's plane travels in its stage header, so one graph serves every combination of slots.
+array, and each camera's plane travels in its stage header, so one graph serves every combination of slots.  With
+since_frame=True both read each frame with the events since it, [max(frame t_us, t_end - window_us), t_end), the layout of
+the reference's interframe evaluation (_FusionDetector).
 
 With sensor=(width, height) any of the four takes the camera's raw events: dagr_stream_ingest runs the reference's 2x
 down-sampler, the crop, 2p - 1 and the time rebase in front of the push, inside the same replay (_RingDetector).  The two fusion
@@ -52,6 +54,7 @@ MAX_STREAMS = 127                     # dagr_stream_push_multi: 1 <= S <= 127
 MAX_RING_SLOTS = 1 << 24              # S * capacity < 2^24: sorted positions are packed in 24 bits
 MAX_RAW = 16384                       # dagr_stream_ingest: raw events per stream per step (DAGR_INGEST_MAX_RAW)
 MAX_CELLS = 1 << 18                   # dagr_stream_ingest: cells of a down-sampling grid (DAGR_INGEST_MAX_CELLS)
+CUT_STAGE = 8                         # ints per stream of the cut stage: the push's stage at max_chunk = 1 (pack_cut_stage)
 _I32_MIN, _I32_MAX = -(1 << 31), (1 << 31) - 1
 
 
@@ -84,7 +87,8 @@ class _RingDetector:
 
     _one_ring = False
 
-    def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device, sensor=None, p_is_01=True):
+    def _setup(self, model, streams: int, window_us: int, max_chunk: int, capacity: int, device, sensor=None, p_is_01=True,
+               cut_block=False):
         S = int(streams)
         if not 1 <= S <= MAX_STREAMS:
             raise ValueError(f"streams={streams}: 1 <= streams <= {MAX_STREAMS}")
@@ -110,15 +114,24 @@ class _RingDetector:
         self.pos = torch.zeros((n, 3), dtype=torch.int32, device=dev)
         self.feat = torch.zeros(n, dtype=torch.float32, device=dev)
         nstage = 4 * S + 4 * S * self.max_chunk
-        self.stage_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
         if self.sensor is not None:
             nstage = 4 * S + 2 * S * self.max_chunk                            # the pinned stage holds the raw chunks
-            self.raw_d = torch.zeros(nstage, dtype=torch.int32, device=dev)
             ow, oh = self.grid
             self._cmap = torch.zeros((S, oh, ow), dtype=torch.float32, device=dev)
             self._tbase = [None] * S          # per stream: raw timestamp of rebased time 0
-            self._tend = [None] * S           # per stream: raw t_end of its last step
             self._nraw = [0] * S              # per stream: raw events of the last submitted chunk
+        self._tend = [None] * S               # per stream: t_end of its last step (raw sensor mode: in raw time)
+        self._cut_off = None
+        if cut_block:                         # the cut stage of the second push rides behind the chunks, 16-byte aligned
+            self._cut_off = (nstage + 3) // 4 * 4
+            nstage = self._cut_off + CUT_STAGE * S
+        up = torch.zeros(nstage, dtype=torch.int32, device=dev)               # what the step's one H2D copy fills
+        if self.sensor is None:
+            self.stage_d = up
+        else:
+            self.raw_d = up
+            self.stage_d = torch.zeros(4 * S + 4 * S * self.max_chunk, dtype=torch.int32, device=dev)
+        self._cut_d = up[self._cut_off:] if cut_block else None
         self.stage_h = torch.zeros(nstage, dtype=torch.int32).pin_memory()
         self._stage_np = self.stage_h.numpy()
         self.stage_bytes = 4 * nstage
@@ -127,7 +140,11 @@ class _RingDetector:
         self._res_h = None
         self._done = None
         self._warm = 0
-        self.ctl = torch.zeros(RING_CTL if self._one_ring else (S + 1) * RING_CTL, dtype=torch.int32, device=dev)
+        # row 0 is the control block the step works on; with the cut stage, row 1 is a copy of it taken between the two
+        # pushes, from which window_state reads the step's appended and evicted counts
+        nctl = RING_CTL if self._one_ring else (S + 1) * RING_CTL
+        self._ctl_rows = torch.zeros((2 if cut_block else 1, nctl), dtype=torch.int32, device=dev)
+        self.ctl = self._ctl_rows[0]
 
     @property
     def graph(self):
@@ -150,9 +167,9 @@ class _RingDetector:
         """word 3 of each stream's stage header: the frame plane of its step (FusionMultiStreamDetector), None for no frames."""
         return None
 
-    def _push(self):
-        _lib.check(self.lib.dagr_stream_push_multi(self.ctl, self.stage_d, self.batch, self.pos, self.feat, self.cap, self.S,
-                                                   self.max_chunk, _lib.stream_ptr()), "stream_push_multi")
+    def _push(self, stage, max_chunk):
+        _lib.check(self.lib.dagr_stream_push_multi(self.ctl, stage, self.batch, self.pos, self.feat, self.cap, self.S,
+                                                   max_chunk, _lib.stream_ptr()), "stream_push_multi")
 
     def _check_sensor(self, sensor, p_is_01):
         """raw sensor mode: the down-sampling factor and grid of a `sensor` = (width, height) stream for this model."""
@@ -189,18 +206,23 @@ class _RingDetector:
         else:
             self.raw_d.copy_(self.stage_h, non_blocking=True)
             self._ingest()
-        self._push()
+        self._push(self.stage_d, self.max_chunk)
         eng.launches += 2
+        if self._cut_d is not None:
+            # a chunk that straddles t_cut was appended behind a window already cut: the same cut again, with no chunk
+            self._ctl_rows[1].copy_(self.ctl)
+            self._push(self._cut_d, 1)
+            eng.launches += 2
         feats, outs = self._image_inputs()
         dec = eng.forward_events(self.batch, self.pos, self.feat, self._B, self.W, self.H, image_feats=feats, image_outs=outs,
                                  ring=self.ctl, ring_streams=self._ring_streams, image_planes=self._image_planes())
         det, ndet = eng.postprocess(dec, m.conf_threshold, m.nms_threshold, self.W, self.H)
         if self._res_h is None:
             self._res_h = (torch.empty(det.shape, dtype=det.dtype).pin_memory(), torch.empty(ndet.shape, dtype=ndet.dtype).pin_memory(),
-                           torch.empty(self.ctl.shape, dtype=torch.int32).pin_memory())
+                           torch.empty(self._ctl_rows.shape, dtype=torch.int32).pin_memory())
         self._res_h[0].copy_(det, non_blocking=True)
         self._res_h[1].copy_(ndet, non_blocking=True)
-        self._res_h[2].copy_(self.ctl, non_blocking=True)
+        self._res_h[2].copy_(self._ctl_rows, non_blocking=True)
 
     def _step(self):
         """enqueue one step (the stage is filled) on the detector's stream behind the caller's stream."""
@@ -245,22 +267,34 @@ class _RingDetector:
                 if c is not None and len(c[2]) > self.max_chunk:
                     raise ValueError(f"stream {s}: chunk of {len(c[2])} events exceeds max_chunk={self.max_chunk}")
             hdr = self._stage_np[:4 * S].reshape(S, 4)
-            t_cut = []
+            t_cut, bases, ends = [], [0] * S, list(self._tend)
             for s, c in enumerate(rows):
                 te = None if t_end is None else t_end[s]
                 if te is None:
-                    te = int(c[2][-1]) if c is not None else int(hdr[s, 1]) + self.window_us
-                t_cut.append(int(te) - self.window_us)
+                    te = int(c[2][-1]) if c is not None else ends[s]
+                ends[s] = None if te is None else int(te)
+                # no end yet (no events and no t_end so far): the ring is empty, the header's cut (0) stands
+                t_cut.append(int(hdr[s, 1]) if te is None else int(te) - self.window_us)
         else:
             rows, t_cut, bases, ends = self._raw_rows(chunks, t_end)
+        t_cut = self._window_cuts(t_cut, ends, bases)
         if self._done is not None:
             self._done.synchronize()                                  # the stage / result buffers of the previous step are free
+        planes = self._stage_planes()
         if self.sensor is None:
-            pack_stage(self._stage_np, rows, t_cut, self.max_chunk, planes=self._stage_planes())
+            pack_stage(self._stage_np, rows, t_cut, self.max_chunk, planes=planes)
         else:
-            self._nraw = pack_raw_stage(self._stage_np, rows, t_cut, self.max_chunk, planes=self._stage_planes())
-            self._tbase, self._tend = bases, ends
+            self._nraw = pack_raw_stage(self._stage_np, rows, t_cut, self.max_chunk, planes=planes)
+            self._tbase = bases
+        self._tend = ends
+        if self._cut_off is not None:
+            pack_cut_stage(self._stage_np[self._cut_off:], t_cut, planes=planes)
         self._step()
+
+    def _window_cuts(self, t_cut, ends, bases):
+        """the t_cut of each stream's step (in the stage's time: rebased in raw sensor mode), from the sliding cuts t_end -
+        window_us, the steps' ends (None: no end yet) and the streams' time bases.  A refusal raises before any device work."""
+        return t_cut
 
     def result(self):
         """detections of the last step, one dict(boxes f32[n,4] xyxy px, scores f32[n], labels i64[n]) per stream (host tensors)."""
@@ -295,8 +329,13 @@ class _RingDetector:
 
     def _state(self, s: int):
         self._done.synchronize()
-        c = self._res_h[2][RING_CTL * s:RING_CTL * (s + 1)]
+        c = self._res_h[2][0, RING_CTL * s:RING_CTL * (s + 1)]
         st = dict(head=int(c[0]), live=int(c[1]), evicted=int(c[2]), appended=int(c[3]), overflow=bool(c[4]))
+        if self._cut_d is not None:
+            # the second push only drops rows of the chunk older than t_cut (the first one left no older window row): the
+            # window lost what the first push evicted and kept the chunk's rows the second push did not
+            m = self._res_h[2][1, RING_CTL * s:RING_CTL * (s + 1)]
+            st.update(evicted=int(m[2]), appended=int(m[3]) - int(c[2]))
         if self.sensor is not None:
             st["raw"] = self._nraw[s]                                 # raw events of the chunk; `appended` = the kept ones
         return st
@@ -371,8 +410,8 @@ class StreamingDetector(_RingDetector):
             raise NotImplementedError("streaming mode drives the events-only model")
         self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
 
-    def _push(self):
-        _lib.check(self.lib.dagr_stream_push(self.ctl, self.stage_d, self.batch, self.pos, self.feat, self.cap, self.max_chunk, 0,
+    def _push(self, stage, max_chunk):
+        _lib.check(self.lib.dagr_stream_push(self.ctl, stage, self.batch, self.pos, self.feat, self.cap, max_chunk, 0,
                                              _lib.stream_ptr()), "stream_push")
 
     # ------------------------------------------------------------------------------------------------------------
@@ -433,7 +472,10 @@ class _CameraFrames:
     buffers are overwritten (by the next frame or a model(data) call) only after the copy out of them.
 
     With the detector's raw_frames a frame is the camera's u8 [sensor_h, sensor_w, 3]; the pinned stage is sized for it,
-    and dagr_frame_preprocess turns it into the trunk's f32 [1, 3, H, W] where `.float() / 255.0` runs otherwise."""
+    and dagr_frame_preprocess turns it into the trunk's f32 [1, 3, H, W] where `.float() / 255.0` runs otherwise.
+
+    With the detector's since_frame, every frame carries its time t_us (non-decreasing), a step takes the pending frame only
+    once t_us <= the step's t_end, and the step's window starts at the frame it reads (plan / take)."""
 
     def __init__(self, det, s):
         self.det, self.s = det, s
@@ -445,6 +487,8 @@ class _CameraFrames:
         self.overlapped = False               # the last submitted step ran while a newer frame's trunk was in flight
         self.nframes = 0
         self.img_h = self.h2d = None
+        self.last_t = None                    # since_frame: t_us of the newest frame set
+        self.begin = self.step_begin = None   # since_frame: t_cut of the step being submitted / of the last submitted step
 
     def check(self, image):
         d = self.det
@@ -477,15 +521,29 @@ class _CameraFrames:
         self.det.stream.wait_event(pend["ready"])                     # no-op once it completed; orders the very first frame
         self.cur, self.cur_frame = pend["slot"], (pend["id"], pend["t_us"])
 
-    def sync(self):
+    def sync(self, promote=True):
+        """wait for the pending frame and make it current; promote=False (since_frame's sync_frame) leaves it to the next step
+        whose t_end reaches its t_us."""
         if self.pending is not None:
             self.pending["ready"].synchronize()
-            self.promote()
+            if promote:
+                self.promote()
+
+    def check_time(self, t_us):
+        """since_frame: a frame's t_us is required and never older than the camera's previous frame."""
+        if t_us is None:
+            raise ValueError(f"camera {self.s}: since_frame windows start at the frame's time: set_frame needs t_us")
+        t = int(t_us)
+        if self.last_t is not None and t < self.last_t:
+            raise ValueError(f"camera {self.s}: frame at t_us={t} is older than the camera's previous frame ({self.last_t})")
+        return t
 
     def set(self, image, t_us):
         from .model.image_branch import branch_of, run_frame
         det = self.det
         img = self.check(image)
+        if det.since_frame:
+            t_us = self.last_t = self.check_time(t_us)
         self.sync()
         slot = 0 if self.cur is None else 1 - self.cur
         fs = det.frame_stream
@@ -522,14 +580,48 @@ class _CameraFrames:
             self.promote()
         self.overlapped = self.pending is not None
 
+    def plan(self, t_end, t_cut, base):
+        """since_frame, before a step that ends at t_end (None: no end yet, the ring is empty): -> (take, cut).  take: the
+        step takes the pending frame, which it does when its copy has finished (a non-blocking query; the first frame
+        whatever its state) and its t_us <= t_end.  cut: where the step's window starts, in the stage's time =
+        max(t_us of the frame the step reads - base, t_cut), t_cut being the sliding cut t_end - window_us (the cap when
+        frames stop) and base the stream's time base (None in raw sensor mode before the stream's first event: t_cut
+        stands).  Changes nothing; ValueError when the step has no frame at or before t_end."""
+        p = self.pending
+        take = p is not None and (self.cur is None or p["ready"].query()) and (t_end is None or p["t_us"] <= t_end)
+        t_us = p["t_us"] if take else None if self.cur is None else self.cur_frame[1]
+        if t_us is None:
+            raise ValueError(f"camera {self.s}: a step ending at t_end={t_end} precedes the camera's first frame "
+                             f"(t_us={p['t_us']})")
+        if t_end is not None and t_us > t_end:
+            raise ValueError(f"camera {self.s}: a step ending at t_end={t_end} precedes the camera's frame in use (t_us={t_us}): "
+                             f"frames were set more than one frame ahead of the chunks")
+        if base is None:
+            return take, t_cut
+        cut = t_us - base
+        if cut > _I32_MAX:
+            raise ValueError(f"camera {self.s}: frame at t_us={t_us} leaves the int32 range of the stream's time base {base}")
+        return take, max(cut, t_cut)
+
+    def take(self, take, begin):
+        """since_frame: apply plan()'s choice; `begin` = the step's cut in the caller's time (frame_state's t_begin)."""
+        if take:
+            self.promote()
+        self.overlapped = self.pending is not None
+        self.begin = begin
+
     def stepped(self, done):
         """after a step was enqueued: it reads the current slot until `done`."""
         self.reader[self.cur] = done
         self.step_frame = self.cur_frame
+        self.step_begin = self.begin
 
     def state(self):
         fid, t_us = self.step_frame
-        return dict(frame=fid, t_us=t_us, pending=None if self.pending is None else self.pending["id"])
+        st = dict(frame=fid, t_us=t_us, pending=None if self.pending is None else self.pending["id"])
+        if self.det.since_frame:
+            st["t_begin"] = self.step_begin
+        return st
 
 
 class _FusionDetector:
@@ -537,15 +629,21 @@ class _FusionDetector:
     detector has a list of one) and the frame policy of a step.  A step is refused before any device work while some
     camera has never had a frame; before the step each camera's newest frame whose copy has finished becomes current (a
     non-blocking query; a camera's first frame is waited for on the device), and after it the step reads that frame's slot
-    until it is done."""
+    until it is done.
 
-    def _frame_setup(self, raw_frames):
+    since_frame: a step's window is [t_cut, t_end) with t_cut = max(t_us of the frame it reads, t_end - window_us), so it
+    never holds an event older than its frame; the frame a step reads is, per camera, the newest finished one with t_us <=
+    t_end (_CameraFrames.plan).  The push evicts before it appends, so a chunk that straddles t_cut would keep its older rows
+    for a step: a second push inside the same step, of the cut stage (pack_cut_stage: no events, the same cuts), evicts them."""
+
+    def _frame_setup(self, raw_frames, since_frame):
         """after _setup: the frame stream, the image branch precision (read once from the model: a later change of
         model.image_precision does not reach the detector), with raw_frames the u8 -> f32 table, the frame store of the S
         cameras' two slots each, and one _CameraFrames per camera."""
         from .model.image_branch import FrameStore
         self.frame_stream = torch.cuda.Stream(device=self.dev)
         self.image_precision = self.model.image_precision
+        self.since_frame = bool(since_frame)
         self.raw_frames = bool(raw_frames)
         self._frame_lut = ingest.frame_lut(self.dev) if self.raw_frames else None
         self._frames = FrameStore(2 * self.S)
@@ -562,11 +660,24 @@ class _FusionDetector:
         if missing:
             raise RuntimeError(f"{type(self).__name__}: set_frame() must be called for every camera before the first step "
                                f"(no frame yet: cameras {missing})")
-        for c in self._cams:
-            c.take_newest()
-        super()._submit(chunks, t_end)
+        if not self.since_frame:
+            for c in self._cams:
+                c.take_newest()
+        super()._submit(chunks, t_end)                                # since_frame: the frames are taken in _window_cuts
         for c in self._cams:
             c.stepped(self._done)
+
+    def _window_cuts(self, t_cut, ends, bases):
+        if not self.since_frame:
+            return t_cut
+        plans = [c.plan(te, cut, base) for c, te, cut, base in zip(self._cams, ends, t_cut, bases)]   # may refuse the step
+        for c, (take, cut), base in zip(self._cams, plans, bases):
+            c.take(take, None if base is None else cut + base)
+        return [cut for _, cut in plans]
+
+    def _sync_frames(self, cams):
+        for c in cams:
+            c.sync(promote=not self.since_frame)
 
     def _frame_state(self, s):
         cam = self._camera(s)
@@ -595,14 +706,23 @@ class FusionStreamingDetector(_FusionDetector, StreamingDetector):
     raw_frames=True (with sensor=(width, height)): set_frame takes the camera's own frame, u8 [height, width, 3] (HWC, the
     camera's channel order), and the reference's crop + cv2.resize(INTER_CUBIC) by the integer factor width / W
     (dsec_data.py:149-154) runs on the device, bit for bit (dagr_frame_preprocess); the detections then equal those of
-    the same detector fed the frame prepared by the reference's loader."""
+    the same detector fed the frame prepared by the reference's loader.
+
+    since_frame=True reads each frame with the events since it, the input of the reference's interframe evaluation
+    (scripts/run_test_interframe.py) and training samples: a step's window is [t_cut, t_end) with t_cut = max(t_us of the
+    frame it reads, t_end - window_us), window_us being only a cap for when frames stop.  set_frame then needs t_us
+    (non-decreasing; with sensor= in the camera's raw clock, otherwise on the chunks' time axis), a step reads the newest
+    finished frame with t_us <= its t_end (a later one waits for a later step), sync_frame() waits for the pending frame
+    without making it current, and frame_state adds t_begin = the step's t_cut.  After every step the detections equal
+    model(data) over [t_cut, t_end) with the frame frame_state reports.  The step stays one replay: a second push of a
+    header-only cut stage evicts the rows of a chunk that straddles t_cut in the same step (_FusionDetector)."""
 
     def __init__(self, model, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None, sensor=None,
-                 p_is_01: bool = True, raw_frames: bool = False):
+                 p_is_01: bool = True, raw_frames: bool = False, since_frame: bool = False):
         _check_fusion_model(model, "FusionStreamingDetector", "StreamingDetector")
         _check_raw_frames(raw_frames, sensor)
-        self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self._frame_setup(raw_frames)
+        self._setup(model, 1, window_us, max_chunk, capacity, device, sensor, p_is_01, cut_block=since_frame)
+        self._frame_setup(raw_frames, since_frame)
 
     @property
     def _cam(self):
@@ -622,13 +742,15 @@ class FusionStreamingDetector(_FusionDetector, StreamingDetector):
     def set_frame(self, image, t_us=None):
         """start a new frame: the trunk runs on the device, this returns without waiting for it.  `image` u8 [3,H,W] or
         [1,3,H,W], with raw_frames the camera's u8 [sensor_h, sensor_w, 3] (host or device; another shape or dtype raises
-        ValueError before any device work); `t_us` is the caller's timestamp of the frame, reported back by frame_state.
-        Returns the frame id (0, 1, 2, ...).  A frame still pending is waited for and becomes current first."""
+        ValueError before any device work); `t_us` is the caller's timestamp of the frame, reported back by frame_state
+        (since_frame: required and non-decreasing, else ValueError before any device work).  Returns the frame id (0, 1, 2,
+        ...).  A frame still pending is waited for and becomes current first."""
         return self._cam.set(image, t_us)
 
     def sync_frame(self):
-        """block until the pending frame (if any) is usable; the next step uses it."""
-        self._cam.sync()
+        """block until the pending frame (if any) is usable; the next step uses it (since_frame: the next step whose t_end
+        reaches the frame's t_us)."""
+        self._sync_frames(self._cams)
 
     def _graph_key(self):
         return self._cam.cur
@@ -639,7 +761,7 @@ class FusionStreamingDetector(_FusionDetector, StreamingDetector):
     @property
     def frame_state(self):
         """dict(frame=id of the frame the last finished step used, t_us=its timestamp, pending=id of a frame not yet in use
-        or None)."""
+        or None); since_frame adds t_begin, the step's t_cut (None in raw sensor mode before the first event)."""
         return self._frame_state(0)
 
 
@@ -696,6 +818,21 @@ def pack_raw_stage(stage: np.ndarray, chunks, t_cut, max_raw: int, planes=None):
             e[:, 1] = np.asarray(t).astype(np.int32)
         o += n
     return ns
+
+
+def pack_cut_stage(stage: np.ndarray, t_cut, planes=None):
+    """write the cut stage of the second push of a since_frame step into the int32 array `stage` (>= CUT_STAGE * S = 8*S
+    entries): the stage of dagr_stream_push[_multi] at max_chunk = 1 with no events, header [S][4] = {0, t_cut, 0, plane}
+    and 4*S zero event words.  Pushed after the chunks, it evicts the rows of a chunk older than its stream's t_cut."""
+    S = len(t_cut)
+    if len(stage) < CUT_STAGE * S:
+        raise ValueError(f"stage of {len(stage)} ints is smaller than {CUT_STAGE}*S = {CUT_STAGE * S}")
+    blk = stage[:CUT_STAGE * S]
+    blk[:] = 0
+    hdr = blk[:4 * S].reshape(S, 4)
+    hdr[:, 1] = [int(c) for c in t_cut]
+    if planes is not None:
+        hdr[:, 3] = [int(p) for p in planes]
 
 
 class MultiStreamDetector(_RingDetector):
@@ -766,14 +903,15 @@ class FusionMultiStreamDetector(_FusionDetector, MultiStreamDetector):
     a camera's first step waits on the device for its first frame; submit raises RuntimeError before any device work while
     some camera has never had a frame.  reset() keeps the frames.  With sensor=(width, height) the event chunks are the
     cameras' raw events (see MultiStreamDetector); frames stay at the model's resolution unless raw_frames=True, which
-    takes every camera's own u8 [height, width, 3] frames (see FusionStreamingDetector)."""
+    takes every camera's own u8 [height, width, 3] frames (see FusionStreamingDetector).  since_frame=True starts each
+    camera's window at the frame it reads, per camera, as FusionStreamingDetector(since_frame=True) does."""
 
     def __init__(self, model, streams: int, window_us: int = 50_000, max_chunk: int = 8192, capacity: int = 1 << 17, device=None,
-                 sensor=None, p_is_01: bool = True, raw_frames: bool = False):
+                 sensor=None, p_is_01: bool = True, raw_frames: bool = False, since_frame: bool = False):
         _check_fusion_model(model, "FusionMultiStreamDetector", "MultiStreamDetector")
         _check_raw_frames(raw_frames, sensor)
-        self._setup(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01)
-        self._frame_setup(raw_frames)
+        self._setup(model, streams, window_us, max_chunk, capacity, device, sensor, p_is_01, cut_block=since_frame)
+        self._frame_setup(raw_frames, since_frame)
 
     @property
     def _overlapped(self):
@@ -787,9 +925,9 @@ class FusionMultiStreamDetector(_FusionDetector, MultiStreamDetector):
         return self._camera(s).set(image, t_us)
 
     def sync_frame(self, s=None):
-        """block until the pending frame of camera s (of every camera when None) is usable; the next step uses it."""
-        for c in (self._cams if s is None else [self._camera(s)]):
-            c.sync()
+        """block until the pending frame of camera s (of every camera when None) is usable; the next step uses it
+        (since_frame: the next step whose t_end reaches the frame's t_us)."""
+        self._sync_frames(self._cams if s is None else [self._camera(s)])
 
     def _image_inputs(self):
         return self._frames.feats, self._frames.outs
@@ -802,7 +940,7 @@ class FusionMultiStreamDetector(_FusionDetector, MultiStreamDetector):
 
     def frame_state(self, s: int):
         """camera s after the last finished step: dict(frame=id of the frame the step used, t_us=its timestamp, pending=id of a
-        frame of camera s not yet in use or None)."""
+        frame of camera s not yet in use or None; since_frame: t_begin, the step's t_cut)."""
         return self._frame_state(s)
 
 
