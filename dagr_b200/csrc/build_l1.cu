@@ -448,9 +448,13 @@ __device__ __forceinline__ void bl_voxel(const dagr_geom_t &g, int64_t N, const 
     __syncthreads();
     if (T.maxidx < 0) return;                                           // block-uniform: no new event in this voxel
     // ---- per-pixel time-bucket ranges ---------------------------------------------------------------
-    // bucket(t) = clamp(t/delta_t - (smin-1), 0, NB-1); an event in bucket e needs records of buckets {e-1, e}.
+    // bucket(t) = clamp(t/delta_t - (smin-1), 0, NB-1); an event in bucket e needs records of buckets {e-1, e}.  That holds
+    // only where no record older in arrival is later in time: the sort's flag proves it for every sample at once, so without
+    // the flag (NULL: order unknown) nothing is pruned.  A clear flag also implies that every pixel's records are time-sorted,
+    // so the per-pixel check below cannot fire for a flag the sort computed on these events; it stays because the code without
+    // it is allocated worse by ptxas (the fp32 lean instance spills, the regular tensor-core instance loads more spilled bytes).
     const int sbase = T.smin - 1;
-    bool bucketed = staged && (T.smax - sbase) < BL_NB && (flags == nullptr || flags[0] == 0);   // block-uniform
+    bool bucketed = staged && (T.smax - sbase) < BL_NB && flags != nullptr && flags[0] == 0;   // block-uniform
     // the ranges of tile pixel i -> s_rng[i]; returns bit e set when bucket e's range is non-empty
     auto pixel_ranges = [&](int i) -> uint32_t {
         const uint32_t pb = s_pbin[i];

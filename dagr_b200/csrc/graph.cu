@@ -172,15 +172,18 @@ __global__ void k_keys_hist(dagr_geom_t g, const int32_t *__restrict__ batch, co
     const RingAt at = ring_at(ctl, S, mask, (int)i);
     const int64_t si = at.slot;
     int x = pos[3 * si], y = pos[3 * si + 1], b = batch[si];
-    // contract check (SURVEY 8b): events are time-sorted within each sample.  If not, flags[0] = 1 and the
-    // build kernel disables its time-bucket pruning (results stay exact, only slower).  In ring mode the predecessor
-    // of a stream's first live event belongs to another sample and is not compared.
-    if (flags != nullptr && at.i > 0) {
-        const int64_t sp = ctl != nullptr ? (si & ~(int64_t)mask) | ((si - 1) & mask) : si - 1;
-        if (batch[sp] == b && pos[3 * sp + 2] > pos[3 * si + 2]) flags[0] = 1;
-    }
     // out-of-range events are clamped into the grid (the reference would index out of bounds)
     x = min(max(x, 0), g.W - 1); y = min(max(y, 0), g.H - 1); b = min(max(b, 0), g.B - 1);
+    // time-order proof for the build kernel's time-bucket pruning (SURVEY 8b): flags[0] = 1 unless the (clamped) samples
+    // come as ascending contiguous runs, each time-sorted in arrival order.  Comparing every event with its predecessor
+    // proves exactly that; interleaved samples count as unproven.  Without the proof the build does not prune (results
+    // stay exact, only slower).  In ring mode the compact order is stream-major with ascending samples by construction,
+    // and the predecessor of a stream's first live event is not compared.
+    if (flags != nullptr && at.i > 0) {
+        const int64_t sp = ctl != nullptr ? (si & ~(int64_t)mask) | ((si - 1) & mask) : si - 1;
+        const int pb = min(max(batch[sp], 0), g.B - 1);
+        if (pb > b || (pb == b && pos[3 * sp + 2] > pos[3 * si + 2])) flags[0] = 1;
+    }
     int k = b * (g.ny1 * g.nx1 * g.CP) + __ldg(g.ykey + y) + __ldg(g.xkey + x);
     key[i] = k;
     atomicAdd(count + k, 1);

@@ -144,7 +144,9 @@ int64_t dagr_scan_blocks(int64_t n);
 int dagr_graph_sort(const dagr_geom_t *g, const int32_t *batch, const int32_t *pos, const float *feat,
                     int64_t N, int32_t *key, int32_t *tmp, int32_t *count, int32_t *blocksums,
                     int32_t *start, int32_t *perm, int32_t *ti, uint32_t *xyb, float *feat_s,
-                    int32_t *flags /* i32[1], zero on entry; [0]=1 if a sample is not time-sorted; may be NULL */,
+                    int32_t *flags /* i32[1], zero on entry, or NULL; [0] = 1 unless the time order is proven: the (clamped) samples
+                                       come as ascending contiguous runs in arrival order, each time-sorted.  Interleaved
+                                       samples set it too */,
                     void *stream);
 
 /* Streaming form of dagr_graph_sort (BASELINE config 5; the sliding window the reference sketches with min_index,
@@ -155,7 +157,8 @@ int dagr_graph_sort(const dagr_geom_t *g, const int32_t *batch, const int32_t *p
  * a whole streaming step can be captured once and replayed as a CUDA graph.  Downstream kernels take N = capacity as the
  * leading dimension of the ELL / activation arrays.
  *   dagr_stream_push : stage i32[4 + 4*max_chunk] on the device = {n_new, t_cut, 0, 0, (x, y, t, polarity +-1) * n_new}:
- *                      evicts the prefix with t < t_cut (binary search, no data movement) and appends the chunk. */
+ *                      evicts the prefix with t < t_cut (binary search, no data movement) and appends the chunk.
+ * flags: as dagr_graph_sort, over the window in arrival order (one sample, so: [0] = 1 where the window is not time-sorted). */
 int dagr_graph_sort_ring(const dagr_geom_t *g, const int32_t *batch, const int32_t *pos, const float *feat,
                          int64_t capacity, const int32_t *ctl, int32_t *key, int32_t *tmp, int32_t *count,
                          int32_t *blocksums, int32_t *start, int32_t *perm, int32_t *ti, uint32_t *xyb, float *feat_s,
@@ -176,7 +179,9 @@ int dagr_stream_push(int32_t *ctl, const int32_t *stage, int32_t *batch, int32_t
  *         window offsets (exclusive scan of the live counts) and the total.  Two launches, grids independent of the counts.
  *   dagr_graph_sort_rings  : dagr_graph_sort over the S live windows read in the compact order c < total: stream s's i-th
  *         live event has arrival index c = offset_s + i.  Outputs as dagr_graph_sort with B = S; downstream kernels take
- *         N = S*capacity.  dagr_graph_sort_ring is this sort with S = 1 and a single i32[8] block.
+ *         N = S*capacity.  dagr_graph_sort_ring is this sort with S = 1 and a single i32[8] block.  flags as dagr_graph_sort:
+ *         the compact order is stream-major with stream s = sample s, so [0] = 1 exactly where some window is not
+ *         time-sorted (a stream's first live event is not compared with the previous stream's last).
  * Limits (DAGR_E_ARG before anything is launched): no null pointer (flags may be NULL), 1 <= S <= 127, capacity a power of
  * two, S*capacity < 2^24 (sorted positions are packed in 24 bits), 1 <= max_chunk <= capacity, and for the sort S == g->B. */
 int dagr_stream_push_multi(int32_t *ctl, const int32_t *stage, int32_t *batch, int32_t *pos, float *feat, int64_t capacity,
@@ -196,7 +201,9 @@ int dagr_graph_sort_rings(const dagr_geom_t *g, const int32_t *batch, const int3
 struct dagr_l1a_params_s;
 int dagr_l1_build(const dagr_geom_t *g, int64_t N, const int32_t *start, const int32_t *ti,
                   const uint32_t *xyb, const float *feat_s,
-                  const struct dagr_l1a_params_s *p_host, const int32_t *flags /* from dagr_graph_sort, or NULL */,
+                  const struct dagr_l1a_params_s *p_host,
+                  const int32_t *flags /* from the sort (any form), or NULL.  The time-bucket pruning runs only where flags[0] == 0
+                                          proves the time order; NULL means the order is unknown (exact, slower) */,
                   int min_idx /* incremental mode: only events with arrival idx >= min_idx are processed and cellmask is
                                  OR-ed into its previous content; 0 = everything */,
                   int32_t *nbr, uint16_t *off, uint32_t *cellmask, float *xa,

@@ -6,7 +6,8 @@ the models below:
     x inside the voxel, arrival index) of the clamped (x, y, sample).  The voxel of a pixel comes from geom.levels[0].cellx /
     celly and vx0 / vy0, not from the key tables the kernels read; the keys only size the start table, and the model asserts
     that they are non-decreasing along its order.  Returns start, perm, ti = (t, arrival index), xyb, feat_s and the
-    not-time-sorted flag (a later event of the same raw sample with a smaller t than its predecessor in arrival order);
+    time-order flag: set unless the clamped samples come as ascending contiguous runs in arrival order, each time-sorted
+    (an event whose predecessor in arrival order has a larger clamped sample, or the same one and a larger t);
   * ref_export: the reference's edge_index from a column-major ELL (slot q of sorted position p at [q][p], slot 15 = degree):
     per destination in arrival order the self loop, then slots 0..deg-1 as ti[src].y.  A row is written only when its end
     is <= cap;
@@ -60,7 +61,7 @@ def ref_sort(geom, batch, pos, feat):
     start[1:] = np.cumsum(np.bincount(key, minlength=geom.NK))
     assert np.all(start[ks] <= arrival) and np.all(arrival < start[ks + 1]), "start does not bound a key's run"
     t = pos[:, 2]
-    flag = bool(N > 1 and np.any((batch[1:] == batch[:-1]) & (t[:-1] > t[1:])))
+    flag = bool(N > 1 and np.any((b[:-1] > b[1:]) | ((b[:-1] == b[1:]) & (t[:-1] > t[1:]))))
     return dict(start=start, perm=order.astype(np.int32), ti=np.stack([t[order], order], 1).astype(np.int32),
                 xyb=(x | y << 12 | b << 24)[order].astype(np.uint32), feat_s=feat[order], flag=flag)
 
@@ -285,15 +286,19 @@ def test_ref_sort_on_a_hand_sorted_stream():
     assert r["start"][-1] == 6 and r["start"][geom.NK // 2] == 5
     assert r["flag"]                                   # event 5 (t = 35) arrives after event 4 (t = 40) of its sample
     ev[5, 2] = 40
-    assert not ref_sort(geom, batch, ev, np.zeros(6, np.float32))["flag"]
+    assert ref_sort(geom, batch, ev, np.zeros(6, np.float32))["flag"]            # sample 1 still arrives before sample 0
+    assert not ref_sort(geom, batch[1:], ev[1:], np.zeros(5, np.float32))["flag"]
 
 
 def test_ref_sort_flag_rules_and_clamping():
     geom = _geom(240, 180, 3)
     pos = np.array([[1, 1, 10], [2, 2, 10], [3, 3, 5], [-1, 180, 7], [240, -5, 8], [10 ** 6, 10 ** 6, 9]])
-    # equal times and a drop across a sample boundary leave the flag clear; the batch values compared are the raw ones
+    # equal times and a drop into the next sample leave the flag clear; the samples compared are the clamped ones (3 and
+    # 2^20 are sample 2 at B = 3, so the times 7, 8, 9 must ascend)
     assert not ref_sort(geom, [0, 0, 1, 2, 3, 1 << 20], pos, np.zeros(6))["flag"]
     assert ref_sort(geom, [0, 0, 0, 2, 3, 1 << 20], pos, np.zeros(6))["flag"]
+    pos[4, 2] = 6
+    assert ref_sort(geom, [0, 0, 1, 2, 3, 1 << 20], pos, np.zeros(6))["flag"]      # 7 -> 6 inside the clamped sample 2
     x, y, b = clamp_xyb(geom, [-1, 3, 1 << 20, 0, 0, 0], pos)
     assert x.tolist() == [1, 2, 3, 0, 239, 239] and y.tolist() == [1, 2, 3, 179, 0, 179] and b.tolist() == [0, 2, 2, 0, 0, 0]
 

@@ -170,7 +170,7 @@ def test_plain_sort_equals_the_model(name):
 
 
 @pytest.mark.parametrize("case,flag", [("inversion-inside-a-sample", 1), ("equal-times", 0), ("drop-across-samples", 0),
-                                       ("drop-across-interleaved-samples", 0)])
+                                       ("drop-across-interleaved-samples", 1)])
 def test_plain_sort_time_order_flag(case, flag):
     geom = _geom(240, 180, 2)
     batch, pos, feat = make_events(240, 180, [0, 1], 3000, 11, interleave="interleaved" in case)

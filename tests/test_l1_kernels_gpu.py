@@ -57,10 +57,12 @@ def _fill(arr, t):
 # one synthetic stream, sorted on the device, with its oracle graph
 # ------------------------------------------------------------------------------------------------------------------------
 class Stream:
-    def __init__(self, W, H, B, seed, n_bg, radius=0.01, K=16, clusters=(), border=0, empty=(), region=None, events=None, feat=None):
+    def __init__(self, W, H, B, seed, n_bg, radius=0.01, K=16, clusters=(), border=0, empty=(), region=None, events=None, feat=None,
+                 time_window=1_000_000, max_queue_size=128, expect_flag=0):
         from dagr_b200.geometry import Geometry
         L, lib = _lib()
-        self.geom = geom = Geometry(W, H, B, radius=radius, max_neighbors=K, device="cuda")
+        self.geom = geom = Geometry(W, H, B, radius=radius, time_window=time_window, max_neighbors=K, max_queue_size=max_queue_size,
+                                    device="cuda")
         if events is None:
             box = []
             for (b, cx, cy, n) in clusters:                     # a cluster fills one pool1 voxel
@@ -86,19 +88,21 @@ class Stream:
         L.check(lib.dagr_graph_sort(C.byref(geom.c_geom), *map(P, inp), N, *map(P, work), P(self.start),
                                     P(self.perm_d), P(self.ti), P(self.xyb), P(self.feat_s), P(flags), st()), "sort")
         torch.cuda.synchronize()
-        assert int(flags[0]) == 0
+        assert int(flags[0]) == expect_flag
+        self.flags = flags
         self.perm = self.perm_d[:N].long().cpu()
         self.pos_of = torch.empty(N, dtype=torch.long)
         self.pos_of[self.perm] = torch.arange(N)
         self.nown, self.total = voxel_stats(geom, self.start[:geom.NK + 1].cpu().numpy())
         self.classes = voxel_classes(self.nown, self.total, CAPS)
-        self.edges = oracle_edges(geom, batch, pos)
+        bc = batch.clamp(0, B - 1)                              # the sample ids the kernels use (the oracle has no others)
+        self.edges = oracle_edges(geom, bc, pos)
         self.deg = degrees(self.edges, N)
         self.cells = geom.cells1
         x, y = pos[:, 0].long(), pos[:, 1].long()
         self.px, self.py = geom.posx0[x], geom.posy0[y]
         lv = geom.levels[0]
-        self.cell_of = (batch.long() * geom.ny1 + lv.celly[y].long()) * geom.nx1 + lv.cellx[x].long()   # arrival order
+        self.cell_of = (bc.long() * geom.ny1 + lv.celly[y].long()) * geom.nx1 + lv.cellx[x].long()   # arrival order
 
     def ev3(self):
         """(polarity, x / W, y / H) per node, arrival order, float64"""
@@ -209,7 +213,7 @@ def l1a(p, relu=1):
     return pa, torch.from_numpy(np.frombuffer(frag, np.float32).copy()).cuda()
 
 
-def run_build(s, pa, wfrag, defer, tc=True, min_idx=0, xa0=None, cellmask0=None):
+def run_build(s, pa, wfrag, defer, tc=True, min_idx=0, xa0=None, cellmask0=None, flags=None):
     L, lib = _lib()
     N = s.N
     nbr = torch.zeros(16 * N, dtype=torch.int32, device="cuda")
@@ -219,7 +223,7 @@ def run_build(s, pa, wfrag, defer, tc=True, min_idx=0, xa0=None, cellmask0=None)
     wl_hdr = torch.zeros(2, dtype=torch.int32, device="cuda")
     wl_ids = torch.zeros(s.cells, dtype=torch.int32, device="cuda")
     head = (C.byref(s.geom.c_geom), N, P(s.start), P(s.ti), P(s.xyb), P(s.feat_s))
-    tail = (None, min_idx, P(nbr), P(off), P(cellmask), P(xa), P(wl_hdr), P(wl_ids), defer, st())
+    tail = (P(flags), min_idx, P(nbr), P(off), P(cellmask), P(xa), P(wl_hdr), P(wl_ids), defer, st())
     if tc:
         L.check(lib.dagr_l1_build_tc(*head, C.byref(pa), P(wfrag), *tail), "l1_build_tc")
     else:
